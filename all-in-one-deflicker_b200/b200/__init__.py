@@ -1,2 +1,2 @@
-"""B200-native stage-1 neural-atlas path: ctypes binding (`_native`), fused trainer (`atlas`),
+"""H100-native stage-1 neural-atlas path: ctypes binding (`_native`), fused trainer (`atlas`),
 synthetic inputs (`synth`)."""

@@ -10,14 +10,14 @@ from . import _native as N
 ACT = {"none": 0, "relu": 1, "leaky": 2, "sigmoid": 3, "tanh": 4}
 
 # Convolution arithmetic: "fp32" = CUDA-core FFMA (bit-comparable with an fp32 cuDNN/CPU convolution up to
-# summation order), "tc" = tcgen05 with fp16 operands and fp32 accumulation — the operand precision the
+# summation order), "tc" = wgmma with fp16 operands and fp32 accumulation — the operand precision the
 # reference itself uses for these layers (fp16 autocast in RAFT, TF32 cuDNN in stage 2).
 _conv_precision = "fp32"
 _weight_images = {}        # id(weight tensor) -> (weakref to it, {(version, layout): packed fp16 images})
 
 
 def set_conv_precision(mode):
-    """'fp32', 'tc' (TMA-fed tcgen05; gather variant for strides it does not take) or 'tc_gather'.
+    """'fp32', 'tc' (TMA-fed wgmma; gather variant for strides it does not take) or 'tc_gather'.
     Returns the previous mode."""
     global _conv_precision
     if mode not in ("fp32", "tc", "tc_gather"):
@@ -66,7 +66,7 @@ _chain_buffers = {}        # (device, n, cin, h, w, kh, kw, ph, pw, tag) -> zero
 class Chain:
     """The packed fp16 NHWC input of ONE consumer convolution (stride 1, zero or reflection padding, Cin * KW > 64), filled directly
     by the epilogues of the convolutions that produce it (`conv2d(..., chain_out=chain)`), then consumed by
-    `conv2d(chain, w, ...)`: no fp32 tensor in between and no repack kernel.  tcgen05 path only.  Buffers are cached per
+    `conv2d(chain, w, ...)`: no fp32 tensor in between and no repack kernel.  wgmma path only.  Buffers are cached per
     geometry and zeroed once: producers overwrite the whole interior every time, halo and channel padding stay zero."""
 
     def __init__(self, n, cin, h, w, kernel, pad, device, tag="", pad_mode="zeros"):
@@ -155,7 +155,7 @@ def conv2d(x, w, b=None, stride=1, pad=(0, 0), pad_mode="zeros", act="none", ups
 
 def _conv2d_chained(x, w, b, stride, pad, pad_mode, act, upsample, out, out_c_off, in_slice, residual, res_c_off, out_scale,
                     upsample_mode, chain_out, chain_c_off, keep_fp32):
-    """b200_conv2d_tma_chain: packed input and / or packed output (tcgen05 path, see `Chain`)."""
+    """b200_conv2d_tma_chain: packed input and / or packed output (wgmma path, see `Chain`)."""
     _check(w); _check(b); _check(residual)
     packed_in = isinstance(x, Chain)
     bilinear = 1 if upsample_mode == "bilinear" else 0
@@ -251,7 +251,7 @@ def convex_upsample(flow, mask):
 
 def corr_build(fmap1, fmap2, impl="tc", out=None):
     """fmaps (1, C, H8, W8) -> flat pyramid tensor (level 0 [HW][H8][W8] then 3 pooled levels).
-    impl 'tc': tcgen05 with (hi, lo) fp16 operand pairs (fp32-grade, like the reference's fp32 matmul);
+    impl 'tc': wgmma with (hi, lo) fp16 operand pairs (fp32-grade, like the reference's fp32 matmul);
     'simt': fp32 CUDA-core GEMM."""
     _check(fmap1); _check(fmap2)
     b, c, h, w = fmap1.shape

@@ -703,7 +703,7 @@ int launch_dp_adam(const B200DpComm& comm, float* m, float* v, int64_t n_params,
                    double b1, double b2, double eps, int64_t* step, unsigned long long* epoch, cudaStream_t st) {
   const int64_t total4 = (n_total + 3) / 4, per = (total4 + comm.world - 1) / comm.world;
   int blocks = (int)((per + 255) / 256);
-  if (blocks > 148) blocks = 148;                 // all blocks must be co-resident (they wait on remote flags)
+  if (blocks > 132) blocks = 132;                 // all blocks must be co-resident (they wait on remote flags)
   if (blocks < 1) blocks = 1;
   timer_begin(TAG_ADAM, st);
   dp_adam_kernel<<<blocks, 256, 0, st>>>(comm, m, v, n_params, n_total, lr, b1, b2, eps, step, epoch);

@@ -1,4 +1,4 @@
-"""Builds libb200deflicker.so (sm_100a) and libb200_hostcheck.so in-tree with nvcc / g++.
+"""Builds libb200deflicker.so (sm_90a) and libb200_hostcheck.so in-tree with nvcc / g++.
 
     python all-in-one-deflicker_b200/csrc/build.py [--force]
 
@@ -14,7 +14,7 @@ PKG = os.path.dirname(HERE)
 LIB = os.path.join(PKG, "b200", "libb200deflicker.so")
 HOSTLIB = os.path.join(PKG, "b200", "libb200_hostcheck.so")
 CU = ["c_api.cu", "mlp_simt.cu", "atlas_kernels.cu", "mlp_tc.cu", "loss_heads.cu", "seg.cu", "eval_maps.cu", "producer.cu", "conv_simt.cu", "conv_tc.cu", "conv_tma.cu", "raft_kernels.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 
 
@@ -54,7 +54,7 @@ def build(force=False, verbose=False):
         if p.returncode != 0:
             sys.stderr.write(out)
             raise RuntimeError(f"nvcc failed on {cu}")
-    subprocess.check_call([nvcc, "-shared", "-o", LIB] + objs)
+    subprocess.check_call([nvcc, "-shared", NVCC_FLAGS[0], NVCC_FLAGS[1], "-o", LIB] + objs)
     subprocess.check_call(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", HOSTLIB,
                            os.path.join(HERE, "hostcheck.cpp")])
     with open(os.path.join(HERE, "build", "ptxas.log"), "w") as f:

@@ -103,7 +103,7 @@ struct AtlasPlan {
   float* d_pe = nullptr;       // [3*cap][enc]
   MlpScratch map, atlas;
   MlpShape ms, as;
-  TcPlan tc;                   // tcgen05 operand buffers (precision == B200_PREC_TC)
+  TcPlan tc;                   // tensor-core operand buffers (precision == B200_PREC_TC)
   int64_t bytes = 0;
 };
 
@@ -163,7 +163,7 @@ int b200_device_supports_tc(void) {
   int dev = 0, major = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return 0;
   if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return 0;
-  return major == 10 ? 1 : 0;
+  return major == 9 ? 1 : 0;
 }
 
 int64_t b200_mlp_layout(const B200MlpDesc* d, int64_t* w_off, int64_t* b_off) {
@@ -235,7 +235,7 @@ static int tc_call_prepare(const B200MlpDesc* d, int64_t rows, void* ws, int64_t
   *arch = tc_architecture(*s);
   B200_REQUIRE(*arch != 0, "B200_PREC_TC serves the stage-1 architectures (mapping: 3-256x{2,4}-2 without encoding; alpha: 3-PE5-256x6-1; "
                "atlas: 2-PE10-256x6-3 with skips 4, 7); use B200_PREC_FP32 for other shapes");
-  if (!b200_device_supports_tc()) { set_error("B200_PREC_TC needs a compute-capability 10.x device"); return B200_ERR_UNSUPPORTED; }
+  if (!b200_device_supports_tc()) { set_error("B200_PREC_TC needs a compute-capability 9.x device"); return B200_ERR_UNSUPPORTED; }
   B200_REQUIRE(rows > 0 && rows < (1ll << 26), "rows out of range: %lld", (long long)rows);
   B200_REQUIRE(ws != nullptr, "null workspace");
   *rows_pad = round_up(rows, kTileRows);
@@ -388,7 +388,7 @@ static int atlas_prepare(const B200AtlasConfig* cfg, void* ws, int64_t ws_bytes,
     return B200_ERR_WORKSPACE;
   }
   if (cfg->precision == B200_PREC_TC && !b200_device_supports_tc()) {
-    set_error("B200_PREC_TC needs a compute-capability 10.x device");
+    set_error("B200_PREC_TC needs a compute-capability 9.x device");
     return B200_ERR_UNSUPPORTED;
   }
   B200_REQUIRE(cfg->precision == B200_PREC_FP32 || cfg->precision == B200_PREC_TC, "unknown precision %d",
@@ -572,7 +572,7 @@ int b200_render(const float* params, int32_t H, int32_t W, int32_t T, int32_t fr
   }
   B200_REQUIRE(precision == B200_PREC_FP32 || precision == B200_PREC_TC, "unknown precision %d", precision);
   if (precision == B200_PREC_TC && !b200_device_supports_tc()) {
-    set_error("B200_PREC_TC needs a compute-capability 10.x device");
+    set_error("B200_PREC_TC needs a compute-capability 9.x device");
     return B200_ERR_UNSUPPORTED;
   }
   MlpShape m, a;
@@ -586,7 +586,7 @@ int b200_render(const float* params, int32_t H, int32_t W, int32_t T, int32_t fr
   const float t_norm = (float)((double)frame / ((double)T / 2.0) - 1.0);   // evaluate.py:657
   B200_PROPAGATE(launch_render_rows(W, half_of(larger), t_norm, pix_begin, count, rows, x_map, st));
   if (precision == B200_PREC_TC) {
-    // the two fused tcgen05 forward kernels without their activation-image stores
+    // the two fused tensor-core forward kernels without their activation-image stores
     float* uv = reinterpret_cast<float*>(carve(p, rows * 8));
     float* y = reinterpret_cast<float*>(carve(p, rows * 12));
     B200_PROPAGATE(tc_infer_forward(m, a, params, x_map, uv, y, rows, p, st));

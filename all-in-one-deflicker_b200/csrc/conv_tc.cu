@@ -1,4 +1,4 @@
-// tcgen05 implicit-GEMM convolution (fp16 operands, fp32 accumulation in TMEM).
+// wgmma implicit-GEMM convolution (fp16 operands, fp32 accumulation in registers).
 //
 // Same operator as conv_simt.cu (B200ConvDesc: NCHW fp32 tensors, channel slices, zero / reflection padding,
 // stride, nearest x2 upsampling, bias, activation, scale, residual) for the layers whose precision in the
@@ -6,16 +6,15 @@
 // (src/models/stage_1/core/raft.py:131, raft_wrapper.py:19) and the stage-2 networks run cuDNN convolutions
 // with TF32 allowed (torch default) — both 10-bit-mantissa operand formats, like fp16.
 //
-// GEMM view: M = 128 output pixels per tile, N = output channels (tile of 64/128/256), K = Cin*KH*KW in chunks
+// GEMM view: M = 128 output pixels per tile, N = output channels (tile of 64/128), K = Cin*KH*KW in chunks
 // of 64.  Persistent CTAs; warp roles:
-//   warp 0      weight producer: cp.async.bulk of pre-built K-major SW128 weight images (b200_conv_weight_images)
-//   warp 1      single-thread tcgen05.mma issuer (SS mode), two TMEM accumulators so the epilogue of tile i
-//               overlaps the MMAs of tile i+1
-//   warps 2-9   im2col gather, two groups of 4 warps taking alternate k chunks: each thread owns one pixel row
+//   warps 0-7   two consumer warpgroups (64 tile rows each): wgmma (SS mode) into register accumulators, then the
+//               epilogue: bias + activation + scale + residual, NCHW stores
+//   warp 8      weight producer: cp.async.bulk of pre-built K-major SW128 weight images (b200_conv_weight_images)
+//   warps 9-16  im2col gather, two groups of 4 warps taking alternate k chunks: each thread owns one pixel row
 //               of the A tile, loads 64 taps (coalesced across the warp: consecutive pixels) through a per-CTA
 //               tap table {input offset, tap id} and a per-pixel 64-bit tap-validity mask (zero padding costs
 //               no branches), converts to fp16 and writes its 128-byte swizzled row
-//   warps 10-13 epilogue: tcgen05.ld, bias + activation + scale + residual, coalesced NCHW stores
 #include "common.cuh"
 #include "tc_ptx.cuh"
 
@@ -26,8 +25,10 @@ constexpr int CT_M = 128;
 constexpr int CT_KC = 64;                       // k chunk
 constexpr int CT_A_STAGES = 4, CT_B_STAGES = 3;
 constexpr int CT_A_BYTES = CT_M * 128;          // 16 KB
-constexpr int CT_B_BYTES = 256 * 128;           // 32 KB (N tile <= 256 rows)
-constexpr int CT_THREADS = 448;                 // 14 warps: producer, MMA, 8 gather, 4 epilogue
+constexpr int CT_B_BYTES = 128 * 128;           // 16 KB (N tile <= 128 rows)
+constexpr int CT_CONSUMER_WARPS = 8;            // two warpgroups: wgmma + epilogue, 64 tile rows each
+constexpr int CT_PRODUCER_WARP = 8;
+constexpr int CT_THREADS = 544;                 // 17 warps: 8 consumer, producer, 8 gather
 constexpr int CT_MAX_K = 6144;                  // padded reduction length the tap table can hold
 constexpr int CT_FIXED_SMEM = CT_A_STAGES * CT_A_BYTES + CT_B_STAGES * CT_B_BYTES + 512;
 
@@ -35,7 +36,7 @@ struct ConvTcArgs {
   B200ConvDesc d;
   const float* x; const char* w_img; const float* bias; const float* res; float* y;
   int OH, OW, R, n_chunks;      // output size, reduction length, ceil(R / 64)
-  int n_tile, n_tiles_n;        // N tile (64/128/256) and number of cout tiles
+  int n_tile, n_tiles_n;        // N tile (64/128) and number of cout tiles
   int64_t pixels; int m_tiles;
 };
 
@@ -58,6 +59,62 @@ __device__ __forceinline__ int ct_atom_off(int m, int k) {
   return (m >> 3) * 1024 + r * 128 + (((k >> 3) ^ r) << 4) + ((k & 7) << 1);
 }
 
+// MMAs + epilogue of the consumer warpgroups for one N-tile width
+template <int NT>
+__device__ __forceinline__ void ct_consume(const ConvTcArgs& a, char* sA, char* sB, uint64_t* a_full, uint64_t* a_empty,
+                                           uint64_t* b_full, uint64_t* b_empty) {
+  const B200ConvDesc& d = a.d;
+  const int warp = warp_uniform(), lane = threadIdx.x & 31, g = warp >> 2, q = lane & 3;
+  const int m0 = 64 * g + 16 * (warp & 3) + (lane >> 2);
+  const int total_tiles = a.m_tiles * a.n_tiles_n;
+  const int64_t oplane = (int64_t)a.OH * a.OW;
+  float acc[NT / 2];
+  uint32_t it = 0;
+  for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+    int pend_a = -1, pend_b = -1;
+    for (int c = 0; c < a.n_chunks; ++c, ++it) {
+      const int sa = it % CT_A_STAGES, sb = it % CT_B_STAGES;
+      mbar_wait(&a_full[sa], (it / CT_A_STAGES) & 1);
+      mbar_wait(&b_full[sb], (it / CT_B_STAGES) & 1);
+      const uint32_t pa = smem_u32(sA + sa * CT_A_BYTES) + g * 8192, pb = smem_u32(sB + sb * CT_B_BYTES);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+        const uint64_t da = make_desc(pa + ks * 32, 16, 1024), db = make_desc(pb + ks * 32, 16, 1024);
+        if constexpr (NT == 128) wgmma_n128<0, 0>(acc, da, db, (c | ks) ? 1u : 0u);
+        else wgmma_n64<0, 0>(acc, da, db, (c | ks) ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (pend_a >= 0 && lane == 0) { mbar_arrive(&a_empty[pend_a]); mbar_arrive(&b_empty[pend_b]); }
+      pend_a = sa; pend_b = sb;
+    }
+    wgmma_wait<0>();
+    acc_fence(acc);
+    if (pend_a >= 0 && lane == 0) { mbar_arrive(&a_empty[pend_a]); mbar_arrive(&b_empty[pend_b]); }
+    const int mt = t / a.n_tiles_n, nt = t % a.n_tiles_n;
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      const int64_t p = (int64_t)mt * CT_M + m0 + 8 * rr;
+      if (p >= a.pixels) continue;
+      const int64_t n = p / oplane, sp = p % oplane;
+#pragma unroll
+      for (int i = 0; i < NT / 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int j = nt * NT + 8 * i + 2 * q + e;
+          if (j < d.Cout) {
+            float val = acc[4 * i + 2 * rr + e];
+            if (a.bias) val += __ldg(a.bias + j);
+            val = ct_act(val, d.act) * d.out_scale;
+            if (a.res) val += __ldg(a.res + (n * d.res_c_total + d.res_c_off + j) * oplane + sp);
+            a.y[(n * d.out_c_total + d.out_c_off + j) * oplane + sp] = val;
+          }
+        }
+    }
+  }
+}
+
 __global__ void __launch_bounds__(CT_THREADS, 1) conv2d_tc_kernel(const __grid_constant__ ConvTcArgs a) {
   extern __shared__ __align__(1024) char smem[];
   char* sA = smem;
@@ -65,22 +122,17 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv2d_tc_kernel(const __grid_c
   uint64_t* bars = reinterpret_cast<uint64_t*>(sB + CT_B_STAGES * CT_B_BYTES);
   int2* ktab = reinterpret_cast<int2*>(sB + CT_B_STAGES * CT_B_BYTES + 512);     // [n_chunks * 64] {offset, tap}
   uint64_t* a_full = bars;                         // [4] 128 gather arrivals
-  uint64_t* a_empty = a_full + CT_A_STAGES;        // [4] commit
+  uint64_t* a_empty = a_full + CT_A_STAGES;        // [4] one arrival per consumer warp
   uint64_t* b_full = a_empty + CT_A_STAGES;        // [3] tx
-  uint64_t* b_empty = b_full + CT_B_STAGES;        // [3] commit
-  uint64_t* d_full = b_empty + CT_B_STAGES;        // [2] commit
-  uint64_t* d_empty = d_full + 2;                  // [2] 128 epilogue arrivals
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(d_empty + 2);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  uint64_t* b_empty = b_full + CT_B_STAGES;        // [3] one arrival per consumer warp
+  const int warp = warp_uniform(), lane = threadIdx.x & 31;
   const B200ConvDesc& d = a.d;
   if (threadIdx.x == 0) {
-    if (smem_u32(smem) & 1023u) { printf("b200: conv smem not 1024-byte aligned\n"); __trap(); }
-    for (int i = 0; i < CT_A_STAGES; ++i) { mbar_init(&a_full[i], 128); mbar_init(&a_empty[i], 1); }
-    for (int i = 0; i < CT_B_STAGES; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&d_full[i], 1); mbar_init(&d_empty[i], 128); }
+    if (smem_u32(smem) & 1023u) __trap();   // the swizzled operand layouts need 1024-byte alignment
+    for (int i = 0; i < CT_A_STAGES; ++i) { mbar_init(&a_full[i], 128); mbar_init(&a_empty[i], CT_CONSUMER_WARPS); }
+    for (int i = 0; i < CT_B_STAGES; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], CT_CONSUMER_WARPS); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
   {
     const int KHW = d.KH * d.KW, plane = d.H * d.W;
     for (int k = threadIdx.x; k < a.n_chunks * CT_KC; k += CT_THREADS) {
@@ -88,14 +140,14 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv2d_tc_kernel(const __grid_c
       ktab[k] = k < a.R ? make_int2(ci * plane + (kk / d.KW) * d.W + (kk % d.KW), kk) : make_int2(0, 63);
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   const int total_tiles = a.m_tiles * a.n_tiles_n;
   const int b_bytes = a.n_tile * 128;
 
-  if (warp == 0) {
+  if (warp < CT_CONSUMER_WARPS) {
+    if (a.n_tile == 128) ct_consume<128>(a, sA, sB, a_full, a_empty, b_full, b_empty);
+    else ct_consume<64>(a, sA, sB, a_full, a_empty, b_full, b_empty);
+  } else if (warp == CT_PRODUCER_WARP) {
     if (lane == 0) {
       uint32_t it = 0;
       for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
@@ -109,34 +161,11 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv2d_tc_kernel(const __grid_c
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc(128, a.n_tile, 0, 0);
-      uint32_t it = 0, tile_i = 0;
-      for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++tile_i) {
-        const int acc = tile_i & 1;
-        mbar_wait(&d_empty[acc], ((tile_i >> 1) & 1) ^ 1);          // epilogue drained this accumulator
-        tc_fence_after();
-        for (int c = 0; c < a.n_chunks; ++c, ++it) {
-          const int sa = it % CT_A_STAGES, sb = it % CT_B_STAGES;
-          mbar_wait(&a_full[sa], (it / CT_A_STAGES) & 1);
-          mbar_wait(&b_full[sb], (it / CT_B_STAGES) & 1);
-          tc_fence_after();
-          const uint32_t pa = smem_u32(sA + sa * CT_A_BYTES), pb = smem_u32(sB + sb * CT_B_BYTES);
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks)
-            mma_ss(tmem + acc * 256, make_desc(pa + ks * 32, 16, 1024), make_desc(pb + ks * 32, 16, 1024), idesc,
-                   (c | ks) ? 1u : 0u);
-          mma_commit(&a_empty[sa]);
-          mma_commit(&b_empty[sb]);
-        }
-        mma_commit(&d_full[acc]);
-      }
-    }
-  } else if (warp < 10) {
+  } else {
     // ------------------------------------------------------------------ im2col gather
-    const int grp = (warp - 2) >> 2;                       // chunk parity this group fills
-    const int m = ((warp - 2) & 3) * 32 + lane;            // row of the A tile
+    const int gw = warp - CT_PRODUCER_WARP - 1;             // 0..7
+    const int grp = gw >> 2;                               // chunk parity this group fills
+    const int m = (gw & 3) * 32 + lane;                    // row of the A tile
     const int HU = d.H * d.upsample, WU = d.W * d.upsample;
     const int KHW = d.KH * d.KW;
     const int plane = d.H * d.W;
@@ -221,45 +250,7 @@ __global__ void __launch_bounds__(CT_THREADS, 1) conv2d_tc_kernel(const __grid_c
         mbar_arrive(&a_full[s]);
       }
     }
-  } else {
-    // ------------------------------------------------------------------ epilogue
-    const int q = warp & 3;                                // warps 10..13 -> TMEM quadrants 2,3,0,1
-    const int m = q * 32 + lane;
-    const uint32_t tlane = tmem + ((uint32_t)(q * 32) << 16);
-    const int64_t oplane = (int64_t)a.OH * a.OW;
-    uint32_t tile_i = 0;
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++tile_i) {
-      const int acc = tile_i & 1;
-      const int mt = t / a.n_tiles_n, nt = t % a.n_tiles_n;
-      const int64_t p = (int64_t)mt * CT_M + m;
-      const bool live = p < a.pixels;
-      const int64_t n = live ? p / oplane : 0, sp = live ? p % oplane : 0;
-      mbar_wait(&d_full[acc], (tile_i >> 1) & 1);
-      tc_fence_after();
-      for (int c = 0; c < a.n_tile / 32; ++c) {
-        uint32_t raw[32];
-        tmem_ld32(tlane + acc * 256 + c * 32, raw);
-        tmem_ld_wait();
-        if (!live) continue;
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const int j = nt * a.n_tile + c * 32 + i;
-          if (j < d.Cout) {
-            float val = __uint_as_float(raw[i]);
-            if (a.bias) val += __ldg(a.bias + j);
-            val = ct_act(val, d.act) * d.out_scale;
-            if (a.res) val += __ldg(a.res + (n * d.res_c_total + d.res_c_off + j) * oplane + sp);
-            a.y[(n * d.out_c_total + d.out_c_off + j) * oplane + sp] = val;
-          }
-        }
-      }
-      tc_fence_before();
-      mbar_arrive(&d_empty[acc]);
-    }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem, 512);
 }
 
 // weights [Cout][R] fp32 -> images [n_tile_idx][chunk][n_tile rows x 64 k] fp16, K-major SW128, zero padded
@@ -282,7 +273,7 @@ __global__ void conv_weight_images_kernel(const float* __restrict__ w, char* __r
   *reinterpret_cast<uint4*>(dst) = pk;
 }
 
-static int pick_n_tile(int cout) { return cout > 128 ? 256 : (cout > 64 ? 128 : 64); }
+static int pick_n_tile(int cout) { return cout > 64 ? 128 : 64; }
 
 }  // namespace b200
 
@@ -317,7 +308,7 @@ int b200_conv2d_tc(const B200ConvDesc* d, const float* x, const void* w_images, 
                "invalid convolution descriptor");
   B200_REQUIRE(d->in_c_off >= 0 && d->in_c_off + d->Cin <= d->in_c_total && d->out_c_off >= 0 &&
                d->out_c_off + d->Cout <= d->out_c_total, "channel slice out of range");
-  if (!b200_device_supports_tc()) { set_error("b200_conv2d_tc needs a compute-capability 10.x device"); return B200_ERR_UNSUPPORTED; }
+  if (!b200_device_supports_tc()) { set_error("b200_conv2d_tc needs a compute-capability 9.x device"); return B200_ERR_UNSUPPORTED; }
   static bool attr_done = false;
   if (!attr_done) {
     B200_CHECK_CUDA(cudaFuncSetAttribute(conv2d_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -339,7 +330,7 @@ int b200_conv2d_tc(const B200ConvDesc* d, const float* x, const void* w_images, 
   a.n_tiles_n = (d->Cout + a.n_tile - 1) / a.n_tile;
   a.pixels = (int64_t)d->N * a.OH * a.OW;
   a.m_tiles = (int)((a.pixels + CT_M - 1) / CT_M);
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int64_t tiles = (int64_t)a.m_tiles * a.n_tiles_n;

@@ -1,9 +1,9 @@
-// TMA-fed tcgen05 convolution (fp16 operands, fp32 accumulation in TMEM) — no im2col gather at all.
+// TMA-fed wgmma convolution (fp16 operands, fp32 accumulation in registers) — no im2col gather at all.
 //
 // With a channels-last fp16 copy of the input, the A operand of the implicit GEMM for ONE filter tap (ky,kx)
 // and one block of 64 input channels is a plain 2-D box of the tensor: 128 consecutive output pixels of one
 // image row x 64 channels.  A tiled TMA load with the 128-byte swizzle lands it in shared memory in exactly the
-// canonical K-major layout tcgen05.mma reads; the tap only shifts the box coordinates (the pixel dimension is
+// canonical K-major layout wgmma reads; the tap only shifts the box coordinates (the pixel dimension is
 // not the innermost one, so any shift is legal for the TMA unit).  The reduction runs over (tap, channel block).
 //
 // Two kernels per convolution:
@@ -11,9 +11,9 @@
 //                           memory transpose, with the padding (zeros / reflection), the nearest x2 upsampling
 //                           and — for stride 2 — a split into the 4 pixel phases materialised, so that the
 //                           convolution proper is a stride-1 "valid" one (HBM-bound)
-//   conv2d_tma_kernel       persistent, warp 0 = TMA producer (1 activation box + 1 weight image per stage),
-//                           warp 1 = tcgen05.mma issuer (two TMEM accumulators), warps 2-9 = epilogue
-//                           (bias, activation, scale, residual, coalesced NCHW fp32 stores)
+//   conv2d_tma_kernel       persistent, warps 0-7 = two consumer warpgroups (wgmma on 64 pixels each, then the
+//                           epilogue: bias, activation, scale, residual, NCHW fp32 / packed fp16 stores),
+//                           warp 8 = TMA producer (1 activation box + 1 weight image per stage)
 //
 // Same operator semantics as b200_conv2d (reference: nn.Conv2d / ReflectionPad2d / nn.Upsample call sites in
 // src/models/stage_1/core/update.py, src/models/network_filter.py, src/models/network_local.py).
@@ -25,16 +25,17 @@
 namespace b200 {
 using namespace ptx;
 
-constexpr int TM_THREADS = 320;
-constexpr int TM_MAX_A = 8, TM_MAX_B = 16, TM_MAX_ACC = 8;
-constexpr int TM_BAR_BYTES = 1024;              // mbarriers + TMEM slot
-constexpr int TM_SMEM_BUDGET = 225 * 1024;
+constexpr int TM_THREADS = 384;                 // 2 consumer warpgroups + the producer warpgroup (one active lane)
+constexpr int TM_CONSUMER_WARPS = 8;
+constexpr int TM_MAX_A = 8, TM_MAX_B = 16;
+constexpr int TM_BAR_BYTES = 1024;              // mbarriers
+constexpr int TM_SMEM_BUDGET = 225 * 1024;             // of the 227 KB a block may use
 
 struct ConvTmaArgs {
   B200ConvDesc d;
   const char* w_img; const float* bias; const float* res; float* y;
   int OH, OW, x_tiles, cchunks, n_chunks, n_tile, n_tiles_n, phases, shift, total_tiles;
-  int a_rows, a_stage, n_a, n_b, n_acc, acc_stride;   // box rows, bytes per A stage, ring depths, TMEM ring
+  int a_rows, a_stage, n_a, n_b;                       // box rows, bytes per A stage, ring depths
   int b_group, b_stage;                                // weight chunks (x taps) per B stage, bytes per B stage
   int split;                                           // 1: both operands are (hi, lo) fp16 pairs, 3 MMAs per product
   int resident;                                        // 1: the whole weight image stays in shared memory (narrow layers)
@@ -65,47 +66,121 @@ __device__ __forceinline__ float tm_act(float v) {
   return v;
 }
 
-// 32 accumulator columns of one pixel -> bias, activation, scale, residual; NCHW fp32 stores (one channel plane apart,
-// yq may be null) and / or 32 consecutive fp16 channels of the pixel's vector in the next layer's packed input (ypk)
-template <int ACT>
-__device__ __forceinline__ void tm_store32(const uint32_t (&raw)[32], const float* __restrict__ bias, float scale,
-                                           const float* __restrict__ resp, float* __restrict__ yq, int64_t oplane,
-                                           int ncols, bool live, int lane, __half* __restrict__ ypk) {
-  const float bl = (bias && lane < ncols) ? __ldg(bias + lane) : 0.f;      // lane i holds bias[i] (ncols is warp-uniform)
-  const int nvalid = live ? ncols : 0;
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    float radd[16];
-    if (resp) {                                            // residual loads in flight before the first store
-      const float* rp = resp + (int64_t)(h * 16) * oplane;
-#pragma unroll
-      for (int i = 0; i < 16; ++i, rp += oplane) radd[i] = (h * 16 + i) < nvalid ? __ldg(rp) : 0.f;
-    }
-    float* p = yq ? yq + (int64_t)(h * 16) * oplane : nullptr;
-    float v16[16];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      float val = __uint_as_float(raw[h * 16 + i]) + __shfl_sync(0xffffffffu, bl, h * 16 + i);
-      val = tm_act<ACT>(val) * scale;
-      if (resp) val += radd[i];
-      v16[i] = val;
-      if (p && h * 16 + i < nvalid) p[(int64_t)i * oplane] = val;
-    }
-    if (ypk) {                                             // channels are consecutive in NHWC: two 16-byte stores
-#pragma unroll
-      for (int g8 = 0; g8 < 2; ++g8) {
-        if (h * 16 + g8 * 8 < nvalid) {                    // ncols is a multiple of 8 on this path
-          uint4 w;
-          w.x = pack_half2(v16[g8 * 8 + 0], v16[g8 * 8 + 1]); w.y = pack_half2(v16[g8 * 8 + 2], v16[g8 * 8 + 3]);
-          w.z = pack_half2(v16[g8 * 8 + 4], v16[g8 * 8 + 5]); w.w = pack_half2(v16[g8 * 8 + 6], v16[g8 * 8 + 7]);
-          *reinterpret_cast<uint4*>(ypk + h * 16 + g8 * 8) = w;
+// Consumer warpgroups for one N-tile width: the MMAs of a tile (this warpgroup's 64 pixels), then the epilogue on the
+// accumulator registers (bias, activation, scale, residual; NCHW fp32 stores and / or the fp16 channel pairs of the
+// next layer's packed input)
+template <int NT, int ACT>
+__device__ __forceinline__ void tma_consume(const ConvTmaArgs& a, char* sA, char* sB, uint64_t* a_full, uint64_t* a_empty,
+                                            uint64_t* b_full, uint64_t* b_empty) {
+  const B200ConvDesc& d = a.d;
+  const int warp = warp_uniform(), lane = threadIdx.x & 31, g = warp >> 2, q = lane & 3;
+  const int m0 = 64 * g + 16 * (warp & 3) + (lane >> 2);
+  const int b_half = a.n_tile * 128;
+  const int b_bytes = a.split ? 2 * b_half : b_half;
+  const int a_half = a.a_stage >> 1;
+  const int s = d.stride;
+  const int64_t oplane = (int64_t)a.OH * a.OW;
+  int sa = 0, sb = 0;
+  uint32_t pha = 0, phb = 0;
+  if (a.resident) mbar_wait(&b_full[0], 0);
+  float acc[NT / 2];
+  for (int t = blockIdx.x; t < a.total_tiles; t += gridDim.x) {
+    uint32_t accum = 0;
+    int jres = 0;                                          // resident mode: index of the next weight chunk
+    for (int ky = 0; ky < d.KH; ++ky)
+      for (int xpar = 0; xpar < s && xpar < d.KW; ++xpar) {
+        const int nsub = (d.KW - xpar + s - 1) / s;
+        for (int cc = 0; cc < a.cchunks; ++cc) {
+          mbar_wait(&a_full[sa], pha);
+          const uint32_t pa = smem_u32(sA + sa * a.a_stage) + g * 8192;
+          const int left = d.Cin - cc * 64;
+          const int ksteps = ((left < 64 ? left : 64) + 15) >> 4;
+          for (int i0 = 0; i0 < nsub; i0 += (a.resident ? nsub : a.b_group)) {
+            const int gn = a.resident ? nsub : (nsub - i0 < a.b_group ? nsub - i0 : a.b_group);
+            uint32_t pb;
+            if (a.resident) {
+              pb = smem_u32(sB) + jres * b_bytes;
+              jres += nsub;
+            } else {
+              mbar_wait(&b_full[sb], phb);
+              pb = smem_u32(sB + sb * a.b_stage);
+            }
+            wgmma_fence();
+            for (int i = 0; i < gn; ++i) {
+              const uint32_t ai = pa + (i0 + i) * 128, bi = pb + i * b_bytes;
+              for (int ks = 0; ks < ksteps; ++ks, accum = 1u) {
+                const uint64_t da = make_desc(ai + ks * 32, 16, 1024), db = make_desc(bi + ks * 32, 16, 1024);
+                if constexpr (NT == 256) wgmma_n256<0, 0>(acc, da, db, accum);
+                else if constexpr (NT == 128) wgmma_n128<0, 0>(acc, da, db, accum);
+                else wgmma_n64<0, 0>(acc, da, db, accum);
+                if (a.split) {                             // (hi + lo)(hi + lo) without the lo*lo term
+                  const uint64_t da_lo = make_desc(ai + a_half + ks * 32, 16, 1024);
+                  const uint64_t db_lo = make_desc(bi + b_half + ks * 32, 16, 1024);
+                  if constexpr (NT == 256) { wgmma_n256<0, 0>(acc, da, db_lo, 1u); wgmma_n256<0, 0>(acc, da_lo, db, 1u); }
+                  else if constexpr (NT == 128) { wgmma_n128<0, 0>(acc, da, db_lo, 1u); wgmma_n128<0, 0>(acc, da_lo, db, 1u); }
+                  else { wgmma_n64<0, 0>(acc, da, db_lo, 1u); wgmma_n64<0, 0>(acc, da_lo, db, 1u); }
+                }
+              }
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            if (!a.resident) {
+              if (lane == 0) mbar_arrive(&b_empty[sb]);
+              if (++sb == a.n_b) { sb = 0; phb ^= 1; }
+            }
+          }
+          if (lane == 0) mbar_arrive(&a_empty[sa]);
+          if (++sa == a.n_a) { sa = 0; pha ^= 1; }
         }
+      }
+    acc_fence(acc);
+    const int nt = t % a.n_tiles_n;
+    int r = t / a.n_tiles_n;
+    const int xb = r % a.x_tiles; r /= a.x_tiles;
+    const int oy = r % a.OH, n = r / a.OH;
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      const int x = xb * 128 + m0 + 8 * rr;
+      if (x >= a.OW) continue;
+      const int64_t sp = (int64_t)oy * a.OW + x;
+      const float* resp = a.res ? a.res + ((int64_t)n * d.res_c_total + d.res_c_off) * oplane + sp : nullptr;
+      float* yp = a.y ? a.y + ((int64_t)n * d.out_c_total + d.out_c_off) * oplane + sp : nullptr;
+      __half* ypix = a.yp ? a.yp + ((((int64_t)n * a.yp_hp2 + oy + a.yp_pad_h) * a.yp_wp2 + x + a.yp_pad_w) * a.yp_cp +
+                                    a.yp_c_off) : nullptr;
+#pragma unroll
+      for (int i = 0; i < NT / 8; ++i) {
+        const int j = nt * a.n_tile + 8 * i + 2 * q;
+        float v[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float val = acc[4 * i + 2 * rr + e];
+          if (j + e < d.Cout) {
+            if (a.bias) val += __ldg(a.bias + j + e);
+            val = tm_act<ACT>(val) * d.out_scale;
+            if (resp) val += __ldg(resp + (int64_t)(j + e) * oplane);
+            if (yp) yp[(int64_t)(j + e) * oplane] = val;
+          }
+          v[e] = val;
+        }
+        if (ypix && j < d.Cout) *reinterpret_cast<uint32_t*>(ypix + j) = pack_half2(v[0], v[1]);   // Cout % 8 == 0 here
       }
     }
   }
 }
 
-// Reduction order shared by the producer, the MMA issuer and the weight images:
+template <int NT>
+__device__ __forceinline__ void tma_consume_act(const ConvTmaArgs& a, char* sA, char* sB, uint64_t* a_full,
+                                                uint64_t* a_empty, uint64_t* b_full, uint64_t* b_empty) {
+  switch (a.d.act) {
+    case 1: tma_consume<NT, 1>(a, sA, sB, a_full, a_empty, b_full, b_empty); break;
+    case 2: tma_consume<NT, 2>(a, sA, sB, a_full, a_empty, b_full, b_empty); break;
+    case 3: tma_consume<NT, 3>(a, sA, sB, a_full, a_empty, b_full, b_empty); break;
+    case 4: tma_consume<NT, 4>(a, sA, sB, a_full, a_empty, b_full, b_empty); break;
+    default: tma_consume<NT, 0>(a, sA, sB, a_full, a_empty, b_full, b_empty); break;
+  }
+}
+
+// Reduction order shared by the producer, the consumers and the weight images:
 //   for ky, for xpar in [0, stride), for cc (64-channel block):   one activation box (all x shifts of that row)
 //     for kx = xpar, xpar + stride, ... < KW:                      one weight chunk, A start shifted by kx>>shift rows
 __global__ void __launch_bounds__(TM_THREADS, 1) conv2d_tma_kernel(const __grid_constant__ ConvTmaArgs a,
@@ -114,197 +189,70 @@ __global__ void __launch_bounds__(TM_THREADS, 1) conv2d_tma_kernel(const __grid_
   extern __shared__ __align__(1024) char smem[];
   const int b_half = a.n_tile * 128;                    // one term of one weight chunk
   const int b_bytes = a.split ? 2 * b_half : b_half;
-  const int a_half = a.a_stage >> 1;                    // split: hi box at +0, lo box at +a_half
   char* sA = smem;
   char* sB = smem + a.n_a * a.a_stage;
   uint64_t* bars = reinterpret_cast<uint64_t*>(sB + a.n_b * a.b_stage);
   uint64_t* a_full = bars;                         // tx
-  uint64_t* a_empty = a_full + TM_MAX_A;           // commit
+  uint64_t* a_empty = a_full + TM_MAX_A;           // one arrival per consumer warp
   uint64_t* b_full = a_empty + TM_MAX_A;           // tx
-  uint64_t* b_empty = b_full + TM_MAX_B;           // commit
-  uint64_t* d_full = b_empty + TM_MAX_B;           // commit
-  uint64_t* d_empty = d_full + TM_MAX_ACC;         // 128 epilogue arrivals
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(d_empty + TM_MAX_ACC);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  uint64_t* b_empty = b_full + TM_MAX_B;           // one arrival per consumer warp
+  const int warp = warp_uniform(), lane = threadIdx.x & 31;
   const B200ConvDesc& d = a.d;
   if (threadIdx.x == 0) {
-    if (smem_u32(smem) & 1023u) { printf("b200: conv smem not 1024-byte aligned\n"); __trap(); }
-    for (int i = 0; i < TM_MAX_A; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 1); }
-    for (int i = 0; i < TM_MAX_B; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 1); }
-    for (int i = 0; i < TM_MAX_ACC; ++i) { mbar_init(&d_full[i], 1); mbar_init(&d_empty[i], 128); }
+    if (smem_u32(smem) & 1023u) __trap();   // the swizzled operand layouts need 1024-byte alignment
+    for (int i = 0; i < TM_MAX_A; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], TM_CONSUMER_WARPS); }
+    for (int i = 0; i < TM_MAX_B; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], TM_CONSUMER_WARPS); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   const int s = d.stride;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      int sa = 0, sb = 0;
-      uint32_t pha = 0, phb = 0;
-      if (a.resident) {                                    // one cout tile, all chunks: loaded once per CTA
-        mbar_expect_tx(&b_full[0], a.n_chunks * b_bytes);
-        for (int j = 0; j < a.n_chunks; ++j) bulk_g2s(sB + j * b_bytes, a.w_img + (int64_t)j * b_bytes, b_bytes, &b_full[0]);
-      }
-      for (int t = blockIdx.x; t < a.total_tiles; t += gridDim.x) {
-        const int nt = t % a.n_tiles_n;
-        int r = t / a.n_tiles_n;
-        const int xb = r % a.x_tiles; r /= a.x_tiles;
-        const int oy = r % a.OH, n = r / a.OH;
-        const char* wsrc = a.w_img + (int64_t)nt * a.n_chunks * b_bytes;
-        for (int ky = 0; ky < d.KH; ++ky)
-          for (int xpar = 0; xpar < s && xpar < d.KW; ++xpar) {
-            const int nsub = (d.KW - xpar + s - 1) / s;
-            const int ph = a.phases == 4 ? ((ky & 1) * 2 + xpar) : 0;
-            for (int cc = 0; cc < a.cchunks; ++cc) {
-              mbar_wait(&a_empty[sa], pha ^ 1);
-              mbar_expect_tx(&a_full[sa], a.a_rows * 128 * (1 + a.split));
-              tma_load_4d(sA + sa * a.a_stage, &xmap, cc * 64, xb * 128, oy + (ky >> a.shift), n * a.phases + ph, &a_full[sa]);
-              if (a.split)
-                tma_load_4d(sA + sa * a.a_stage + a_half, &xmap_lo, cc * 64, xb * 128, oy + (ky >> a.shift), n * a.phases + ph,
-                            &a_full[sa]);
-              if (++sa == a.n_a) { sa = 0; pha ^= 1; }
-              if (a.resident) continue;
-              for (int i0 = 0; i0 < nsub; i0 += a.b_group) {
-                const int gn = nsub - i0 < a.b_group ? nsub - i0 : a.b_group;
-                mbar_wait(&b_empty[sb], phb ^ 1);
-                mbar_expect_tx(&b_full[sb], gn * b_bytes);
-                bulk_g2s(sB + sb * a.b_stage, wsrc, gn * b_bytes, &b_full[sb]);
-                wsrc += gn * b_bytes;
-                if (++sb == a.n_b) { sb = 0; phb ^= 1; }
-              }
-            }
-          }
-      }
+  if (warp < TM_CONSUMER_WARPS) {
+    setmaxnreg_inc<232>();                               // 128 * 40 + 256 * 232 <= 64 K
+    if (a.n_tile == 256) tma_consume_act<256>(a, sA, sB, a_full, a_empty, b_full, b_empty);
+    else if (a.n_tile == 128) tma_consume_act<128>(a, sA, sB, a_full, a_empty, b_full, b_empty);
+    else tma_consume_act<64>(a, sA, sB, a_full, a_empty, b_full, b_empty);
+    return;
+  }
+  setmaxnreg_dec<40>();
+  if (warp == TM_CONSUMER_WARPS && lane == 0) {
+    int sa = 0, sb = 0;
+    uint32_t pha = 0, phb = 0;
+    if (a.resident) {                                      // one cout tile, all chunks: loaded once per CTA
+      mbar_expect_tx(&b_full[0], a.n_chunks * b_bytes);
+      for (int j = 0; j < a.n_chunks; ++j) bulk_g2s(sB + j * b_bytes, a.w_img + (int64_t)j * b_bytes, b_bytes, &b_full[0]);
     }
-  } else if (warp == 1) {
-    // The whole warp runs the (uniform) loop control so that descriptors stay in uniform registers; one elected
-    // lane issues.  Ring positions are kept incrementally (no runtime divisions on this latency-critical path).
-    const uint32_t idesc = make_idesc(128, a.n_tile, 0, 0);
-    const uint64_t desc_hi = make_desc(0, 16, 1024);              // everything but the start address
-    const bool leader = elect_one();
-    int sa = 0, sb = 0, acc = 0;
-    uint32_t pha = 0, phb = 0, phd = 0;
-    if (a.resident) mbar_wait(&b_full[0], 0);
-    const uint64_t db_res = desc_hi + (uint64_t)(smem_u32(sB) >> 4);
-    const uint64_t db_step = (uint64_t)(b_bytes >> 4);
     for (int t = blockIdx.x; t < a.total_tiles; t += gridDim.x) {
-      mbar_wait(&d_empty[acc], phd ^ 1);
-      tc_fence_after();
-      const uint32_t dcol = tmem + acc * a.acc_stride;
-      uint32_t accum = 0;
-      uint64_t db_run = db_res;                            // resident mode: descriptor of the next weight chunk
-      for (int ky = 0; ky < d.KH; ++ky)
-        for (int xpar = 0; xpar < s && xpar < d.KW; ++xpar) {
-          const int nsub = (d.KW - xpar + s - 1) / s;
-          for (int cc = 0; cc < a.cchunks; ++cc) {
-            mbar_wait(&a_full[sa], pha);
-            const uint32_t pa = smem_u32(sA + sa * a.a_stage);
-            const int left = d.Cin - cc * 64;
-            const int ksteps = ((left < 64 ? left : 64) + 15) >> 4;
-            if (a.resident) {
-              tc_fence_after();
-              if (leader) {
-                uint64_t da = desc_hi + (uint64_t)(pa >> 4);
-                for (int i = 0; i < nsub; ++i, da += 8, db_run += db_step)
-                  for (int ks = 0; ks < ksteps; ++ks, accum = 1u) mma_ss(dcol, da + 2 * ks, db_run + 2 * ks, idesc, accum);
-                mma_commit(&a_empty[sa]);
-              } else {
-                db_run += db_step * nsub;
-              }
-              __syncwarp();
-              if (++sa == a.n_a) { sa = 0; pha ^= 1; }
-              continue;
-            }
-            for (int i0 = 0; i0 < nsub; i0 += a.b_group) {
-              const int gn = nsub - i0 < a.b_group ? nsub - i0 : a.b_group;
-              mbar_wait(&b_full[sb], phb);
-              tc_fence_after();
-              const uint32_t pb = smem_u32(sB + sb * a.b_stage);
-              if (leader) {
-                for (int i = 0; i < gn; ++i) {
-                  const uint64_t da = desc_hi + (uint64_t)((pa + (i0 + i) * 128) >> 4);
-                  const uint64_t db = desc_hi + (uint64_t)((pb + i * b_bytes) >> 4);
-                  if (!a.split) {
-                    for (int ks = 0; ks < ksteps; ++ks, accum = 1u) mma_ss(dcol, da + 2 * ks, db + 2 * ks, idesc, accum);
-                  } else {                                 // (hi + lo)(hi + lo) without the lo*lo term
-                    const uint64_t da_lo = da + (uint64_t)(a_half >> 4), db_lo = db + (uint64_t)(b_half >> 4);
-                    for (int ks = 0; ks < ksteps; ++ks, accum = 1u) {
-                      mma_ss(dcol, da + 2 * ks, db + 2 * ks, idesc, accum);
-                      mma_ss(dcol, da + 2 * ks, db_lo + 2 * ks, idesc, 1u);
-                      mma_ss(dcol, da_lo + 2 * ks, db + 2 * ks, idesc, 1u);
-                    }
-                  }
-                }
-                mma_commit(&b_empty[sb]);
-              }
-              __syncwarp();
-              if (++sb == a.n_b) { sb = 0; phb ^= 1; }
-            }
-            if (leader) mma_commit(&a_empty[sa]);
-            __syncwarp();
-            if (++sa == a.n_a) { sa = 0; pha ^= 1; }
-          }
-        }
-      if (leader) mma_commit(&d_full[acc]);
-      __syncwarp();
-      if (++acc == a.n_acc) { acc = 0; phd ^= 1; }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue: two sets of 4 warps, alternate tiles
-    const int q = warp & 3, set = (warp - 2) >> 2;
-    const uint32_t tlane = tmem + ((uint32_t)(q * 32) << 16);
-    const int64_t oplane = (int64_t)a.OH * a.OW;
-    uint32_t tile_i = 0;
-    int acc = -1;
-    uint32_t phd = 1;
-    for (int t = blockIdx.x; t < a.total_tiles; t += gridDim.x, ++tile_i) {
-      if (++acc == a.n_acc) acc = 0;
-      if (acc == 0) phd ^= 1;
-      if ((int)(tile_i & 1) != set) continue;
       const int nt = t % a.n_tiles_n;
       int r = t / a.n_tiles_n;
       const int xb = r % a.x_tiles; r /= a.x_tiles;
       const int oy = r % a.OH, n = r / a.OH;
-      const int x = xb * 128 + q * 32 + lane;
-      const bool live = x < a.OW;
-      const int64_t sp = (int64_t)oy * a.OW + x;
-      const float* resp = a.res ? a.res + ((int64_t)n * d.res_c_total + d.res_c_off) * oplane + sp : nullptr;
-      float* yp = a.y ? a.y + ((int64_t)n * d.out_c_total + d.out_c_off) * oplane + sp : nullptr;
-      __half* ypix = (a.yp && live) ? a.yp + ((((int64_t)n * a.yp_hp2 + oy + a.yp_pad_h) * a.yp_wp2 + x + a.yp_pad_w) * a.yp_cp +
-                                               a.yp_c_off) : nullptr;
-      mbar_wait(&d_full[acc], phd);
-      tc_fence_after();
-      for (int c0 = 0; c0 < a.n_tile; c0 += 32) {
-        uint32_t raw[32];
-        tmem_ld32(tlane + acc * a.acc_stride + c0, raw);
-        tmem_ld_wait();
-        const int jb = nt * a.n_tile + c0;
-        int nvalid = a.n_tile - c0;
-        if (nvalid > d.Cout - jb) nvalid = d.Cout - jb;
-        if (nvalid > 32) nvalid = 32;
-        const float* bq = a.bias ? a.bias + jb : nullptr;
-        const float* rq = resp ? resp + (int64_t)jb * oplane : nullptr;
-        float* yq = yp ? yp + (int64_t)jb * oplane : nullptr;
-        __half* yk = ypix ? ypix + jb : nullptr;
-        switch (d.act) {
-          case 1: tm_store32<1>(raw, bq, d.out_scale, rq, yq, oplane, nvalid, live, lane, yk); break;
-          case 2: tm_store32<2>(raw, bq, d.out_scale, rq, yq, oplane, nvalid, live, lane, yk); break;
-          case 3: tm_store32<3>(raw, bq, d.out_scale, rq, yq, oplane, nvalid, live, lane, yk); break;
-          case 4: tm_store32<4>(raw, bq, d.out_scale, rq, yq, oplane, nvalid, live, lane, yk); break;
-          default: tm_store32<0>(raw, bq, d.out_scale, rq, yq, oplane, nvalid, live, lane, yk); break;
+      const char* wsrc = a.w_img + (int64_t)nt * a.n_chunks * b_bytes;
+      for (int ky = 0; ky < d.KH; ++ky)
+        for (int xpar = 0; xpar < s && xpar < d.KW; ++xpar) {
+          const int nsub = (d.KW - xpar + s - 1) / s;
+          const int ph = a.phases == 4 ? ((ky & 1) * 2 + xpar) : 0;
+          for (int cc = 0; cc < a.cchunks; ++cc) {
+            mbar_wait(&a_empty[sa], pha ^ 1);
+            mbar_expect_tx(&a_full[sa], a.a_rows * 128 * (1 + a.split));
+            tma_load_4d(sA + sa * a.a_stage, &xmap, cc * 64, xb * 128, oy + (ky >> a.shift), n * a.phases + ph, &a_full[sa]);
+            if (a.split)
+              tma_load_4d(sA + sa * a.a_stage + (a.a_stage >> 1), &xmap_lo, cc * 64, xb * 128, oy + (ky >> a.shift),
+                          n * a.phases + ph, &a_full[sa]);
+            if (++sa == a.n_a) { sa = 0; pha ^= 1; }
+            if (a.resident) continue;
+            for (int i0 = 0; i0 < nsub; i0 += a.b_group) {
+              const int gn = nsub - i0 < a.b_group ? nsub - i0 : a.b_group;
+              mbar_wait(&b_empty[sb], phb ^ 1);
+              mbar_expect_tx(&b_full[sb], gn * b_bytes);
+              bulk_g2s(sB + sb * a.b_stage, wsrc, gn * b_bytes, &b_full[sb]);
+              wsrc += gn * b_bytes;
+              if (++sb == a.n_b) { sb = 0; phb ^= 1; }
+            }
+          }
         }
-      }
-      tc_fence_before();
-      mbar_arrive(&d_empty[acc]);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem, 512);
 }
 
 __device__ __forceinline__ int tm_reflect(int i, int n) {
@@ -503,7 +451,8 @@ static int tma_geometry(const B200ConvDesc* d, TmaGeom* g) {
     g->n_chunks = d->KH;
   }
   g->n_tiles_n = (d->Cout + 255) / 256;
-  g->n_tile = ((d->Cout + g->n_tiles_n - 1) / g->n_tiles_n + 15) / 16 * 16;
+  const int per_tile = (d->Cout + g->n_tiles_n - 1) / g->n_tiles_n;
+  g->n_tile = per_tile <= 64 ? 64 : (per_tile <= 128 ? 128 : 256);   // the wgmma N shapes the kernel is built for
   g->pack_bytes = (int64_t)d->N * g->phases * g->HP2 * g->WP2 * g->Cp * 2;
   return B200_OK;
 }
@@ -606,16 +555,11 @@ static int launch_conv_tma(const B200ConvDesc* d, const TmaGeom& g, const float*
   }
   B200_REQUIRE(n_a >= 2 && (a.resident || n_b >= 2), "tile does not fit in shared memory");
   a.n_a = n_a; a.n_b = n_b;
-  const int cols = (g.n_tile + 31) / 32 * 32;
-  a.n_acc = 512 / cols; if (a.n_acc > TM_MAX_ACC) a.n_acc = TM_MAX_ACC; a.n_acc &= ~1;
-  a.acc_stride = 512 / a.n_acc;
-  int smem_bytes = n_a * a.a_stage + n_b * a.b_stage + TM_BAR_BYTES;
-  // each CTA allocates all 512 TMEM columns: never let two CTAs share an SM (a second tcgen05.alloc would wait forever)
-  if (smem_bytes < 120 * 1024) smem_bytes = 120 * 1024;
+  const int smem_bytes = n_a * a.a_stage + n_b * a.b_stage + TM_BAR_BYTES;
   const int64_t tiles = (int64_t)d->N * g.OH * a.x_tiles * g.n_tiles_n;
   B200_REQUIRE(tiles < (1ll << 31), "too many tiles");
   a.total_tiles = (int)tiles;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   conv2d_tma_kernel<<<(unsigned)(tiles < sms ? tiles : sms), TM_THREADS, smem_bytes, st>>>(a, map, map_lo);
@@ -657,7 +601,7 @@ int b200_conv2d_tma(const B200ConvDesc* d, const float* x, const void* w_images,
   if (int rc = tma_geometry(d, &g)) return rc;
   B200_REQUIRE(d->in_c_off >= 0 && d->in_c_off + d->Cin <= d->in_c_total && d->out_c_off >= 0 &&
                d->out_c_off + d->Cout <= d->out_c_total, "channel slice out of range");
-  if (!b200_device_supports_tc()) { set_error("b200_conv2d_tma needs a compute-capability 10.x device"); return B200_ERR_UNSUPPORTED; }
+  if (!b200_device_supports_tc()) { set_error("b200_conv2d_tma needs a compute-capability 9.x device"); return B200_ERR_UNSUPPORTED; }
   char* base = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
   if (base + g.pack_bytes > reinterpret_cast<char*>(workspace) + workspace_bytes) {
     set_error("b200_conv2d_tma: workspace too small (%lld < %lld)", (long long)workspace_bytes, (long long)(g.pack_bytes + 256));
@@ -684,7 +628,7 @@ int b200_conv2d_tma_chain(const B200ConvDesc* d, const float* x, void* in_packed
   if (int rc = tma_geometry(d, &g)) return rc;
   B200_REQUIRE(d->in_c_off >= 0 && d->in_c_off + d->Cin <= d->in_c_total && d->out_c_off >= 0 &&
                d->out_c_off + d->Cout <= d->out_c_total, "channel slice out of range");
-  if (!b200_device_supports_tc()) { set_error("b200_conv2d_tma_chain needs a compute-capability 10.x device"); return B200_ERR_UNSUPPORTED; }
+  if (!b200_device_supports_tc()) { set_error("b200_conv2d_tma_chain needs a compute-capability 9.x device"); return B200_ERR_UNSUPPORTED; }
   char* base = nullptr;
   if (in_packed) {
     B200_REQUIRE(b200_conv_tma_chainable(d), "this convolution cannot take a pre-packed input");
@@ -753,7 +697,7 @@ int64_t b200_corr_build_tc_workspace_bytes(int32_t dim, int32_t H8, int32_t W8) 
 int b200_corr_build_tc(const float* fmap1, const float* fmap2, int32_t dim, int32_t H8, int32_t W8, float* pyramid,
                        void* workspace, int64_t workspace_bytes, void* stream) {
   B200_REQUIRE(fmap1 && fmap2 && pyramid && workspace && dim > 0 && H8 >= 8 && W8 >= 8, "bad arguments");
-  if (!b200_device_supports_tc()) { set_error("b200_corr_build_tc needs a compute-capability 10.x device"); return B200_ERR_UNSUPPORTED; }
+  if (!b200_device_supports_tc()) { set_error("b200_corr_build_tc needs a compute-capability 9.x device"); return B200_ERR_UNSUPPORTED; }
   B200ConvDesc d; corr_desc(dim, H8, W8, &d);
   TmaGeom g;
   if (int rc = tma_geometry(&d, &g)) return rc;

@@ -1,6 +1,6 @@
 // fp32 CUDA-core path of the IMLP layers (B200_PREC_FP32): a register-blocked SGEMM with fused
 // epilogues, driven layer by layer.  This is the bit-faithful-fp32 mode (FFMA, fp32 accumulate) used
-// for strict parity and as the on-device cross-check of the tcgen05 path (mlp_tc.cu).
+// for strict parity and as the on-device cross-check of the tensor-core path (mlp_tc.cu).
 //
 // Restates: nn.Linear stack + ReLU + skip concat + tanh of
 //   src/models/stage_1/implicit_neural_networks.py:62-81 and its autograd.

@@ -1,7 +1,8 @@
-// tcgen05 path of the two IMLPs (B200_PREC_TC).
+// wgmma path of the two IMLPs (B200_PREC_TC).
 //
-// Every 256-wide Linear layer is a UMMA (tcgen05.mma kind::f16, M=128 rows per CTA tile, fp32
-// accumulators in TMEM).  fp32 fidelity comes from a 2-term fp16 split of BOTH operands,
+// Every 256-wide Linear layer runs on the tensor cores (wgmma m64n256k16, fp16 operands, fp32 accumulators in the
+// registers of a consumer warpgroup, 128-row CTA tiles split over two warpgroups).  fp32 fidelity comes from a 2-term
+// fp16 split of BOTH operands,
 //     v * S = hi + lo,   hi = rn_f16(v*S),  lo = rn_f16(v*S - hi)          (22-bit significand)
 // and three MMAs per product  hi*hi + hi*lo + lo*hi  (the dropped lo*lo term is 2^-22 relative).
 // S is a power of two per operand class (activations 2^4, weights 2^8, gradients chosen per
@@ -9,17 +10,16 @@
 //
 // Kernels
 //   tc_prep_kernel   fp32 parameters -> split fp16 "stage images" (the exact 128B-swizzled smem
-//                    layout a UMMA descriptor reads), W for the forward and W^T for the dgrad
-//   tc_fwd_kernel    persistent; one 128-row tile walks through ALL layers on chip: activations live
-//                    in TMEM (A operand, TS-mode MMA), weights stream L2->smem through the TMA engine
-//                    (cp.async.bulk + mbarrier ring), epilogue (8 warps) = bias + ReLU + split ->
-//                    TMEM store (next layer's A) and, via a swizzled smem staging tile + bulk store,
-//                    the activation image the weight-gradient kernel consumes; first/last (K=3 / N=2,3)
-//                    layers and the positional encoding run on CUDA cores inside the same kernel
+//                    layout a wgmma descriptor reads), W for the forward and W^T for the dgrad
+//   tc_fwd_kernel    persistent; one 128-row tile walks through ALL layers on chip: the A operand lives in
+//                    shared memory in the image layout, weights stream L2->smem through the TMA engine
+//                    (cp.async.bulk + mbarrier ring, one producer warp), the epilogue of each warpgroup
+//                    (bias + ReLU + split) rewrites its rows of the A tile in place and bulk-stores them as the
+//                    activation image the weight-gradient kernel consumes; first/last (K=3 / N=2,3) layers and the
+//                    positional encoding run on CUDA cores inside the same kernel
 //   tc_bwd_kernel    same structure for dL/dz: tanh', last layer on CUDA cores, hidden layers as
-//                    dZ * W (B = W^T images), ReLU mask from 1-bit flags, bias gradients by an
-//                    in-register butterfly column sum
-//   tc_wgrad_kernel  dW = dZ^T * H as UMMA with both operands MN-major straight from the images
+//                    dZ * W (B = W^T images), ReLU mask from 1-bit flags, bias gradients by shuffle column sums
+//   tc_wgrad_kernel  dW = dZ^T * H as wgmma with both operands MN-major straight from the images
 //                    the two kernels above left in HBM; split over rows, fp32 vector reductions
 //
 // Restates nn.Linear/ReLU/tanh/skip-concat forward+autograd of
@@ -36,7 +36,7 @@
 namespace b200 {
 using namespace ptx;
 
-constexpr int TM = 128;                 // rows per tile (UMMA M)
+constexpr int TM = 128;                 // rows per tile
 constexpr int HID = 256;
 constexpr int STAGE_BYTES = 32768;      // one weight image: 256 rows x 64 k (fp16), 128B swizzle
 constexpr float S_ACT = 16.0f;          // activation scale before the fp16 split
@@ -45,14 +45,8 @@ constexpr int ATOM_BYTES = TM * 128;    // one 64-column block of a tile image, 
 constexpr int TILE_IMG_BYTES = 4 * ATOM_BYTES;   // one term of one [128 x 256] activation tile image: 64 KB
 constexpr int PE_COLS = 40;
 
-constexpr int EPI_WARPS = 16;
-constexpr int EPI_THREADS = EPI_WARPS * 32;
-constexpr int TC_THREADS = 64 + EPI_THREADS;   // warp 0: TMA producer, warp 1: MMA issuer, warps 2..17: epilogue
-constexpr uint32_t TMEM_COLS = 512;
-constexpr uint32_t TM_D = 0, TM_AHI = 256, TM_ALO = 384;
-
 // Tile image = 4 atom blocks (64 columns each); an atom block is [16 groups of 8 rows][8 rows x 128 B]
-// with the 16-byte chunks of a row XOR-swizzled by (row & 7).  The same bytes are a K-major SW128 UMMA
+// with the 16-byte chunks of a row XOR-swizzled by (row & 7).  The same bytes are a K-major SW128 wgmma
 // operand (M/N = rows, K = the 64 columns) and an MN-major SW128 operand (MN = columns, K = rows).
 __host__ __device__ __forceinline__ int atom_off(int m, int k) {          // k in [0, 64)
   const int r = m & 7;
@@ -166,7 +160,7 @@ __global__ void tc_prep_kernel(const PrepJobs* __restrict__ jobs_ptr) {
 // shared pieces of the fused kernels
 // ---------------------------------------------------------------------------------------------
 template <int NST>
-struct Pipe {                        // weight-image ring shared by producer and MMA warp
+struct Pipe {                        // weight-image ring shared by the producer warp and the consumer warpgroups
   uint64_t* full; uint64_t* empty; char* stage;
   uint32_t it;                       // running item counter
   __device__ __forceinline__ int slot() const { return it % NST; }
@@ -197,66 +191,6 @@ struct TileIter {                    // static round-robin over the live tiles o
   }
 };
 
-// MMAs of one 64-wide k chunk whose A operand is in TMEM (hi at TM_AHI, lo at TM_ALO):
-//   D += A_hi*B_hi + A_lo*B_hi   (B_hi image)    then   D += A_hi*B_lo   (B_lo image)
-template <int NST>
-__device__ __forceinline__ void mma_chunk_ts(Pipe<NST>& pp, uint32_t tmem, int kchunk, uint32_t idesc, bool& first) {
-  {
-    mbar_wait(&pp.full[pp.slot()], pp.parity());
-    tc_fence_after();
-    const uint32_t sb = smem_u32(pp.stage + pp.slot() * STAGE_BYTES);
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-      const uint64_t bd = make_desc(sb + ks * 32, 16, 1024);
-      mma_ts(tmem + TM_D, tmem + TM_AHI + kchunk * 32 + ks * 8, bd, idesc, first ? 0u : 1u);
-      first = false;
-      mma_ts(tmem + TM_D, tmem + TM_ALO + kchunk * 32 + ks * 8, bd, idesc, 1u);
-    }
-    mma_commit(&pp.empty[pp.slot()]);
-    ++pp.it;
-  }
-  {
-    mbar_wait(&pp.full[pp.slot()], pp.parity());
-    tc_fence_after();
-    const uint32_t sb = smem_u32(pp.stage + pp.slot() * STAGE_BYTES);
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks)
-      mma_ts(tmem + TM_D, tmem + TM_AHI + kchunk * 32 + ks * 8, make_desc(sb + ks * 32, 16, 1024), idesc, 1u);
-    mma_commit(&pp.empty[pp.slot()]);
-    ++pp.it;
-  }
-}
-// same with the A operand in shared memory (64-wide K-major SW128 tile: hi image, lo image)
-template <int NST>
-__device__ __forceinline__ void mma_chunk_ss(Pipe<NST>& pp, uint32_t tmem, const char* a_hi, const char* a_lo,
-                                             uint32_t idesc, bool& first) {
-  const uint32_t ah = smem_u32(a_hi), al = smem_u32(a_lo);
-  {
-    mbar_wait(&pp.full[pp.slot()], pp.parity());
-    tc_fence_after();
-    const uint32_t sb = smem_u32(pp.stage + pp.slot() * STAGE_BYTES);
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-      const uint64_t bd = make_desc(sb + ks * 32, 16, 1024);
-      mma_ss(tmem + TM_D, make_desc(ah + ks * 32, 16, 1024), bd, idesc, first ? 0u : 1u);
-      first = false;
-      mma_ss(tmem + TM_D, make_desc(al + ks * 32, 16, 1024), bd, idesc, 1u);
-    }
-    mma_commit(&pp.empty[pp.slot()]);
-    ++pp.it;
-  }
-  {
-    mbar_wait(&pp.full[pp.slot()], pp.parity());
-    tc_fence_after();
-    const uint32_t sb = smem_u32(pp.stage + pp.slot() * STAGE_BYTES);
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks)
-      mma_ss(tmem + TM_D, make_desc(ah + ks * 32, 16, 1024), make_desc(sb + ks * 32, 16, 1024), idesc, 1u);
-    mma_commit(&pp.empty[pp.slot()]);
-    ++pp.it;
-  }
-}
-
 template <int NST>
 __device__ __forceinline__ void produce_items(Pipe<NST>& pp, const char* src, int n_items) {
   for (int i = 0; i < n_items; ++i) {
@@ -267,112 +201,162 @@ __device__ __forceinline__ void produce_items(Pipe<NST>& pp, const char* src, in
   }
 }
 
-// dynamic shared memory map: [weight stages][staging 2 x (hi 16K | lo 16K)][aux tile 32 KB (atlas)][consts][barriers]
-constexpr int SMEM_STAGING = 2 * 2 * ATOM_BYTES;             // 64 KB
-constexpr int SMEM_AUX = 2 * ATOM_BYTES;                     // 32 KB
-constexpr int SMEM_CONST_FLOATS = 4608;                      // 18 KB
-constexpr int SMEM_BARS = 256;
-// Both kernels stream the weights through a 4-stage ring (128 KB: a 64 KB k chunk is consumed in ~1.8 k cycles, the
-// bulk copies take 2-4 k cycles to arrive, so three stages starved the atlas kernels' MMA warp).  The atlas kernels
-// pay for the fourth stage and their positional-encoding tile with single-buffered image staging.
-template <bool ATLAS> struct KCfg {
-  static constexpr int NST = 4;
-  static constexpr int STAGING_BUFS = ATLAS ? 1 : 2;
-  static constexpr int STAGING = STAGING_BUFS * 4 * 8192;
-  static constexpr int SMEM = NST * STAGE_BYTES + STAGING + (ATLAS ? SMEM_AUX : 0) + SMEM_CONST_FLOATS * 4 + SMEM_BARS;
+// Thread geometry of the fused kernels: warps 0..7 are two consumer warpgroups, each owning 64 rows of the 128-row tile
+// (its A operand rows, its wgmma accumulator rows); warps 8..11 are the producer warpgroup (one lane streams the weight
+// images).  Registers are allotted per warpgroup: the producer gives most of its share to the consumers.
+constexpr int CONSUMER_WGS = 2;
+constexpr int CONSUMERS = CONSUMER_WGS * 128;
+constexpr int TC_THREADS = CONSUMERS + 128;
+constexpr int PRODUCER_REGS = 56, CONSUMER_REGS = 224;      // 128 * 56 + 256 * 224 <= 64 K
+constexpr int EMPTY_ARRIVALS = CONSUMER_WGS * 4;      // one per consumer warp
+constexpr int WG_ROW_BYTES = 8192;                    // a warpgroup's 64 rows inside one 64-column atom block
+
+struct Consumer {
+  int g, w4, lane, q, tid;       // warpgroup, warp in the group, lane, lane % 4, thread index in the group
+  int m0;                        // first of this thread's two tile rows (m0, m0 + 8)
+  bool warp_leader, leader;      // lane 0 of the warp / thread 0 of the warpgroup
+  __device__ __forceinline__ void init() {
+    const int warp = warp_uniform();
+    lane = threadIdx.x & 31; q = lane & 3;
+    g = warp >> 2; w4 = warp & 3;
+    tid = threadIdx.x & 127;
+    m0 = 64 * g + 16 * w4 + (lane >> 2);
+    warp_leader = lane == 0;
+    leader = tid == 0;
+  }
+  __device__ __forceinline__ void sync() const { named_bar(1 + g, 128); }
 };
 
-template <int NST, bool ATLAS>
+// A operand tile in shared memory: [term][4 atom blocks of 64 columns][128 rows x 128 B], i.e. exactly the byte layout
+// of one tile of an activation / dZ image, so it doubles as the staging buffer of the image's bulk store
+__host__ __device__ __forceinline__ int tile_off(int m, int col) { return (col >> 6) * ATOM_BYTES + atom_off(m, col & 63); }
+
+// One 32 KB weight item (B: 256 rows x 64 k, K-major SW128) against a 64-column A chunk of this warpgroup's rows:
+// D += A_hi * B (+ A_lo * B when with_lo).  The item read before this one is released once its MMAs have completed.
+template <int NST, int NN>
+__device__ __forceinline__ void consume_item(Pipe<NST>& pp, float (&acc)[NN / 2], uint32_t a_hi, uint32_t a_lo, bool with_lo,
+                                             uint32_t& scale, int& pending, const Consumer& c) {
+  mbar_wait(&pp.full[pp.slot()], pp.parity());
+  const uint32_t sb = smem_u32(pp.stage + pp.slot() * STAGE_BYTES);
+  wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) {
+    const uint64_t bd = make_desc(sb + ks * 32, 16, 1024);
+    if constexpr (NN == 256) wgmma_n256<0, 0>(*reinterpret_cast<float(*)[128]>(&acc), make_desc(a_hi + ks * 32, 16, 1024), bd, scale);
+    else wgmma_n64<0, 0>(*reinterpret_cast<float(*)[32]>(&acc), make_desc(a_hi + ks * 32, 16, 1024), bd, scale);
+    scale = 1u;
+    if (with_lo) {
+      if constexpr (NN == 256) wgmma_n256<0, 0>(*reinterpret_cast<float(*)[128]>(&acc), make_desc(a_lo + ks * 32, 16, 1024), bd, 1u);
+      else wgmma_n64<0, 0>(*reinterpret_cast<float(*)[32]>(&acc), make_desc(a_lo + ks * 32, 16, 1024), bd, 1u);
+    }
+  }
+  wgmma_commit();
+  wgmma_wait<1>();
+  if (pending >= 0 && c.warp_leader) mbar_arrive(&pp.empty[pending]);
+  pending = pp.slot();
+  ++pp.it;
+}
+// MMAs of one 64-wide k chunk:  D += A_hi*B_hi + A_lo*B_hi  (B_hi item)  then  D += A_hi*B_lo  (B_lo item)
+template <int NST, int NN>
+__device__ __forceinline__ void consume_chunk(Pipe<NST>& pp, float (&acc)[NN / 2], uint32_t a_hi, uint32_t a_lo,
+                                              uint32_t& scale, int& pending, const Consumer& c) {
+  consume_item<NST, NN>(pp, acc, a_hi, a_lo, true, scale, pending, c);
+  consume_item<NST, NN>(pp, acc, a_hi, a_lo, false, scale, pending, c);
+}
+template <int NST, int R>
+__device__ __forceinline__ void finish_pass(Pipe<NST>& pp, float (&acc)[R], int& pending, const Consumer& c) {
+  wgmma_wait<0>();
+  acc_fence(acc);
+  if (pending >= 0 && c.warp_leader) mbar_arrive(&pp.empty[pending]);
+  pending = -1;
+}
+
+// this warpgroup's rows of the A tile -> the tile of an HBM image (both terms), one bulk store per atom block and term
+__device__ __forceinline__ void store_tile_rows(const Consumer& c, const char* a_tile, char* g_img, int64_t term_stride) {
+  if (!c.leader) return;
+#pragma unroll
+  for (int term = 0; term < 2; ++term)
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      bulk_s2g(g_img + term * term_stride + j * ATOM_BYTES + c.g * WG_ROW_BYTES,
+               a_tile + term * TILE_IMG_BYTES + j * ATOM_BYTES + c.g * WG_ROW_BYTES, WG_ROW_BYTES);
+  bulk_commit();
+}
+// before the A tile is overwritten: every MMA of the warpgroup has completed (finish_pass) and the bulk store of the
+// previous contents has read them
+__device__ __forceinline__ void a_tile_reusable(const Consumer& c) {
+  if (c.leader) bulk_wait_read0();
+  c.sync();
+}
+// after the A tile was written with generic stores: visible to the next MMAs (async proxy) and to the bulk store
+__device__ __forceinline__ void a_tile_written(const Consumer& c) {
+  fence_proxy_async_smem();
+  c.sync();
+}
+
+__device__ __forceinline__ uint32_t relu_flag(float v) { return (uint32_t)(-(int)__float_as_uint(v)) >> 31; }   // v > +0
+
+// ReLU flags of this thread's pair of columns (col, col+1) in its 16-column piece, OR-ed over the quad -> 16-bit word
+// (flag of column i of the piece at bit 15 - i); lane q == 0 of the quad stores it
+__device__ __forceinline__ uint32_t piece_bits(uint32_t f0, uint32_t f1, int col) {
+  const int i = col & 15;
+  uint32_t b = (f0 << (15 - i)) | (f1 << (14 - i));
+  return b;
+}
+__device__ __forceinline__ uint32_t quad_or(uint32_t b) {
+  b |= __shfl_xor_sync(0xffffffffu, b, 1);
+  b |= __shfl_xor_sync(0xffffffffu, b, 2);
+  return b;
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+// sum over the 16 rows of a warp of v (this thread's two rows already added): every lane of a column ends with it
+__device__ __forceinline__ float rows_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 4);
+  v += __shfl_xor_sync(0xffffffffu, v, 8);
+  return v + __shfl_xor_sync(0xffffffffu, v, 16);
+}
+
+// dynamic shared memory map: [A tile hi 64 KB | lo 64 KB][weight stages][aux tile 32 KB (atlas forward)][consts][barriers]
+constexpr int SMEM_A = 2 * TILE_IMG_BYTES;
+constexpr int SMEM_AUX = 2 * ATOM_BYTES;
+constexpr int SMEM_BWD_CONST_FLOATS = 7 * 256 + 768;         // bias-gradient accumulators (+ dW0 of the mapping)
+constexpr int SMEM_BARS = 256;
+// The forward kernels keep as many 32 KB weight stages as the 227 KB of shared memory allow next to the A tile (and the
+// atlas's positional-encoding tile); the backward kernels need room for their gradient accumulators.
+template <bool ATLAS, bool BWD> struct KCfg {
+  static constexpr int NST = (BWD || ATLAS) ? 2 : 3;
+  static constexpr int SMEM = SMEM_A + NST * STAGE_BYTES + (ATLAS && !BWD ? SMEM_AUX : 0) +
+                              (BWD ? SMEM_BWD_CONST_FLOATS * 4 : 0) + SMEM_BARS;
+};
+
+template <int NST>
 struct SmemMap {
-  char* stage; char* staging; char* aux; float* cst;
-  uint64_t* full; uint64_t* empty; uint64_t* a_ready; uint64_t* x_ready; uint64_t* d_ready; uint64_t* d_free;
-  uint64_t* misc; uint32_t* tmem_slot;
-  __device__ __forceinline__ void init(char* raw) {
-    char* p = raw;                                   // 1024-aligned (checked in setup_cta): keeps the
-    stage = p; p += NST * STAGE_BYTES;               // shared address space visible to the compiler (LDS/STS)
-    staging = p; p += KCfg<ATLAS>::STAGING;
-    aux = p; if (ATLAS) p += SMEM_AUX;
-    cst = reinterpret_cast<float*>(p); p += SMEM_CONST_FLOATS * 4;
+  char* a_tile; char* stage; char* aux; float* cst;
+  uint64_t* full; uint64_t* empty;
+  __device__ __forceinline__ void init(char* raw, int aux_bytes, int cst_floats) {
+    char* p = raw;                                   // 1024-aligned (checked in setup_cta)
+    a_tile = p; p += SMEM_A;
+    stage = p; p += NST * STAGE_BYTES;
+    aux = p; p += aux_bytes;
+    cst = reinterpret_cast<float*>(p); p += cst_floats * 4;
     full = reinterpret_cast<uint64_t*>(p);
     empty = full + NST;
-    a_ready = empty + NST;          // [4]: one per 64-column k chunk of the next layer's A operand
-    x_ready = a_ready + 4;          // layer-0 input of a tile is in place (atlas: positional-encoding tile)
-    d_ready = x_ready + 1;          // accumulator of the current layer pass is complete
-    d_free = d_ready + 1;           // ... and has been drained into registers by every epilogue thread
-    misc = d_free + 1;
-    tmem_slot = reinterpret_cast<uint32_t*>(misc + 2);
   }
 };
 
-template <int NST, bool ATLAS>
-__device__ __forceinline__ uint32_t setup_cta(SmemMap<NST, ATLAS>& sm, int warp) {
+template <int NST>
+__device__ __forceinline__ void setup_cta(SmemMap<NST>& sm) {
   if (threadIdx.x == 0) {
-    if (smem_u32(sm.stage) & 1023u) { printf("b200: dynamic shared memory is not 1024-byte aligned\n"); __trap(); }
-    for (int i = 0; i < NST; ++i) { mbar_init(&sm.full[i], 1); mbar_init(&sm.empty[i], 1); }
-    for (int i = 0; i < 4; ++i) mbar_init(&sm.a_ready[i], EPI_THREADS);       // every epilogue thread owns a piece of every chunk
-    mbar_init(sm.x_ready, EPI_THREADS);
-    mbar_init(sm.d_ready, 1);
-    mbar_init(sm.d_free, EPI_THREADS);
-    mbar_init(&sm.misc[0], 1);
-    mbar_init(&sm.misc[1], EPI_THREADS);
+    if (smem_u32(sm.a_tile) & 1023u) __trap();   // the swizzled operand layouts need 1024-byte alignment
+    for (int i = 0; i < NST; ++i) { mbar_init(&sm.full[i], 1); mbar_init(&sm.empty[i], EMPTY_ARRIVALS); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(sm.tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  return *sm.tmem_slot;
 }
-
-// Epilogue thread geometry: 16 warps.  A warp may only touch the TMEM lanes of quadrant (warp_id & 3); the four
-// warps of a quadrant are the column slices j = 0..3, and every warp owns a 16-column piece of EACH of the four
-// 64-column k chunks: columns [64c + 16j, 64c + 16j + 16), c = 0..3.  All 16 warps therefore finish k chunk 0 a quarter
-// of the way through the epilogue, chunk 1 at half, ...: the next layer's A operand is released chunk by chunk in
-// exactly the order the MMA warp consumes it.
-struct EpiThread {
-  int e, q, j, lane, m, tid;        // epilogue warp, TMEM quadrant, column slice, lane, tile row, 0..511
-  uint32_t tlane;
-  __device__ __forceinline__ void init(uint32_t tmem) {
-    const int warp = threadIdx.x >> 5;
-    lane = threadIdx.x & 31;
-    e = warp - 2; q = warp & 3; j = e >> 2;
-    m = q * 32 + lane;
-    tid = threadIdx.x - 64;
-    tlane = tmem + ((uint32_t)(q * 32) << 16);
-  }
-  __device__ __forceinline__ int col0(int c) const { return c * 64 + j * 16; }      // first column of the piece in chunk c
-};
-
-// Pushes one finished 16-column piece (packed hi/lo words of this thread's row) to the HBM image.  The four warps of
-// a quadrant fill one 32-row x 64-column part of an atom block = 4 KB contiguous bytes of the image per term, staged
-// in the quadrant's buffer `buf` (two alternate) and written with one bulk store per term.  Called by all four warps.
-template <int BUFS>
-__device__ __forceinline__ void stage_quad(const EpiThread& t, char* staging, int piece, const uint32_t (&ph)[8],
-                                           const uint32_t (&pl)[8], char* g_hi_atom, char* g_lo_atom) {
-  char* sh = staging + ((BUFS == 2 ? (piece & 1) : 0) * 4 + t.q) * 8192;
-  char* sl = sh + 4096;
-  const bool issuer = (t.j == 0) && t.lane == 0;
-  if (issuer) {                                          // the previous store out of this buffer has read it
-    if (BUFS == 2) bulk_wait_read1(); else bulk_wait_read0();
-  }
-  named_bar(1 + t.q, 128);
-  const int r = t.m & 7;
-  const int base = ((t.m & 31) >> 3) * 1024 + r * 128;
-#pragma unroll
-  for (int u = 0; u < 2; ++u) {
-    const int off = base + (((t.j * 2 + u) ^ r) << 4);
-    *reinterpret_cast<uint4*>(sh + off) = make_uint4(ph[4 * u], ph[4 * u + 1], ph[4 * u + 2], ph[4 * u + 3]);
-    *reinterpret_cast<uint4*>(sl + off) = make_uint4(pl[4 * u], pl[4 * u + 1], pl[4 * u + 2], pl[4 * u + 3]);
-  }
-  fence_proxy_async_smem();
-  named_bar(1 + t.q, 128);
-  if (issuer) {
-    bulk_s2g(g_hi_atom + t.q * 4096, sh, 4096);
-    bulk_s2g(g_lo_atom + t.q * 4096, sl, 4096);
-    bulk_commit();
-  }
-}
-constexpr int BAR_EPI = 9;                               // named barrier of all epilogue threads
+constexpr int BAR_CONSUMERS = 9;                         // named barrier of all consumer threads
 
 struct FwdParams {
   const float* x;            // mapping: [rows][4] (x, y, t, 0);  atlas: uv [rows][2]
@@ -390,20 +374,17 @@ struct FwdParams {
 // =============================================================================================
 // forward
 // =============================================================================================
-// Schedule of one layer pass (both fused kernels).  The accumulator D of pass n is drained into registers by the
-// 16 epilogue warps as soon as it is complete (d_ready -> 2 tcgen05.ld per thread -> d_free), which frees TMEM for
-// pass n+1 while the epilogue arithmetic of pass n is still running: the epilogue releases the next A operand one
-// 64-column k chunk at a time (a_ready[kc]: chunks 0, 1 after the block-0 half of the epilogue, 2, 3 after the
-// block-1 half) and the MMA warp consumes them in that order, so the tensor pipe works on layer l+1 underneath the
-// epilogue of layer l.
+// One 128-row tile walks through all layers on chip.  Per layer each consumer warpgroup runs the MMAs of its 64 rows
+// (A tile in shared memory, weight items from the ring), then its epilogue turns the accumulator registers into the next
+// layer's A operand (bias + ReLU + flag bits + 2-term split) in place and bulk-stores those rows to the activation image.
 // VAR (with ATLAS = true): 0 = the atlas network (2 inputs, 10 frequencies, skips at 4 and 7, 3 outputs), 1 = the alpha
 // network of the segmentation variant (3 inputs, 5 frequencies, no skips, 1 output, no input gradient)
 template <bool ATLAS, int NL = (ATLAS ? 8 : 6), int VAR = 0>
 __global__ void __launch_bounds__(TC_THREADS, 1) tc_fwd_kernel(const __grid_constant__ FwdParams P) {
   extern __shared__ __align__(1024) char smem_raw[];
-  constexpr int NST = KCfg<ATLAS>::NST;
-  SmemMap<NST, ATLAS> sm; sm.init(smem_raw);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  constexpr int NST = KCfg<ATLAS, false>::NST;
+  SmemMap<NST> sm; sm.init(smem_raw, ATLAS ? SMEM_AUX : 0, 0);
+  const int warp = warp_uniform(), lane = threadIdx.x & 31;
   constexpr int L = NL;                                   // mapping-shaped networks: 6 (stage-1 script) or 4 layers
   constexpr int FIRST_TC = ATLAS ? 0 : 1;
   constexpr int LAST_TC = L - 2;
@@ -411,26 +392,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_fwd_kernel(const __grid_cons
   constexpr bool SKIPS = ATLAS && !ALPHA;                 // PE chunk concatenated at layers 4 and L-1
   constexpr int OUT = ATLAS ? (ALPHA ? 1 : 3) : 2;
   constexpr int KLAST = SKIPS ? 296 : 256;
-  // constants in shared memory: biases of layers 0..L-2 (pre-multiplied by S_ACT) at [l*256], last-layer
-  // weights (pre-divided by S_ACT) + bias, (mapping) W0, and an exchange area for the output layer
-  float* s_bias = sm.cst;
-  float* s_wlast = sm.cst + (L - 1) * 256;
-  float* s_blast = s_wlast + OUT * KLAST;
-  float* s_w0 = s_blast + 4;                              // mapping only: 768 floats
-  float* s_xch = sm.cst + SMEM_CONST_FLOATS - 3 * TM * 4; // [3][128][4] partial outputs of column slices 1..3
-  for (int i = threadIdx.x; i < (L - 1) * 256; i += blockDim.x)
-    s_bias[i] = P.params[P.b_off[i >> 8] + (i & 255)] * S_ACT;
-  for (int i = threadIdx.x; i < OUT * KLAST; i += blockDim.x) s_wlast[i] = P.params[P.w_off[L - 1] + i] * (1.0f / S_ACT);
-  if (threadIdx.x < OUT) s_blast[threadIdx.x] = P.params[P.b_off[L - 1] + threadIdx.x];
-  if (!ATLAS)      // W0 (256 x 3) transposed to [3][256] so that column pairs are adjacent (FFMA2)
-    for (int i = threadIdx.x; i < 768; i += blockDim.x) s_w0[(i % 3) * 256 + i / 3] = P.params[P.w_off[0] + i] * S_ACT;
-  const uint32_t tmem = setup_cta(sm, warp);
+  setup_cta(sm);
   TileIter ti; ti.init(P.cap, P.n_groups, P.n_valid, P.flow_groups);
-  constexpr uint32_t IDESC = make_idesc(128, 256, 0, 0);
 
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer (consumption order)
-    if (lane == 0) {
+  if (warp >= CONSUMER_WGS * 4) {
+    // ------------------------------------------------------------------ producer (consumption order)
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == CONSUMER_WGS * 4 && lane == 0) {
       Pipe<NST> pp{sm.full, sm.empty, sm.stage, 0};
       for (int t = blockIdx.x; t < ti.total; t += gridDim.x)
         for (int l = FIRST_TC; l <= LAST_TC; ++l) {
@@ -440,45 +408,48 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_fwd_kernel(const __grid_cons
           produce_items(pp, base, 8);
         }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      Pipe<NST> pp{sm.full, sm.empty, sm.stage, 0};
-      uint32_t pass = 0, ts_pass = 0, x_par = 0;
-      for (int t = blockIdx.x; t < ti.total; t += gridDim.x) {
-        for (int l = FIRST_TC; l <= LAST_TC; ++l) {
-          if (pass > 0) mbar_wait(sm.d_free, (pass - 1) & 1);      // D of the previous pass is in registers
-          bool first = true;
-          if (ATLAS && l == 0) { mbar_wait(sm.x_ready, x_par); x_par ^= 1; }
-          tc_fence_after();
-          if (ATLAS && (l == 0 || (SKIPS && l == 4))) mma_chunk_ss(pp, tmem, sm.aux, sm.aux + ATOM_BYTES, IDESC, first);
-          if (l > 0) {
-            for (int kc = 0; kc < 4; ++kc) {
-              mbar_wait(&sm.a_ready[kc], ts_pass & 1);
-              tc_fence_after();
-              mma_chunk_ts(pp, tmem, kc, IDESC, first);
-            }
-            ++ts_pass;
-          }
-          mma_commit(sm.d_ready);
-          ++pass;
-        }
+    return;
+  }
+  // ------------------------------------------------------------------ consumer warpgroups
+  setmaxnreg_inc<CONSUMER_REGS>();
+  Consumer c; c.init();
+  Pipe<NST> pp{sm.full, sm.empty, sm.stage, 0};
+  int pending = -1;
+  const float inv_scale = 1.0f / S_W;                   // D / (S_a S_w) * S_a : activations stay scaled by S_ACT
+  uint16_t* bits16 = reinterpret_cast<uint16_t*>(P.img.bits);
+  const float* wlast = P.params + P.w_off[L - 1];
+  const uint32_t a_rows = smem_u32(sm.a_tile) + c.g * WG_ROW_BYTES;
+  const uint32_t aux_rows = smem_u32(sm.aux) + c.g * WG_ROW_BYTES;
+  float acc[128];
+  for (int t = blockIdx.x; t < ti.total; t += gridDim.x) {
+    const int gt = ti.global_tile(t);
+    const int64_t row0 = (int64_t)gt * TM + c.m0;
+    // epilogue store of one column pair of one row: split into the A tile, flags into `bw`
+    auto put = [&](int m, int col, float v0, float v1) {
+      uint32_t h, lo;
+      split2_packed(v0, v1, h, lo);
+      const int off = tile_off(m, col);
+      *reinterpret_cast<uint32_t*>(sm.a_tile + off) = h;
+      *reinterpret_cast<uint32_t*>(sm.a_tile + TILE_IMG_BYTES + off) = lo;
+    };
+    // flags of the two 8-column groups of a 16-column piece: the even group is held, the odd one completes the word
+    uint32_t held0 = 0, held1 = 0;
+    auto flags_out = [&](int slot, int i, int col, uint32_t b0, uint32_t b1) {
+      if ((i & 1) == 0) { held0 = b0; held1 = b1; return; }
+      b0 = quad_or(b0 | held0); b1 = quad_or(b1 | held1);
+      if (P.store_images && c.q == 0) {
+        bits16[((int64_t)slot * P.img.rows + row0) * 16 + (col >> 4)] = (uint16_t)b0;
+        bits16[((int64_t)slot * P.img.rows + row0 + 8) * 16 + (col >> 4)] = (uint16_t)b1;
       }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue warps (512 threads)
-    EpiThread et; et.init(tmem);
-    const int m = et.m, j = et.j;
-    uint32_t d_par = 0;
-    const float inv_scale = 1.0f / S_W;                 // D / (S_a S_w) * S_a : activations stay scaled by S_ACT
-    uint16_t* bits16 = reinterpret_cast<uint16_t*>(P.img.bits);
-    for (int t = blockIdx.x; t < ti.total; t += gridDim.x) {
-      const int gt = ti.global_tile(t);
-      const int64_t row = (int64_t)gt * TM + m;
-      // ---------------- prologue: layer-0 input
-      if (ATLAS) {
-        // positional encoding of in = x*in_scale+in_shift (implicit_neural_networks.py:9-13) into the aux tile
-        // (K-major SW128, columns k*4 + {sin x0, sin x1, cos x0, cos x1}); slice j does the 8-column chunks 2j, 2j+1
+    };
+    // ---------------- prologue: layer-0 input
+    if (ATLAS) {
+      // positional encoding of in = x*in_scale+in_shift (implicit_neural_networks.py:9-13) into the aux tile
+      // (K-major SW128, columns k*4 + {sin x0, sin x1, cos x0, cos x1}); 8-column chunks of this warpgroup's rows
+      c.sync();                                          // previous tile's readers of the aux rows are done
+      for (int task = c.tid; task < 64 * 8; task += 128) {
+        const int m = 64 * c.g + (task & 63), c8 = task >> 6;
+        const int64_t row = (int64_t)gt * TM + m;
         float in[3] = {0.f, 0.f, 0.f};
         if (ALPHA) {                                     // rows padded to 4 floats, like the mapping's
           const float4 xv = *reinterpret_cast<const float4*>(P.x + row * 4);
@@ -487,26 +458,21 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_fwd_kernel(const __grid_cons
           const float2 uv = *reinterpret_cast<const float2*>(P.x + row * 2);
           in[0] = uv.x * P.in_scale + P.in_shift; in[1] = uv.y * P.in_scale + P.in_shift;
         }
-        char* a_hi = sm.aux;
-        char* a_lo = sm.aux + ATOM_BYTES;
-        char* g_hi = P.img.pe + (int64_t)gt * ATOM_BYTES;
-        char* g_lo = g_hi + P.img.w64_term_stride;
-        for (int c8 = 2 * j; c8 < 2 * j + 2; ++c8) {     // chunks of 8 columns (atlas: 2 frequencies)
-          float vals[8];
-          if (ALPHA) {
-            // column c = k*6 + r: r < 3 -> sin(x_r b_k), else cos(x_{r-3} b_k); 30 real columns
+        float vals[8];
+        if (ALPHA) {
+          // column c = k*6 + r: r < 3 -> sin(x_r b_k), else cos(x_{r-3} b_k); 30 real columns
 #pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const int c = c8 * 8 + i;
-              float v = 0.f;
-              if (c < 30) {
-                const int k = c / 6, r = c - k * 6;
-                const float a = in[r < 3 ? r : r - 3] * pe_freq(k);
-                v = r < 3 ? sinf(a) : cosf(a);
-              }
-              vals[i] = v * S_ACT;
+          for (int i = 0; i < 8; ++i) {
+            const int cc = c8 * 8 + i;
+            float v = 0.f;
+            if (cc < 30) {
+              const int k = cc / 6, r = cc - k * 6;
+              const float a = in[r < 3 ? r : r - 3] * pe_freq(k);
+              v = r < 3 ? sinf(a) : cosf(a);
             }
-          } else {
+            vals[i] = v * S_ACT;
+          }
+        } else {
 #pragma unroll
           for (int half_k = 0; half_k < 2; ++half_k) {
             const int k = c8 * 2 + half_k;
@@ -519,143 +485,119 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_fwd_kernel(const __grid_cons
             vals[half_k * 4 + 0] = s0 * S_ACT; vals[half_k * 4 + 1] = s1 * S_ACT;
             vals[half_k * 4 + 2] = c0 * S_ACT; vals[half_k * 4 + 3] = c1 * S_ACT;
           }
-          }
-          uint32_t h[4], lo[4];
-#pragma unroll
-          for (int q2 = 0; q2 < 4; ++q2) split2_f16(vals[2 * q2], vals[2 * q2 + 1], h[q2], lo[q2]);
-          const int off = atom_off(m, c8 * 8);
-          const uint4 vh = make_uint4(h[0], h[1], h[2], h[3]), vl = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-          *reinterpret_cast<uint4*>(a_hi + off) = vh;
-          *reinterpret_cast<uint4*>(a_lo + off) = vl;
-          if (P.store_images) {
-            *reinterpret_cast<uint4*>(g_hi + off) = vh;
-            *reinterpret_cast<uint4*>(g_lo + off) = vl;
-          }
         }
-        fence_proxy_async_smem();                      // generic-proxy smem writes -> visible to the MMA
-        tc_fence_before();
-        mbar_arrive(sm.x_ready);
-      } else {
-        // layer 0 (3 -> 256) on CUDA cores: h0 = relu(W0 x + b0), this thread's four 16-column pieces
-        const float4 xv = *reinterpret_cast<const float4*>(P.x + row * 4);
-        char* img = P.img.act + (int64_t)gt * TILE_IMG_BYTES;
+        uint32_t h[4], lo[4];
 #pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          const int c0 = et.col0(c);
-          uint32_t ph[8], pl[8];
-          uint32_t bw = 0;
-          const uint64_t x0 = pack2f(xv.x, xv.x), x1 = pack2f(xv.y, xv.y), x2 = pack2f(xv.z, xv.z);
-#pragma unroll
-          for (int i = 0; i < 16; i += 2) {
-            const int n = c0 + i;
-            uint64_t a = *reinterpret_cast<const uint64_t*>(s_bias + n);
-            a = fma2(x0, *reinterpret_cast<const uint64_t*>(s_w0 + n), a);
-            a = fma2(x1, *reinterpret_cast<const uint64_t*>(s_w0 + 256 + n), a);
-            a = fma2(x2, *reinterpret_cast<const uint64_t*>(s_w0 + 512 + n), a);
-            float z0, z1;
-            unpack2f(a, z0, z1);
-            const float v0 = fmaxf(z0, 0.f), v1 = fmaxf(z1, 0.f);
-            bw = push_flag(push_flag(bw, v0), v1);
-            split2_packed(v0, v1, ph[i / 2], pl[i / 2]);
-          }
-          tmem_st8(et.tlane + TM_AHI + c0 / 2, ph);
-          tmem_st8(et.tlane + TM_ALO + c0 / 2, pl);
-          tmem_st_wait();
-          tc_fence_before();
-          mbar_arrive(&sm.a_ready[c]);                 // this thread's share of k chunk c of A_1 is in TMEM
-          if (P.store_images) {
-            char* g = img + c * ATOM_BYTES;
-            stage_quad<KCfg<ATLAS>::STAGING_BUFS>(et, sm.staging, c, ph, pl, g, g + P.img.term_stride);
-            bits16[((int64_t)0 * P.img.rows + row) * 16 + (c0 >> 4)] = (uint16_t)bw;
-          }
+        for (int q2 = 0; q2 < 4; ++q2) split2_f16(vals[2 * q2], vals[2 * q2 + 1], h[q2], lo[q2]);
+        const int off = atom_off(m, c8 * 8);
+        const uint4 vh = make_uint4(h[0], h[1], h[2], h[3]), vl = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+        *reinterpret_cast<uint4*>(sm.aux + off) = vh;
+        *reinterpret_cast<uint4*>(sm.aux + ATOM_BYTES + off) = vl;
+        if (P.store_images) {
+          char* g_hi = P.img.pe + (int64_t)gt * ATOM_BYTES;
+          *reinterpret_cast<uint4*>(g_hi + off) = vh;
+          *reinterpret_cast<uint4*>(g_hi + P.img.w64_term_stride + off) = vl;
         }
       }
-      // ---------------- tensor-core layers
-      float outacc[OUT];
+      fence_proxy_async_smem();                          // generic-proxy smem writes -> visible to the MMAs
+      c.sync();
+    } else {
+      // layer 0 (3 -> 256) on CUDA cores: h0 = relu(W0 x + b0)
+      const float4 x0 = *reinterpret_cast<const float4*>(P.x + row0 * 4);
+      const float4 x1 = *reinterpret_cast<const float4*>(P.x + (row0 + 8) * 4);
+      const float* W0 = P.params + P.w_off[0];
+      const float* b0p = P.params + P.b_off[0];
+      a_tile_reusable(c);
 #pragma unroll
-      for (int jj = 0; jj < OUT; ++jj) outacc[jj] = 0.f;
-#pragma unroll 1
-      for (int l = FIRST_TC; l <= LAST_TC; ++l) {
-        mbar_wait(sm.d_ready, d_par); d_par ^= 1;
-        tc_fence_after();
-        // drain this thread's 64 accumulator columns, then hand D back to the MMA warp
-        uint32_t raw[4][16];
+      for (int i = 0; i < 32; ++i) {
+        const int col = 8 * i + 2 * c.q;
 #pragma unroll
-        for (int c = 0; c < 4; ++c) tmem_ld16(et.tlane + TM_D + et.col0(c), raw[c]);
-        tmem_ld_wait();
-        tc_fence_before();
-        mbar_arrive(sm.d_free);
-        const bool last = (l == LAST_TC);
-        char* img = P.img.act + (int64_t)l * P.img.slot_stride + (int64_t)gt * TILE_IMG_BYTES;
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          const int c0 = et.col0(c);
-          const float* bias = s_bias + l * 256 + c0;
-          uint32_t ph[8], pl[8];
-          uint32_t bw = 0;
-          const uint64_t inv2 = pack2f(inv_scale, inv_scale);
-#pragma unroll
-          for (int i = 0; i < 16; i += 2) {
-            float z0, z1;
-            unpack2f(fma2(pack2u(raw[c][i], raw[c][i + 1]), inv2, *reinterpret_cast<const uint64_t*>(bias + i)), z0, z1);
-            const float v0 = fmaxf(z0, 0.f), v1 = fmaxf(z1, 0.f);
-            bw = push_flag(push_flag(bw, v0), v1);      // flag of column i is bit 15 - i
-            if (last) {
-#pragma unroll
-              for (int jj = 0; jj < OUT; ++jj) {
-                outacc[jj] = fmaf(v0, s_wlast[jj * KLAST + c0 + i], outacc[jj]);
-                outacc[jj] = fmaf(v1, s_wlast[jj * KLAST + c0 + i + 1], outacc[jj]);
-              }
-            }
-            split2_packed(v0, v1, ph[i / 2], pl[i / 2]);
-          }
-          if (!last) {
-            tmem_st8(et.tlane + TM_AHI + c0 / 2, ph);
-            tmem_st8(et.tlane + TM_ALO + c0 / 2, pl);
-            tmem_st_wait();
-            tc_fence_before();
-            mbar_arrive(&sm.a_ready[c]);                // next layer's MMAs on k chunk c may start
-          }
-          if (P.store_images) {
-            char* g = img + c * ATOM_BYTES;
-            stage_quad<KCfg<ATLAS>::STAGING_BUFS>(et, sm.staging, c, ph, pl, g, g + P.img.term_stride);
-            bits16[((int64_t)l * P.img.rows + row) * 16 + (c0 >> 4)] = (uint16_t)bw;
-          }
+        for (int e = 0; e < 2; ++e) {
+          const int n = col + e;
+          const float bs = __ldg(b0p + n) * S_ACT;
+          const float w0 = __ldg(W0 + n * 3) * S_ACT, w1 = __ldg(W0 + n * 3 + 1) * S_ACT, w2 = __ldg(W0 + n * 3 + 2) * S_ACT;
+          acc[4 * i + e] = fmaxf(__fmaf_rn(x0.z, w2, __fmaf_rn(x0.y, w1, __fmaf_rn(x0.x, w0, bs))), 0.f);
+          acc[4 * i + 2 + e] = fmaxf(__fmaf_rn(x1.z, w2, __fmaf_rn(x1.y, w1, __fmaf_rn(x1.x, w0, bs))), 0.f);
         }
+        put(c.m0, col, acc[4 * i], acc[4 * i + 1]);
+        put(c.m0 + 8, col, acc[4 * i + 2], acc[4 * i + 3]);
+        flags_out(0, i, col, piece_bits(relu_flag(acc[4 * i]), relu_flag(acc[4 * i + 1]), col),
+                  piece_bits(relu_flag(acc[4 * i + 2]), relu_flag(acc[4 * i + 3]), col));
       }
-      // ---------------- output layer (+ skip part for the atlas) and tanh; the four column slices of a row
-      // combine through shared memory
-      if (SKIPS) {
-        const char* a_hi = sm.aux;
-        const char* a_lo = sm.aux + ATOM_BYTES;
-        for (int k = j * 10; k < j * 10 + 10; ++k) {
-          const int off = atom_off(m, k);
-          const float pv = __half2float(*reinterpret_cast<const __half*>(a_hi + off)) +
-                           __half2float(*reinterpret_cast<const __half*>(a_lo + off));     // S_ACT * pe
-#pragma unroll
-          for (int jj = 0; jj < OUT; ++jj) outacc[jj] = fmaf(pv, s_wlast[jj * KLAST + 256 + k], outacc[jj]);
-        }
-      }
-      if (j > 0) {
-#pragma unroll
-        for (int jj = 0; jj < OUT; ++jj) s_xch[((j - 1) * TM + m) * 4 + jj] = outacc[jj];
-      }
-      named_bar(BAR_EPI, EPI_THREADS);
-      if (j == 0) {
-#pragma unroll
-        for (int jj = 0; jj < OUT; ++jj) {
-          const float o = ((outacc[jj] + s_xch[(0 * TM + m) * 4 + jj]) + s_xch[(1 * TM + m) * 4 + jj]) +
-                          s_xch[(2 * TM + m) * 4 + jj] + s_blast[jj];
-          P.y[row * OUT + jj] = P.tanh_out ? tanhf(o) : o;
-        }
-      }
-      named_bar(BAR_EPI, EPI_THREADS);                   // s_xch / aux tile reuse by the next tile
+      a_tile_written(c);
+      if (P.store_images) store_tile_rows(c, sm.a_tile, P.img.act + (int64_t)gt * TILE_IMG_BYTES, P.img.term_stride);
     }
-    if (j == 0 && lane == 0) bulk_wait_all0();
+    // ---------------- tensor-core layers
+    float outacc[2][OUT];
+#pragma unroll
+    for (int jj = 0; jj < OUT; ++jj) outacc[0][jj] = outacc[1][jj] = 0.f;
+#pragma unroll 1
+    for (int l = FIRST_TC; l <= LAST_TC; ++l) {
+      uint32_t scale = 0u;
+      if (ATLAS && (l == 0 || (SKIPS && l == 4)))
+        consume_chunk<NST, 256>(pp, acc, aux_rows, aux_rows + ATOM_BYTES, scale, pending, c);
+      if (l > 0)
+        for (int kc = 0; kc < 4; ++kc)
+          consume_chunk<NST, 256>(pp, acc, a_rows + kc * ATOM_BYTES, a_rows + TILE_IMG_BYTES + kc * ATOM_BYTES, scale,
+                                  pending, c);
+      finish_pass(pp, acc, pending, c);
+      const bool last = (l == LAST_TC);
+      const float* bias = P.params + P.b_off[l];
+      a_tile_reusable(c);
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int col = 8 * i + 2 * c.q;
+        const float bs0 = __ldg(bias + col) * S_ACT, bs1 = __ldg(bias + col + 1) * S_ACT;
+        float v[4];
+        v[0] = fmaxf(__fmaf_rn(acc[4 * i], inv_scale, bs0), 0.f);
+        v[1] = fmaxf(__fmaf_rn(acc[4 * i + 1], inv_scale, bs1), 0.f);
+        v[2] = fmaxf(__fmaf_rn(acc[4 * i + 2], inv_scale, bs0), 0.f);
+        v[3] = fmaxf(__fmaf_rn(acc[4 * i + 3], inv_scale, bs1), 0.f);
+        if (last) {
+#pragma unroll
+          for (int jj = 0; jj < OUT; ++jj) {
+            const float wa = __ldg(wlast + jj * KLAST + col) * (1.0f / S_ACT);
+            const float wb = __ldg(wlast + jj * KLAST + col + 1) * (1.0f / S_ACT);
+            outacc[0][jj] = fmaf(v[1], wb, fmaf(v[0], wa, outacc[0][jj]));
+            outacc[1][jj] = fmaf(v[3], wb, fmaf(v[2], wa, outacc[1][jj]));
+          }
+        }
+        if (!last || P.store_images) {
+          put(c.m0, col, v[0], v[1]);
+          put(c.m0 + 8, col, v[2], v[3]);
+        }
+        flags_out(l, i, col, piece_bits(relu_flag(v[0]), relu_flag(v[1]), col),
+                  piece_bits(relu_flag(v[2]), relu_flag(v[3]), col));
+      }
+      a_tile_written(c);
+      if (P.store_images)
+        store_tile_rows(c, sm.a_tile, P.img.act + (int64_t)l * P.img.slot_stride + (int64_t)gt * TILE_IMG_BYTES,
+                        P.img.term_stride);
+    }
+    // ---------------- output layer (+ skip part for the atlas) and tanh; the four lanes of a quad share the rows
+    if (SKIPS) {
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int m = c.m0 + 8 * rr;
+        for (int k = c.q * 10; k < c.q * 10 + 10; ++k) {
+          const int off = atom_off(m, k);
+          const float pv = __half2float(*reinterpret_cast<const __half*>(sm.aux + off)) +
+                           __half2float(*reinterpret_cast<const __half*>(sm.aux + ATOM_BYTES + off));     // S_ACT * pe
+#pragma unroll
+          for (int jj = 0; jj < OUT; ++jj)
+            outacc[rr][jj] = fmaf(pv, __ldg(wlast + jj * KLAST + 256 + k) * (1.0f / S_ACT), outacc[rr][jj]);
+        }
+      }
+    }
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr)
+#pragma unroll
+      for (int jj = 0; jj < OUT; ++jj) {
+        const float o = quad_sum(outacc[rr][jj]) + __ldg(P.params + P.b_off[L - 1] + jj);
+        if (c.q == 0) P.y[(row0 + 8 * rr) * OUT + jj] = P.tanh_out ? tanhf(o) : o;
+      }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem, TMEM_COLS);
+  if (c.leader) bulk_wait_all0();
 }
 
 // =============================================================================================
@@ -678,70 +620,6 @@ struct BwdParams {
   int tanh_out;
 };
 
-// column sums over the 32 rows of a warp: lane j ends with sum_rows v[j]
-__device__ __forceinline__ float warp_colsum32(const float (&v)[32], int lane) {
-  float a[16];
-#pragma unroll
-  for (int i = 0; i < 16; ++i) {
-    const float send = (lane & 16) ? v[i] : v[i + 16];
-    const float keep = (lane & 16) ? v[i + 16] : v[i];
-    a[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-  }
-  float b[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const float send = (lane & 8) ? a[i] : a[i + 8];
-    const float keep = (lane & 8) ? a[i + 8] : a[i];
-    b[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
-  }
-  float c[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const float send = (lane & 4) ? b[i] : b[i + 4];
-    const float keep = (lane & 4) ? b[i + 4] : b[i];
-    c[i] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
-  }
-  float d[2];
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    const float send = (lane & 2) ? c[i] : c[i + 2];
-    const float keep = (lane & 2) ? c[i + 2] : c[i];
-    d[i] = keep + __shfl_xor_sync(0xffffffffu, send, 2);
-  }
-  const float send = (lane & 1) ? d[0] : d[1];
-  const float keep = (lane & 1) ? d[1] : d[0];
-  return keep + __shfl_xor_sync(0xffffffffu, send, 1);
-}
-
-// column sums of 16 values over the 32 rows of a warp: lanes 2k and 2k+1 end with sum_rows v[k]
-__device__ __forceinline__ float warp_colsum16(const float (&v)[16], int lane) {
-  float a[8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const float send = (lane & 16) ? v[i] : v[i + 8];
-    const float keep = (lane & 16) ? v[i + 8] : v[i];
-    a[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-  }
-  float b[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const float send = (lane & 8) ? a[i] : a[i + 4];
-    const float keep = (lane & 8) ? a[i + 4] : a[i];
-    b[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
-  }
-  float c[2];
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    const float send = (lane & 4) ? b[i] : b[i + 2];
-    const float keep = (lane & 4) ? b[i + 2] : b[i];
-    c[i] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
-  }
-  const float send = (lane & 2) ? c[0] : c[1];
-  const float keep = (lane & 2) ? c[1] : c[0];
-  const float d = keep + __shfl_xor_sync(0xffffffffu, send, 2);
-  return d + __shfl_xor_sync(0xffffffffu, d, 1);
-}
-
 // gmax_bits[0]: max |dL/drgb| (atlas network);  gmax_bits[1]: max |dL/duv| (mapping network: loss head,
 // then raised by the atlas backward, whose positional encoding multiplies gradients by up to 2^9*pi).
 __device__ __forceinline__ void grad_scales(const int* gmax_bits, bool mapping, float& s_g, float& inv_sg) {
@@ -756,99 +634,83 @@ __device__ __forceinline__ void grad_scales(const int* gmax_bits, bool mapping, 
 template <bool ATLAS, int NL = (ATLAS ? 8 : 6), int VAR = 0>
 __global__ void __launch_bounds__(TC_THREADS, 1) tc_bwd_kernel(const __grid_constant__ BwdParams P) {
   extern __shared__ __align__(1024) char smem_raw[];
-  constexpr int NST = KCfg<ATLAS>::NST;
-  SmemMap<NST, ATLAS> sm; sm.init(smem_raw);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  constexpr int NST = KCfg<ATLAS, true>::NST;
+  SmemMap<NST> sm; sm.init(smem_raw, 0, SMEM_BWD_CONST_FLOATS);
+  const int warp = warp_uniform(), lane = threadIdx.x & 31;
   constexpr int L = NL;                                   // mapping-shaped networks: 6 (stage-1 script) or 4 layers
   constexpr bool ALPHA = ATLAS && VAR == 1;
   constexpr bool SKIPS = ATLAS && !ALPHA;                 // PE chunk concatenated at layers 4 and L-1
   constexpr int OUT = ATLAS ? (ALPHA ? 1 : 3) : 2;
   constexpr int KLAST = SKIPS ? 296 : 256;
   constexpr int LOW = 1;                                  // dgrad layers L-2 .. 1 (atlas: + the dPE product)
-  constexpr int N_DGRAD = L - 2 - LOW + 1;
   constexpr bool HAS_DPE = ATLAS && !ALPHA;               // input gradient through the positional encoding
-  // shared constants: last-layer weights; bias-gradient accumulators for layers 0..L-2; (mapping) dW0; (atlas) the
-  // exchange area of the dPE partial sums
-  float* s_wlast = sm.cst;                               // OUT*KLAST (<= 888)
-  float* s_bacc = sm.cst + 896;                          // (L-1)*256 (<= 1792)
-  float* s_w0acc = s_bacc + (L - 1) * 256;               // mapping: 768   (896+1280+768 = 2944)
-  float* s_xch = sm.cst + SMEM_CONST_FLOATS - 3 * TM * 2; // atlas: [3][128][2] partial dPE sums of slices 1..3
-  for (int i = threadIdx.x; i < OUT * KLAST; i += blockDim.x) s_wlast[i] = P.params[P.w_off[L - 1] + i];
+  // shared accumulators: bias gradients of layers 0..L-2; (mapping) dW0
+  float* s_bacc = sm.cst;                                // (L-1)*256
+  float* s_w0acc = s_bacc + (L - 1) * 256;               // mapping: 768
   for (int i = threadIdx.x; i < (L - 1) * 256 + (ATLAS ? 0 : 768); i += blockDim.x) s_bacc[i] = 0.f;
-  const uint32_t tmem = setup_cta(sm, warp);
+  setup_cta(sm);
   TileIter ti; ti.init(P.cap, P.n_groups, P.n_valid, P.flow_groups);
-  constexpr uint32_t IDESC = make_idesc(128, 256, 0, 0);
-  constexpr uint32_t IDESC64 = make_idesc(128, 64, 0, 0);
   float s_g, inv_sg;
   grad_scales(P.gmax_bits, !ATLAS, s_g, inv_sg);
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp >= CONSUMER_WGS * 4) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == CONSUMER_WGS * 4 && lane == 0) {
       Pipe<NST> pp{sm.full, sm.empty, sm.stage, 0};
-      uint32_t h_par = 0;
-      for (int t = blockIdx.x; t < ti.total; t += gridDim.x) {
-        const int gt = ti.global_tile(t);
-        if (HAS_DPE) {
-          // aux tile <- positional-encoding image of this tile (hi, lo), completion on misc[0]
-          mbar_wait(&sm.misc[1], h_par ^ 1);             // previous tile's readers are done with aux
-          mbar_expect_tx(&sm.misc[0], 2 * ATOM_BYTES);
-          bulk_g2s(sm.aux, P.img.pe + (int64_t)gt * ATOM_BYTES, ATOM_BYTES, &sm.misc[0]);
-          bulk_g2s(sm.aux + ATOM_BYTES, P.img.pe + P.img.w64_term_stride + (int64_t)gt * ATOM_BYTES, ATOM_BYTES,
-                   &sm.misc[0]);
-          h_par ^= 1;
-        }
+      for (int t = blockIdx.x; t < ti.total; t += gridDim.x)
         for (int l = L - 2; l >= (HAS_DPE ? 0 : LOW); --l) produce_items(pp, P.img.w_bwd + P.img.w_bwd_layer[l], 8);
-      }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      Pipe<NST> pp{sm.full, sm.empty, sm.stage, 0};
-      uint32_t pass = 0;
-      for (int t = blockIdx.x; t < ti.total; t += gridDim.x) {
-        for (int l = 0; l < N_DGRAD + (HAS_DPE ? 1 : 0); ++l) {
-          if (pass > 0) mbar_wait(sm.d_free, (pass - 1) & 1);
-          tc_fence_after();
-          bool first = true;
-          const uint32_t idesc = (HAS_DPE && l == N_DGRAD) ? IDESC64 : IDESC;
-          for (int kc = 0; kc < 4; ++kc) {
-            mbar_wait(&sm.a_ready[kc], pass & 1);        // every pass of this kernel is a TMEM-operand pass
-            tc_fence_after();
-            mma_chunk_ts(pp, tmem, kc, idesc, first);
-          }
-          mma_commit(sm.d_ready);
-          ++pass;
-        }
-      }
-    }
-  } else {
-    EpiThread et; et.init(tmem);
-    const int m = et.m, j = et.j;
-    uint32_t d_par = 0, aux_par = 0;
-    const float inv_dgrad = inv_sg * (1.0f / S_W);        // D = (S_g dZ)(S_w W)
-    const uint16_t* bits16 = reinterpret_cast<const uint16_t*>(P.img.bits);
-    const int col_lane = lane >> 1;                        // warp_colsum16: lanes 2k, 2k+1 hold column k
-    for (int t = blockIdx.x; t < ti.total; t += gridDim.x) {
-      const int gt = ti.global_tile(t);
-      const int64_t row = (int64_t)gt * TM + m;
-      // ---------------- output layer: tanh', bias gradient, the 64-wide dZ_L image, dA_{L-1}
-      float dzl[OUT];
+    return;
+  }
+  setmaxnreg_inc<CONSUMER_REGS>();
+  Consumer c; c.init();
+  Pipe<NST> pp{sm.full, sm.empty, sm.stage, 0};
+  int pending = -1;
+  const float inv_dgrad = inv_sg * (1.0f / S_W);          // D = (S_g dZ)(S_w W)
+  const uint16_t* bits16 = reinterpret_cast<const uint16_t*>(P.img.bits);
+  const float* wlast = P.params + P.w_off[L - 1];
+  const uint32_t a_rows = smem_u32(sm.a_tile) + c.g * WG_ROW_BYTES;
+  float acc[128];
+  // bias-gradient column sums of one column pair (this thread's two rows), then over the warp's 16 rows
+  auto col_sums = [&](float* dst, int col, float a0, float a1) {
+    a0 = rows_sum(a0); a1 = rows_sum(a1);
+    if ((lane >> 2) == 0) { atomicAdd(dst + col, a0); atomicAdd(dst + col + 1, a1); }
+  };
+  auto put = [&](int m, int col, float v0, float v1) {
+    uint32_t h, lo;
+    split2_packed(__fmul_rn(v0, s_g), __fmul_rn(v1, s_g), h, lo);
+    const int off = tile_off(m, col);
+    *reinterpret_cast<uint32_t*>(sm.a_tile + off) = h;
+    *reinterpret_cast<uint32_t*>(sm.a_tile + TILE_IMG_BYTES + off) = lo;
+  };
+  for (int t = blockIdx.x; t < ti.total; t += gridDim.x) {
+    const int gt = ti.global_tile(t);
+    const int64_t row0 = (int64_t)gt * TM + c.m0;
+    // ---------------- output layer: tanh', bias gradient, the 64-wide dZ_L image, dA_{L-1}
+    float dzl[2][OUT];
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr)
 #pragma unroll
       for (int jj = 0; jj < OUT; ++jj) {
+        const int64_t row = row0 + 8 * rr;
         const float yv = P.y[row * OUT + jj];
-        dzl[jj] = P.dy[row * OUT + jj] * (P.tanh_out ? (1.0f - yv * yv) : 1.0f);
+        dzl[rr][jj] = P.dy[row * OUT + jj] * (P.tanh_out ? (1.0f - yv * yv) : 1.0f);
       }
-      if (j == 0) {
 #pragma unroll
-        for (int jj = 0; jj < OUT; ++jj) {
-          float sj = dzl[jj];
+    for (int jj = 0; jj < OUT; ++jj) {
+      float sj = c.q == 0 ? dzl[0][jj] + dzl[1][jj] : 0.f;
 #pragma unroll
-          for (int o = 16; o > 0; o >>= 1) sj += __shfl_xor_sync(0xffffffffu, sj, o);
-          if (lane == 0 && sj != 0.f) atomicAdd(P.grads + P.b_off[L - 1] + jj, sj);
-        }
-        // image row: columns 0..OUT-1 = S_g * dz, rest zero
+      for (int o = 16; o > 0; o >>= 1) sj += __shfl_xor_sync(0xffffffffu, sj, o);
+      if (lane == 0 && sj != 0.f) atomicAdd(P.grads + P.b_off[L - 1] + jj, sj);
+    }
+    if (c.q == 0) {
+      // image row: columns 0..OUT-1 = S_g * dz, rest zero
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int m = c.m0 + 8 * rr;
         uint32_t h0, l0, h1 = 0, l1 = 0;
-        split2_f16(dzl[0] * s_g, OUT > 1 ? dzl[OUT > 1 ? 1 : 0] * s_g : 0.f, h0, l0);
-        if (OUT == 3) split2_f16(dzl[OUT - 1] * s_g, 0.f, h1, l1);
+        split2_f16(dzl[rr][0] * s_g, OUT > 1 ? dzl[rr][OUT > 1 ? 1 : 0] * s_g : 0.f, h0, l0);
+        if (OUT == 3) split2_f16(dzl[rr][OUT - 1] * s_g, 0.f, h1, l1);
         char* g_hi = P.img.dzl + (int64_t)gt * ATOM_BYTES;
         char* g_lo = g_hi + P.img.w64_term_stride;
         const int r = m & 7;
@@ -860,177 +722,143 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_bwd_kernel(const __grid_cons
           *reinterpret_cast<uint4*>(g_lo + off) = c16 == 0 ? make_uint4(l0, l1, 0, 0) : make_uint4(0, 0, 0, 0);
         }
       }
-      // dA_{L-1}[k] = sum_j dz[j] W_last[j][k], masked by relu'(h_{L-2}) -> dZ_{L-2}
-      {
-        char* img = P.img.dz + (int64_t)(L - 2) * P.img.slot_stride + (int64_t)gt * TILE_IMG_BYTES;
+    }
+    // dA_{L-1}[k] = sum_j dz[j] W_last[j][k], masked by relu'(h_{L-2}) -> dZ_{L-2}
+    a_tile_reusable(c);
 #pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          const int c0 = et.col0(c);
-          const uint32_t bits = bits16[((int64_t)(L - 2) * P.img.rows + row) * 16 + (c0 >> 4)];
-          float v[16];
+    for (int i = 0; i < 32; ++i) {
+      const int col = 8 * i + 2 * c.q;
+      const uint32_t bits0 = bits16[((int64_t)(L - 2) * P.img.rows + row0) * 16 + (col >> 4)];
+      const uint32_t bits1 = bits16[((int64_t)(L - 2) * P.img.rows + row0 + 8) * 16 + (col >> 4)];
+      float v[4];
 #pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            float a = 0.f;
+      for (int e = 0; e < 2; ++e) {
+        float a0 = 0.f, a1 = 0.f;
 #pragma unroll
-            for (int jj = 0; jj < OUT; ++jj) a = fmaf(dzl[jj], s_wlast[jj * KLAST + c0 + i], a);
-            v[i] = ((bits >> (15 - i)) & 1u) ? a : 0.f;
-          }
-          {
-            const float cs = warp_colsum16(v, lane);
-            if (!(lane & 1)) atomicAdd(&s_bacc[(L - 2) * 256 + c0 + col_lane], cs);
-          }
-          uint32_t ph[8], pl[8];
-          const uint64_t sg2 = pack2f(s_g, s_g);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            float w0, w1;
-            unpack2f(mul2(pack2f(v[2 * i], v[2 * i + 1]), sg2), w0, w1);
-            split2_packed(w0, w1, ph[i], pl[i]);
-          }
-          tmem_st8(et.tlane + TM_AHI + c0 / 2, ph);
-          tmem_st8(et.tlane + TM_ALO + c0 / 2, pl);
-          tmem_st_wait();
-          tc_fence_before();
-          mbar_arrive(&sm.a_ready[c]);
-          char* g = img + c * ATOM_BYTES;
-          stage_quad<KCfg<ATLAS>::STAGING_BUFS>(et, sm.staging, c, ph, pl, g, g + P.img.term_stride);
+        for (int jj = 0; jj < OUT; ++jj) {
+          const float w = __ldg(wlast + jj * KLAST + col + e);
+          a0 = fmaf(dzl[0][jj], w, a0);
+          a1 = fmaf(dzl[1][jj], w, a1);
         }
+        const int sh = 15 - ((col + e) & 15);
+        v[e] = ((bits0 >> sh) & 1u) ? a0 : 0.f;
+        v[2 + e] = ((bits1 >> sh) & 1u) ? a1 : 0.f;
       }
-      // ---------------- hidden layers: dA_l = dZ_l W_l  ->  dZ_{l-1}
+      col_sums(s_bacc + (L - 2) * 256, col, v[0] + v[2], v[1] + v[3]);
+      put(c.m0, col, v[0], v[1]);
+      put(c.m0 + 8, col, v[2], v[3]);
+    }
+    a_tile_written(c);
+    store_tile_rows(c, sm.a_tile, P.img.dz + (int64_t)(L - 2) * P.img.slot_stride + (int64_t)gt * TILE_IMG_BYTES,
+                    P.img.term_stride);
+    // ---------------- hidden layers: dA_l = dZ_l W_l  ->  dZ_{l-1}
 #pragma unroll 1
-      for (int l = L - 2; l >= LOW; --l) {
-        mbar_wait(sm.d_ready, d_par); d_par ^= 1;
-        tc_fence_after();
-        uint32_t raw[4][16];
+    for (int l = L - 2; l >= LOW; --l) {
+      uint32_t scale = 0u;
+      for (int kc = 0; kc < 4; ++kc)
+        consume_chunk<NST, 256>(pp, acc, a_rows + kc * ATOM_BYTES, a_rows + TILE_IMG_BYTES + kc * ATOM_BYTES, scale,
+                                pending, c);
+      finish_pass(pp, acc, pending, c);
+      const int slot = l - 1;                           // produces dZ_{l-1}
+      const bool need_img = ATLAS || slot >= 1;         // mapping dZ_0 feeds only the CUDA-core layer-0 gradient
+      const bool need_a = HAS_DPE ? true : (slot >= 1); // dZ_0 is an MMA operand only for the dPE product
+      float4 x0 = make_float4(0.f, 0.f, 0.f, 0.f), x1 = x0;
+      if (!ATLAS && slot == 0) {
+        x0 = *reinterpret_cast<const float4*>(P.x + row0 * 4);
+        x1 = *reinterpret_cast<const float4*>(P.x + (row0 + 8) * 4);
+      }
+      a_tile_reusable(c);
 #pragma unroll
-        for (int c = 0; c < 4; ++c) tmem_ld16(et.tlane + TM_D + et.col0(c), raw[c]);
-        tmem_ld_wait();
-        tc_fence_before();
-        mbar_arrive(sm.d_free);
-        const int slot = l - 1;                           // produces dZ_{l-1}
-        const bool need_img = ATLAS || slot >= 1;         // mapping dZ_0 feeds only the CUDA-core layer-0 gradient
-        const bool need_tmem = HAS_DPE ? true : (slot >= 1);   // dZ_0 is an MMA operand only for the dPE product
-        char* img = P.img.dz + (int64_t)slot * P.img.slot_stride + (int64_t)gt * TILE_IMG_BYTES;
-        float4 xv = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (!ATLAS && slot == 0) xv = *reinterpret_cast<const float4*>(P.x + row * 4);
+      for (int i = 0; i < 32; ++i) {
+        const int col = 8 * i + 2 * c.q;
+        const uint32_t bits0 = bits16[((int64_t)slot * P.img.rows + row0) * 16 + (col >> 4)];
+        const uint32_t bits1 = bits16[((int64_t)slot * P.img.rows + row0 + 8) * 16 + (col >> 4)];
+        const int sh = 15 - (col & 15);
+        float v[4];
+        v[0] = ((bits0 >> sh) & 1u) ? __fmul_rn(acc[4 * i], inv_dgrad) : 0.f;
+        v[1] = ((bits0 >> (sh - 1)) & 1u) ? __fmul_rn(acc[4 * i + 1], inv_dgrad) : 0.f;
+        v[2] = ((bits1 >> sh) & 1u) ? __fmul_rn(acc[4 * i + 2], inv_dgrad) : 0.f;
+        v[3] = ((bits1 >> (sh - 1)) & 1u) ? __fmul_rn(acc[4 * i + 3], inv_dgrad) : 0.f;
+        col_sums(s_bacc + slot * 256, col, v[0] + v[2], v[1] + v[3]);
+        if (!ATLAS && slot == 0) {
+          // layer-0 weight gradient dW0[n][d] = sum_m dZ0[m][n] * x[m][d]
+          const float xa[3] = {x0.x, x0.y, x0.z}, xb[3] = {x1.x, x1.y, x1.z};
 #pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          const int c0 = et.col0(c);
-          const uint32_t bits = bits16[((int64_t)slot * P.img.rows + row) * 16 + (c0 >> 4)];
-          float v[16];
-          const uint64_t invd2 = pack2f(inv_dgrad, inv_dgrad);
-#pragma unroll
-          for (int i = 0; i < 16; i += 2) {
-            float a0, a1;
-            unpack2f(mul2(pack2u(raw[c][i], raw[c][i + 1]), invd2), a0, a1);
-            v[i] = ((bits >> (15 - i)) & 1u) ? a0 : 0.f;
-            v[i + 1] = ((bits >> (14 - i)) & 1u) ? a1 : 0.f;
+          for (int dd = 0; dd < 3; ++dd) {
+            float s0 = rows_sum(v[0] * xa[dd] + v[2] * xb[dd]);
+            float s1 = rows_sum(v[1] * xa[dd] + v[3] * xb[dd]);
+            if ((lane >> 2) == 0) { atomicAdd(&s_w0acc[col * 3 + dd], s0); atomicAdd(&s_w0acc[(col + 1) * 3 + dd], s1); }
           }
-          {
-            const float cs = warp_colsum16(v, lane);
-            if (!(lane & 1)) atomicAdd(&s_bacc[slot * 256 + c0 + col_lane], cs);
-          }
-          if (!ATLAS && slot == 0) {
-            // layer-0 weight gradient dW0[n][d] = sum_m dZ0[m][n] * x[m][d]
-            const int n = c0 + col_lane;
-            float w[16];
+        }
+        if (need_img || need_a) {
+          put(c.m0, col, v[0], v[1]);
+          put(c.m0 + 8, col, v[2], v[3]);
+        }
+      }
+      a_tile_written(c);
+      if (need_img)
+        store_tile_rows(c, sm.a_tile, P.img.dz + (int64_t)slot * P.img.slot_stride + (int64_t)gt * TILE_IMG_BYTES,
+                        P.img.term_stride);
+    }
+    if (HAS_DPE) {
+      // ---------------- dPE = dZ_0 W_0 (64 columns, 40 real) -> d(in) -> d_in += in_scale * d(in)
+      float acc64[32];
+      uint32_t scale = 0u;
+      for (int kc = 0; kc < 4; ++kc)
+        consume_chunk<NST, 64>(pp, acc64, a_rows + kc * ATOM_BYTES, a_rows + TILE_IMG_BYTES + kc * ATOM_BYTES, scale,
+                               pending, c);
+      finish_pass(pp, acc64, pending, c);
+      const char* pe_hi = P.img.pe + (int64_t)gt * ATOM_BYTES;
+      const char* pe_lo = pe_hi + P.img.w64_term_stride;
+      float din[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
 #pragma unroll
-            for (int i = 0; i < 16; ++i) w[i] = v[i] * xv.x;
-            float cs = warp_colsum16(w, lane);
-            if (!(lane & 1)) atomicAdd(&s_w0acc[n * 3 + 0], cs);
+      for (int i = 0; i < 5; ++i) {                      // columns < PE_COLS = 40
 #pragma unroll
-            for (int i = 0; i < 16; ++i) w[i] = v[i] * xv.y;
-            cs = warp_colsum16(w, lane);
-            if (!(lane & 1)) atomicAdd(&s_w0acc[n * 3 + 1], cs);
+        for (int e = 0; e < 2; ++e) {
+          const int col = 8 * i + 2 * c.q + e;
+          const int k = col >> 2, ee = col & 3;          // ee: 0,1 = sin(x0),sin(x1); 2,3 = cos(x0),cos(x1)
+          const int pcol = (ee < 2) ? col + 2 : col - 2;  // d sin = cos * b,  d cos = -sin * b
+          const float bk = pe_freq(k);
 #pragma unroll
-            for (int i = 0; i < 16; ++i) w[i] = v[i] * xv.z;
-            cs = warp_colsum16(w, lane);
-            if (!(lane & 1)) atomicAdd(&s_w0acc[n * 3 + 2], cs);
-          }
-          if (need_img || need_tmem) {
-            uint32_t ph[8], pl[8];
-            const uint64_t sg2 = pack2f(s_g, s_g);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              float w0, w1;
-              unpack2f(mul2(pack2f(v[2 * i], v[2 * i + 1]), sg2), w0, w1);
-              split2_packed(w0, w1, ph[i], pl[i]);
-            }
-            if (need_tmem) {
-              tmem_st8(et.tlane + TM_AHI + c0 / 2, ph);
-              tmem_st8(et.tlane + TM_ALO + c0 / 2, pl);
-              tmem_st_wait();
-              tc_fence_before();
-              mbar_arrive(&sm.a_ready[c]);
-            }
-            if (need_img) {
-              char* g = img + c * ATOM_BYTES;
-              stage_quad<KCfg<ATLAS>::STAGING_BUFS>(et, sm.staging, c, ph, pl, g, g + P.img.term_stride);
-            }
+          for (int rr = 0; rr < 2; ++rr) {
+            const float g = __fmul_rn(acc64[4 * i + 2 * rr + e], inv_dgrad);
+            const int off = atom_off(c.m0 + 8 * rr, pcol);
+            const float partner = (__half2float(*reinterpret_cast<const __half*>(pe_hi + off)) +
+                                   __half2float(*reinterpret_cast<const __half*>(pe_lo + off))) * (1.0f / S_ACT);
+            din[rr][e] += (ee < 2) ? g * partner * bk : -g * partner * bk;     // ee & 1 == e
           }
         }
       }
-      if (HAS_DPE) {
-        // ---------------- dPE = dZ_0 W_0 (64 columns, 40 real) -> d(in) -> d_in += in_scale * d(in)
-        mbar_wait(sm.d_ready, d_par); d_par ^= 1;
-        tc_fence_after();
-        mbar_wait(&sm.misc[0], aux_par);                  // PE tile of this row block
-        uint32_t raw[16];                                 // slice j holds accumulator columns [16j, 16j + 16)
-        tmem_ld16(et.tlane + TM_D + j * 16, raw);
-        tmem_ld_wait();
-        tc_fence_before();
-        mbar_arrive(sm.d_free);
-        float din[2] = {0.f, 0.f};
+      float mx = 0.f;
 #pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const int col = j * 16 + i;
-          if (col < PE_COLS) {
-            const int k = col >> 2, e = col & 3;           // e: 0,1 = sin(x0),sin(x1); 2,3 = cos(x0),cos(x1)
-            const float g = __uint_as_float(raw[i]) * inv_dgrad;
-            const int pcol = (e < 2) ? col + 2 : col - 2;       // d sin = cos * b,  d cos = -sin * b
-            const int off = atom_off(m, pcol);
-            const float partner = (__half2float(*reinterpret_cast<const __half*>(sm.aux + off)) +
-                                   __half2float(*reinterpret_cast<const __half*>(sm.aux + ATOM_BYTES + off))) *
-                                  (1.0f / S_ACT);
-            const float bk = pe_freq(k);
-            din[e & 1] += (e < 2) ? g * partner * bk : -g * partner * bk;
-          }
-        }
-        if (j > 0) { s_xch[((j - 1) * TM + m) * 2] = din[0]; s_xch[((j - 1) * TM + m) * 2 + 1] = din[1]; }
-        named_bar(BAR_EPI, EPI_THREADS);
-        if (j == 0 && P.d_in) {
-          float2* dst = reinterpret_cast<float2*>(P.d_in + row * 2);
+      for (int rr = 0; rr < 2; ++rr) {
+        const float d0 = quad_sum(din[rr][0]), d1 = quad_sum(din[rr][1]);
+        if (c.q == 0 && P.d_in) {
+          float2* dst = reinterpret_cast<float2*>(P.d_in + (row0 + 8 * rr) * 2);
           float2 cur = P.d_in_accumulate ? *dst : make_float2(0.f, 0.f);
-          cur.x += P.in_scale * (((din[0] + s_xch[m * 2]) + s_xch[(TM + m) * 2]) + s_xch[(2 * TM + m) * 2]);
-          cur.y += P.in_scale * (((din[1] + s_xch[m * 2 + 1]) + s_xch[(TM + m) * 2 + 1]) + s_xch[(2 * TM + m) * 2 + 1]);
+          cur.x += P.in_scale * d0;
+          cur.y += P.in_scale * d1;
           *dst = cur;
-          float mx = fmaxf(fabsf(cur.x), fabsf(cur.y));
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-          if (lane == 0 && mx > 0.f) atomicMax(P.gmax_bits + 1, __float_as_int(mx));
+          mx = fmaxf(mx, fmaxf(fabsf(cur.x), fabsf(cur.y)));
         }
-        named_bar(BAR_EPI, EPI_THREADS);                  // s_xch reuse
-        tc_fence_before();
-        mbar_arrive(&sm.misc[1]);                         // aux tile may be overwritten
-        aux_par ^= 1;
       }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+      if (lane == 0 && mx > 0.f) atomicMax(P.gmax_bits + 1, __float_as_int(mx));
     }
-    if (j == 0 && lane == 0) bulk_wait_all0();
-    // flush the per-CTA accumulators
-    named_bar(BAR_EPI, EPI_THREADS);
-    for (int i = et.tid; i < (L - 1) * 256; i += EPI_THREADS) {
-      const float v = s_bacc[i];
-      if (v != 0.f) atomicAdd(P.grads + P.b_off[i >> 8] + (i & 255), v);
-    }
-    if (!ATLAS)
-      for (int i = et.tid; i < 768; i += EPI_THREADS) {
-        const float v = s_w0acc[i];
-        if (v != 0.f) atomicAdd(P.grads + P.w_off[0] + i, v);
-      }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem, TMEM_COLS);
+  if (c.leader) bulk_wait_all0();
+  // flush the per-CTA accumulators
+  named_bar(BAR_CONSUMERS, CONSUMERS);
+  for (int i = threadIdx.x; i < (L - 1) * 256; i += CONSUMERS) {
+    const float v = s_bacc[i];
+    if (v != 0.f) atomicAdd(P.grads + P.b_off[i >> 8] + (i & 255), v);
+  }
+  if (!ATLAS)
+    for (int i = threadIdx.x; i < 768; i += CONSUMERS) {
+      const float v = s_w0acc[i];
+      if (v != 0.f) atomicAdd(P.grads + P.w_off[0] + i, v);
+    }
 }
 
 // =============================================================================================
@@ -1041,8 +869,8 @@ struct WgradItem {
   const char* b_img;      // input image, hi (lo at +b_term): same two shapes
   int64_t a_term, b_term;
   float* out; int ld_out; // fp32 dW block [a_cols rows][ld_out], columns [0, n_cols)
-  int a_cols;             // 256: two M=128 MMAs;  64: one M=64 MMA (output-layer gradient, n_rows real rows)
-  int b_cols;             // 256 or 64
+  int a_cols;             // 256: four M=64 blocks;  64: one M=64 block (output-layer gradient, n_rows real rows)
+  int b_cols;             // 256 (four passes of 64 columns) or 64
   int n_rows, n_cols;     // real rows / columns to write
   int cap, n_groups;      // row geometry of the network this item belongs to
   int split, n_split;     // this CTA's share of the live tiles
@@ -1055,39 +883,101 @@ struct WgradItems { WgradItem it[MAX_WGRAD_ITEMS]; int n; long long cycles[256];
 constexpr int WG_STAGE = 65536;          // 32 rows: A hi 16K | A lo 16K | B hi 16K | B lo 16K, each [atom][4 groups][1 KB]
 constexpr int WG_NSTAGE = 3;
 constexpr int WG_SMEM = WG_NSTAGE * WG_STAGE + 256;
-constexpr int WG_THREADS = 192;
+constexpr int WG_THREADS = TC_THREADS;
+
+// MMAs of one 32-row step for this warpgroup's M blocks (MN-major operands: LBO = atom stride, SBO = 8-row group).
+// NMB = 2: a 256-row dW block, warpgroup g owns M blocks 2g, 2g+1;  NMB = 1: a 64-row block (output layer), both
+// warpgroups compute it (keeps the MMA sequence free of warpgroup-dependent branches), warpgroup 0 stores it.
+template <int NB, int NMB>
+__device__ __forceinline__ void wgrad_step(float (&acc)[NMB][NB / 2], uint32_t sb, int g, uint32_t& scale) {
+#pragma unroll
+  for (int ks = 0; ks < 2; ++ks) {                      // 16 rows = 2 groups per MMA
+    const uint64_t b_hi = make_desc(sb + 32768 + ks * 2048, 4096, 1024);
+    const uint64_t b_lo = make_desc(sb + 49152 + ks * 2048, 4096, 1024);
+#pragma unroll
+    for (int mb = 0; mb < NMB; ++mb) {
+      const uint32_t a = sb + (NMB == 2 ? (2 * g + mb) * 4096 : 0) + ks * 2048;
+      const uint64_t a_hi = make_desc(a, 4096, 1024), a_lo = make_desc(a + 16384, 4096, 1024);
+      if constexpr (NB == 128) {
+        wgmma_n128<1, 1>(acc[mb], a_hi, b_hi, scale);
+        wgmma_n128<1, 1>(acc[mb], a_hi, b_lo, 1u);
+        wgmma_n128<1, 1>(acc[mb], a_lo, b_hi, 1u);
+      } else {
+        wgmma_n64<1, 1>(acc[mb], a_hi, b_hi, scale);
+        wgmma_n64<1, 1>(acc[mb], a_hi, b_lo, 1u);
+        wgmma_n64<1, 1>(acc[mb], a_lo, b_hi, 1u);
+      }
+    }
+    scale = 1u;
+  }
+}
+
+template <int NB, int NMB>
+__device__ __forceinline__ void wgrad_pass(const WgradItem& W, int n_steps, int n0, char* stage, uint64_t* full,
+                                           uint64_t* empty, uint32_t& gs, const Consumer& c, float inv) {
+  float acc[NMB][NB / 2];
+  uint32_t scale = 0u;
+  int pending = -1;
+  for (int s = 0; s < n_steps; ++s, ++gs) {
+    const int slot = gs % WG_NSTAGE;
+    mbar_wait(&full[slot], (gs / WG_NSTAGE) & 1);
+    wgmma_fence();
+    wgrad_step<NB, NMB>(acc, smem_u32(stage + slot * WG_STAGE), c.g, scale);
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (pending >= 0 && c.warp_leader) mbar_arrive(&empty[pending]);
+    pending = slot;
+  }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int mb = 0; mb < NMB; ++mb) acc_fence(acc[mb]);
+  if (pending >= 0 && c.warp_leader) mbar_arrive(&empty[pending]);
+  if (NMB == 1 && c.g != 0) return;
+#pragma unroll
+  for (int mb = 0; mb < NMB; ++mb) {
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      const int n = (NMB == 2 ? (2 * c.g + mb) * 64 : 0) + 16 * c.w4 + (c.lane >> 2) + 8 * rr;   // dW row
+      if (NMB == 1 && n >= W.n_rows) continue;
+      float* orow = W.out + (int64_t)n * W.ld_out;
+#pragma unroll
+      for (int i = 0; i < NB / 8; ++i) {
+        const int k = n0 + 8 * i + 2 * c.q;
+        const float v0 = acc[mb][4 * i + 2 * rr] * inv, v1 = acc[mb][4 * i + 2 * rr + 1] * inv;
+        if (((W.ld_out & 1) == 0) && k + 1 < W.n_cols) {
+          atomicAdd(reinterpret_cast<float2*>(orow + k), make_float2(v0, v1));
+        } else {
+          if (k < W.n_cols) atomicAdd(orow + k, v0);
+          if (k + 1 < W.n_cols) atomicAdd(orow + k + 1, v1);
+        }
+      }
+    }
+  }
+}
 
 // Work units ("items" = one dW GEMM restricted to a share of the rows) are dealt round-robin: CTA b processes items b,
-// b + grid, b + 2 grid, ... (WG_UNITS_PER_CTA of them; the host builds the list).  The operand ring runs across units; the
-// accumulator is flushed (vector atomics) after every unit.
+// b + grid, b + 2 grid, ... (WG_UNITS_PER_CTA of them; the host builds the list).  A 256-column B operand is covered in
+// four passes of 64 columns, each re-reading A: a wider accumulator leaves too few registers for the asynchronous wgmma
+// pipeline.  The operand ring runs across passes and units; the accumulator is flushed (vector atomics) after every pass.
 __global__ void __launch_bounds__(WG_THREADS, 1)
 tc_wgrad_kernel(const WgradItems* __restrict__ items, const int* __restrict__ n_valid, const int* __restrict__ gmax_bits) {
   extern __shared__ __align__(1024) char smem_raw[];
-  char* p = smem_raw;
-  char* stage = p;
-  uint64_t* full = reinterpret_cast<uint64_t*>(p + WG_NSTAGE * WG_STAGE);
+  char* stage = smem_raw;
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + WG_NSTAGE * WG_STAGE);
   uint64_t* empty = full + WG_NSTAGE;
-  uint64_t* d_ready = empty + WG_NSTAGE;
-  uint64_t* d_free = d_ready + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(d_free + 1);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = warp_uniform(), lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
-    if (smem_u32(stage) & 1023u) { printf("b200: dynamic shared memory is not 1024-byte aligned\n"); __trap(); }
-    for (int i = 0; i < WG_NSTAGE; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    mbar_init(d_ready, 1);
-    mbar_init(d_free, WG_THREADS - 64);
+    if (smem_u32(stage) & 1023u) __trap();   // the swizzled operand layouts need 1024-byte alignment
+    for (int i = 0; i < WG_NSTAGE; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], EMPTY_ARRIVALS); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   const int n_items = items->n;
   const long long t_start = clock64();
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp >= CONSUMER_WGS * 4) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == CONSUMER_WGS * 4 && lane == 0) {
       uint32_t gs = 0;                                  // running stage counter across units
       for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
         const WgradItem W = items->it[it];
@@ -1095,116 +985,53 @@ tc_wgrad_kernel(const WgradItems* __restrict__ items, const int* __restrict__ n_
         const int t_begin = (int)((int64_t)ti.total * W.split / W.n_split);
         const int t_end = (int)((int64_t)ti.total * (W.split + 1) / W.n_split);
         const int a_atoms = W.a_cols / 64, b_atoms = W.b_cols / 64;
+        const int passes = b_atoms, pass_atoms = 1;     // one 64-column atom of B per pass
         const int n_steps = (t_end - t_begin) * 4;     // 32-row steps
-        for (int s = 0; s < n_steps; ++s, ++gs) {
-          const int slot = gs % WG_NSTAGE;
-          mbar_wait(&empty[slot], ((gs / WG_NSTAGE) & 1) ^ 1);
-          const int gt = ti.global_tile(t_begin + (s >> 2));
-          const int ch = s & 3;                        // 32-row chunk = groups 4ch .. 4ch+3 of every atom block
-          char* dst = stage + slot * WG_STAGE;
-          mbar_expect_tx(&full[slot], 2 * 4096 * (a_atoms + b_atoms));
-          const char* a = W.a_img + (int64_t)gt * a_atoms * ATOM_BYTES + ch * 4096;
-          for (int j = 0; j < a_atoms; ++j) {
-            bulk_g2s(dst + j * 4096, a + (int64_t)j * ATOM_BYTES, 4096, &full[slot]);
-            bulk_g2s(dst + 16384 + j * 4096, a + W.a_term + (int64_t)j * ATOM_BYTES, 4096, &full[slot]);
-          }
-          const char* b = W.b_img + (int64_t)gt * b_atoms * ATOM_BYTES + ch * 4096;
-          for (int j = 0; j < b_atoms; ++j) {
-            bulk_g2s(dst + 32768 + j * 4096, b + (int64_t)j * ATOM_BYTES, 4096, &full[slot]);
-            bulk_g2s(dst + 49152 + j * 4096, b + W.b_term + (int64_t)j * ATOM_BYTES, 4096, &full[slot]);
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      uint32_t gs = 0, unit = 0;
-      for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
-        const WgradItem W = items->it[it];
-        TileIter ti; ti.init(W.cap, W.n_groups, n_valid, W.flow_groups);
-        const int t_begin = (int)((int64_t)ti.total * W.split / W.n_split);
-        const int t_end = (int)((int64_t)ti.total * (W.split + 1) / W.n_split);
-        const int n_steps = (t_end - t_begin) * 4;
-        if (n_steps == 0) continue;
-        // smem operand: [atom][4 groups][1 KB] -> MN-major SW128: LBO (atom stride) 4096, SBO (8-row group) 1024
-        const int m_inst = W.a_cols == 256 ? 128 : 64;
-        const uint32_t idesc = make_idesc(m_inst, W.b_cols, 1, 1);
-        const int m_halves = W.a_cols == 256 ? 2 : 1;
-        if (unit > 0) { mbar_wait(d_free, (unit - 1) & 1); tc_fence_after(); }   // previous accumulator flushed
-        for (int s = 0; s < n_steps; ++s, ++gs) {
-          const int slot = gs % WG_NSTAGE;
-          mbar_wait(&full[slot], (gs / WG_NSTAGE) & 1);
-          tc_fence_after();
-          const uint32_t sb = smem_u32(stage + slot * WG_STAGE);
-#pragma unroll
-          for (int ks = 0; ks < 2; ++ks) {             // 16 rows = 2 groups per MMA
-            for (int mh = 0; mh < m_halves; ++mh) {
-              const uint32_t acc = (s | ks) ? 1u : 0u;
-              const uint32_t d = tmem + mh * W.b_cols;
-              const uint64_t a_hi = make_desc(sb + ks * 2048 + mh * 8192, 4096, 1024);
-              const uint64_t a_lo = make_desc(sb + 16384 + ks * 2048 + mh * 8192, 4096, 1024);
-              const uint64_t b_hi = make_desc(sb + 32768 + ks * 2048, 4096, 1024);
-              const uint64_t b_lo = make_desc(sb + 49152 + ks * 2048, 4096, 1024);
-              mma_ss(d, a_hi, b_hi, idesc, acc);
-              mma_ss(d, a_hi, b_lo, idesc, 1u);
-              mma_ss(d, a_lo, b_hi, idesc, 1u);
+        for (int ps = 0; ps < passes; ++ps)
+          for (int s = 0; s < n_steps; ++s, ++gs) {
+            const int slot = gs % WG_NSTAGE;
+            mbar_wait(&empty[slot], ((gs / WG_NSTAGE) & 1) ^ 1);
+            const int gt = ti.global_tile(t_begin + (s >> 2));
+            const int ch = s & 3;                      // 32-row chunk = groups 4ch .. 4ch+3 of every atom block
+            char* dst = stage + slot * WG_STAGE;
+            mbar_expect_tx(&full[slot], 2 * 4096 * (a_atoms + pass_atoms));
+            const char* a = W.a_img + (int64_t)gt * a_atoms * ATOM_BYTES + ch * 4096;
+            for (int j = 0; j < a_atoms; ++j) {
+              bulk_g2s(dst + j * 4096, a + (int64_t)j * ATOM_BYTES, 4096, &full[slot]);
+              bulk_g2s(dst + 16384 + j * 4096, a + W.a_term + (int64_t)j * ATOM_BYTES, 4096, &full[slot]);
+            }
+            const char* b = W.b_img + (int64_t)gt * b_atoms * ATOM_BYTES + ch * 4096 + (int64_t)ps * pass_atoms * ATOM_BYTES;
+            for (int j = 0; j < pass_atoms; ++j) {
+              bulk_g2s(dst + 32768 + j * 4096, b + (int64_t)j * ATOM_BYTES, 4096, &full[slot]);
+              bulk_g2s(dst + 49152 + j * 4096, b + W.b_term + (int64_t)j * ATOM_BYTES, 4096, &full[slot]);
             }
           }
-          mma_commit(&empty[slot]);
-        }
-        mma_commit(d_ready);
-        ++unit;
       }
     }
   } else {
+    setmaxnreg_inc<CONSUMER_REGS>();
+    Consumer c; c.init();
     float s_gm, inv_gm, s_ga, inv_ga;
     grad_scales(gmax_bits, true, s_gm, inv_gm);
     grad_scales(gmax_bits, false, s_ga, inv_ga);
-    const int q = warp & 3;
-    const uint32_t tlane = tmem + ((uint32_t)(q * 32) << 16);
-    uint32_t unit = 0;
+    uint32_t gs = 0;
     for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
       const WgradItem W = items->it[it];
       TileIter ti; ti.init(W.cap, W.n_groups, n_valid, W.flow_groups);
       const int t_begin = (int)((int64_t)ti.total * W.split / W.n_split);
       const int t_end = (int)((int64_t)ti.total * (W.split + 1) / W.n_split);
-      if (t_end == t_begin) continue;
+      const int n_steps = (t_end - t_begin) * 4;
+      if (n_steps == 0) continue;
       const float inv = (W.mapping ? inv_gm : inv_ga) * (1.0f / S_ACT);
-      mbar_wait(d_ready, unit & 1);
-      tc_fence_after();
-      const int m_halves = W.a_cols == 256 ? 2 : 1;
-      for (int mh = 0; mh < m_halves; ++mh) {
-        // M=128: accumulator row i of half mh lives in TMEM lane i.  M=64: rows 0..15 in lanes 0..15 of quadrant 0.
-        const int n = mh * 128 + q * 32 + lane;              // layer output index of this thread's accumulator row
-        const bool live = W.a_cols == 256 ? true : (q == 0 && lane < W.n_rows);
-        float* orow = W.out + (int64_t)n * W.ld_out;
-        for (int c = 0; c < W.b_cols / 32; ++c) {
-          uint32_t raw[32];
-          tmem_ld32(tlane + mh * W.b_cols + c * 32, raw);
-          tmem_ld_wait();
-          if (!live) continue;
-          if (((W.ld_out & 3) == 0) && c * 32 + 32 <= W.n_cols) {
-#pragma unroll
-            for (int i = 0; i < 32; i += 4)
-              atomicAdd(reinterpret_cast<float4*>(orow + c * 32 + i),
-                        make_float4(__uint_as_float(raw[i]) * inv, __uint_as_float(raw[i + 1]) * inv,
-                                    __uint_as_float(raw[i + 2]) * inv, __uint_as_float(raw[i + 3]) * inv));
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (c * 32 + i < W.n_cols) atomicAdd(orow + c * 32 + i, __uint_as_float(raw[i]) * inv);
-          }
-        }
+      // 64 output columns per pass: the accumulator (two 64 x 64 blocks) stays in registers next to the pipeline
+      for (int n0 = 0; n0 < W.b_cols; n0 += 64) {
+        if (W.a_cols == 256) wgrad_pass<64, 2>(W, n_steps, n0, stage, full, empty, gs, c, inv);
+        else wgrad_pass<64, 1>(W, n_steps, n0, stage, full, empty, gs, c, inv);
       }
-      tc_fence_before();
-      mbar_arrive(d_free);                                   // the MMA warp may overwrite the accumulator
-      ++unit;
     }
   }
-  tc_fence_before();
   __syncthreads();
   if (threadIdx.x == 0 && blockIdx.x < 256) const_cast<WgradItems*>(items)->cycles[blockIdx.x] = clock64() - t_start;
-  if (warp == 1) tmem_dealloc(tmem, TMEM_COLS);
 }
 
 // =============================================================================================
@@ -1216,7 +1043,7 @@ static int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, dev);
-    if (g_sm_count <= 0) g_sm_count = 148;
+    if (g_sm_count <= 0) g_sm_count = 132;
   }
   return g_sm_count;
 }
@@ -1229,14 +1056,14 @@ static int ensure_attrs() {
   B200_REQUIRE(dev >= 0 && dev < 64, "device ordinal %d out of range", dev);
   bool& done = done_dev[dev];
   if (done) return B200_OK;
-  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<false>::SMEM));
-  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<true>::SMEM));
-  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<false>::SMEM));
-  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<true>::SMEM));
-  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_fwd_kernel<false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<false>::SMEM));
-  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_bwd_kernel<false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<false>::SMEM));
-  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_fwd_kernel<true, 8, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<true>::SMEM));
-  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_bwd_kernel<true, 8, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<true>::SMEM));
+  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<false, false>::SMEM));
+  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<true, false>::SMEM));
+  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<false, true>::SMEM));
+  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<true, true>::SMEM));
+  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_fwd_kernel<false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<false, false>::SMEM));
+  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_bwd_kernel<false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<false, true>::SMEM));
+  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_fwd_kernel<true, 8, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<true, false>::SMEM));
+  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_bwd_kernel<true, 8, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<true, true>::SMEM));
   B200_CHECK_CUDA(cudaFuncSetAttribute(tc_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM));
   done = true;
   return B200_OK;
@@ -1306,13 +1133,14 @@ static void prep_jobs_for_net(PrepJobs& pj, const MlpShape& sh, const NetImages&
   }
 }
 
-// wgrad work list.  The kernel is HBM-bound: CTAs are balanced by bytes read per tile
-// (A + B, both terms) corrected by the measured cost of narrow steps (step_cost): with plain byte counts the CTAs of
-// the narrow GEMMs ran 1.3 - 1.6x longer than everyone else and the average SM idled 43 % of the kernel
-// measured per-CTA busy time of the kernel at the benchmark shape (tests/perf/wgrad_balance.py), per 32-row step, in units
-// of "image columns loaded": a 256x256 step (512 columns, 64 KB) is HBM-bound; a 320-column step costs 0.81 of it
-// rather than 0.625, a 128-column step 0.66 rather than 0.25 (barrier round trips and M=64 / N=64 MMAs do not shrink)
-static double step_cost(int cols) { return cols >= 512 ? 512.0 : (cols >= 320 ? 416.0 : 340.0); }
+// wgrad work list.  CTAs are balanced by a per-32-row-step cost of each GEMM, indexed by the image columns of its two
+// operands (a_cols + b_cols): narrow steps cost more than their bytes (barrier round trips and M = 64 MMAs do not
+// shrink).  On an H100 (700 W) these weights gave 1.07 ms for the kernel at the benchmark shape; plain loaded-column counts
+// over the 64-column passes gave 1.39 ms.
+static double step_cost(int a_cols, int b_cols) {
+  const int cols = a_cols + b_cols;
+  return cols >= 512 ? 512.0 : (cols >= 320 ? 416.0 : 340.0);
+}
 
 struct WgProto { const char* a; int64_t a_term; int a_cols; const char* b; int64_t b_term; int b_cols;
                  float* out; int ld; int n_rows, n_cols, groups; double bytes; int mapping; };
@@ -1322,7 +1150,7 @@ static void protos_for_net(WgProto* protos, int& np, const MlpShape& sh, const N
   auto add = [&](const char* a, int64_t a_term, int a_cols, const char* b, int64_t b_term, int b_cols, float* out, int ld,
                  int n_rows, int n_cols) {
     protos[np++] = WgProto{a, a_term, a_cols, b, b_term, b_cols, out, ld, n_rows, n_cols, groups,
-                           (double)groups * step_cost(a_cols + b_cols), is_atlas ? 0 : 1};
+                           (double)groups * step_cost(a_cols, b_cols), is_atlas ? 0 : 1};
   };
   for (int l = 1; l <= sh.L - 2; ++l)
     add(im.dz + (int64_t)l * im.slot_stride, im.term_stride, 256, im.act + (int64_t)(l - 1) * im.slot_stride,
@@ -1342,10 +1170,9 @@ static void protos_for_net(WgProto* protos, int& np, const MlpShape& sh, const N
   }
 }
 
-// One CTA per SM (each CTA owns all 512 TMEM columns); the GEMMs are cut into WG_UNITS_PER_CTA x SMs units of equal
+// One CTA per SM (each CTA needs most of the shared memory); the GEMMs are cut into WG_UNITS_PER_CTA x SMs units of equal
 // cost (largest-remainder apportionment) that the CTAs take round-robin (see tc_wgrad_kernel).  More than one unit
-// per CTA balances any cost-model error but multiplies the accumulator flushes (64 K fp32 vector atomics each): 4 units
-// per CTA cost as much in L2 atomics as they gained in balance (measured), so the default is 1.
+// per CTA balances any cost-model error but multiplies the accumulator flushes (fp32 vector atomics), so the default is 1.
 constexpr int WG_UNITS_PER_CTA = 1;
 static void apportion_items(WgradItems& wi, const WgProto* protos, int np, int cap, int flow_groups) {
   double total_bytes = 0;
@@ -1474,14 +1301,14 @@ static int run_forward(const TcStep& s, bool with_atlas, cudaStream_t st) {
   fill_fwd(pm, *s.ms, lay.map, s.x_map, s.uv, s.params, s.cap, s.n_groups, s.counters);
   pm.flow_groups = s.flow_groups;
   timer_begin(TAG_MAP_FWD, st);
-  tc_fwd_kernel<false><<<min(sm_count(), tiles_map), TC_THREADS, KCfg<false>::SMEM, st>>>(pm);
+  tc_fwd_kernel<false><<<min(sm_count(), tiles_map), TC_THREADS, KCfg<false, false>::SMEM, st>>>(pm);
   timer_end(TAG_MAP_FWD, st);
   B200_CHECK_LAUNCH();
   if (with_atlas) {
     FwdParams pa{};
     fill_fwd(pa, *s.as, lay.atl, s.uv, s.y_atlas, s.params + s.ms->total, s.cap, 3, s.counters);
     timer_begin(TAG_ATLAS_FWD, st);
-    tc_fwd_kernel<true><<<min(sm_count(), 3 * (s.cap / TM)), TC_THREADS, KCfg<true>::SMEM, st>>>(pa);
+    tc_fwd_kernel<true><<<min(sm_count(), 3 * (s.cap / TM)), TC_THREADS, KCfg<true, false>::SMEM, st>>>(pa);
     timer_end(TAG_ATLAS_FWD, st);
     B200_CHECK_LAUNCH();
   }
@@ -1521,7 +1348,7 @@ static int run_backward(const TcStep& s, bool with_atlas, cudaStream_t st) {
     fill(pa, *s.as, lay.atl, s.d_y, s.y_atlas, nullptr, const_cast<float*>(s.d_uv), s.params + s.ms->total,
          s.grads + s.ms->total, 3);
     timer_begin(TAG_ATLAS_BWD, st);
-    tc_bwd_kernel<true><<<min(sm_count(), 3 * (s.cap / TM)), TC_THREADS, KCfg<true>::SMEM, st>>>(pa);
+    tc_bwd_kernel<true><<<min(sm_count(), 3 * (s.cap / TM)), TC_THREADS, KCfg<true, true>::SMEM, st>>>(pa);
     timer_end(TAG_ATLAS_BWD, st);
     B200_CHECK_LAUNCH();
   }
@@ -1529,7 +1356,7 @@ static int run_backward(const TcStep& s, bool with_atlas, cudaStream_t st) {
   fill(pm, *s.ms, lay.map, s.d_uv, s.uv, s.x_map, nullptr, s.params, s.grads, s.n_groups);
   pm.flow_groups = s.flow_groups;
   timer_begin(TAG_MAP_BWD, st);
-  tc_bwd_kernel<false><<<min(sm_count(), s.n_groups * (s.cap / TM)), TC_THREADS, KCfg<false>::SMEM, st>>>(pm);
+  tc_bwd_kernel<false><<<min(sm_count(), s.n_groups * (s.cap / TM)), TC_THREADS, KCfg<false, true>::SMEM, st>>>(pm);
   timer_end(TAG_MAP_BWD, st);
   B200_CHECK_LAUNCH();
   timer_begin(TAG_WGRAD, st);
@@ -1601,12 +1428,12 @@ int tc_infer_forward(const MlpShape& ms, const MlpShape& as, const float* params
   FwdParams pm{};
   fill_fwd(pm, ms, im_map, x_map, uv, params, (int)rows, 1, nullptr);
   pm.store_images = 0;
-  tc_fwd_kernel<false><<<min(sm_count(), tiles), TC_THREADS, KCfg<false>::SMEM, st>>>(pm);
+  tc_fwd_kernel<false><<<min(sm_count(), tiles), TC_THREADS, KCfg<false, false>::SMEM, st>>>(pm);
   B200_CHECK_LAUNCH();
   FwdParams pa{};
   fill_fwd(pa, as, im_atl, uv, y, params + ms.total, (int)rows, 1, nullptr);
   pa.store_images = 0;
-  tc_fwd_kernel<true><<<min(sm_count(), tiles), TC_THREADS, KCfg<true>::SMEM, st>>>(pa);
+  tc_fwd_kernel<true><<<min(sm_count(), tiles), TC_THREADS, KCfg<true, false>::SMEM, st>>>(pa);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
@@ -1717,10 +1544,10 @@ int tc_single_forward(const MlpShape& sh, bool is_atlas, const float* params, co
   fill_fwd(P, sh, pl.im, x, y, params, (int)rows, 1, nullptr);
   P.in_scale = 1.0f; P.in_shift = 0.0f; P.store_images = training ? 1 : 0; P.tanh_out = sh.tanh_out ? 1 : 0;
   const int grid = min(sm_count(), (int)(rows / TM));
-  if (is_atlas && sh.in_dim == 3) tc_fwd_kernel<true, 8, 1><<<grid, TC_THREADS, KCfg<true>::SMEM, st>>>(P);
-  else if (is_atlas) tc_fwd_kernel<true><<<grid, TC_THREADS, KCfg<true>::SMEM, st>>>(P);
-  else if (sh.L == 4) tc_fwd_kernel<false, 4><<<grid, TC_THREADS, KCfg<false>::SMEM, st>>>(P);
-  else tc_fwd_kernel<false><<<grid, TC_THREADS, KCfg<false>::SMEM, st>>>(P);
+  if (is_atlas && sh.in_dim == 3) tc_fwd_kernel<true, 8, 1><<<grid, TC_THREADS, KCfg<true, false>::SMEM, st>>>(P);
+  else if (is_atlas) tc_fwd_kernel<true><<<grid, TC_THREADS, KCfg<true, false>::SMEM, st>>>(P);
+  else if (sh.L == 4) tc_fwd_kernel<false, 4><<<grid, TC_THREADS, KCfg<false, false>::SMEM, st>>>(P);
+  else tc_fwd_kernel<false><<<grid, TC_THREADS, KCfg<false, false>::SMEM, st>>>(P);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
@@ -1761,10 +1588,10 @@ int tc_single_backward(const MlpShape& sh, bool is_atlas, const float* params, f
   P.in_scale = 1.0f; P.d_in_accumulate = 0; P.tanh_out = sh.tanh_out ? 1 : 0; P.flow_groups = 0;
   for (int l = 0; l < sh.L; ++l) { P.w_off[l] = sh.w_off[l]; P.b_off[l] = sh.b_off[l]; }
   const int grid = min(sm_count(), (int)(rows / TM));
-  if (is_atlas && sh.in_dim == 3) tc_bwd_kernel<true, 8, 1><<<grid, TC_THREADS, KCfg<true>::SMEM, st>>>(P);
-  else if (is_atlas) tc_bwd_kernel<true><<<grid, TC_THREADS, KCfg<true>::SMEM, st>>>(P);
-  else if (sh.L == 4) tc_bwd_kernel<false, 4><<<grid, TC_THREADS, KCfg<false>::SMEM, st>>>(P);
-  else tc_bwd_kernel<false><<<grid, TC_THREADS, KCfg<false>::SMEM, st>>>(P);
+  if (is_atlas && sh.in_dim == 3) tc_bwd_kernel<true, 8, 1><<<grid, TC_THREADS, KCfg<true, true>::SMEM, st>>>(P);
+  else if (is_atlas) tc_bwd_kernel<true><<<grid, TC_THREADS, KCfg<true, true>::SMEM, st>>>(P);
+  else if (sh.L == 4) tc_bwd_kernel<false, 4><<<grid, TC_THREADS, KCfg<false, true>::SMEM, st>>>(P);
+  else tc_bwd_kernel<false><<<grid, TC_THREADS, KCfg<false, true>::SMEM, st>>>(P);
   B200_CHECK_LAUNCH();
   tc_wgrad_kernel<<<min(n_wg, sm_count()), WG_THREADS, WG_SMEM, st>>>(d_wg, nullptr, gmax2);
   B200_CHECK_LAUNCH();

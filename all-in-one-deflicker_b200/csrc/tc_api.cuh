@@ -1,4 +1,4 @@
-// Interface between c_api.cu and the tcgen05 path (mlp_tc.cu).
+// Interface between c_api.cu and the tensor-core (wgmma) path (mlp_tc.cu).
 #pragma once
 #include "common.cuh"
 

@@ -35,7 +35,7 @@ class UNet(nn.Module):
     def _run_block(block, x, out=None, out_c_off=0, chain_out=None, chain_c_off=0, keep_fp32=True):
         convs = [m for m in block if isinstance(m, nn.Conv2d)]
         if K.Chain.available():
-            # tcgen05 path: conv1's epilogue writes conv2's packed fp16 input directly — the intermediate tensor is
+            # wgmma path: conv1's epilogue writes conv2's packed fp16 input directly — the intermediate tensor is
             # never written in fp32 nor repacked.  `x` may itself be a chained input, and conv2 may feed a chain.
             n, h, w = (x.n, x.h, x.w) if isinstance(x, K.Chain) else (x.shape[0], x.shape[2], x.shape[3])
             dev = x.buf.device if isinstance(x, K.Chain) else x.device
@@ -53,7 +53,7 @@ class UNet(nn.Module):
         dev = x.device
         cur = x
         if K.Chain.available():
-            # tcgen05 path: the skip concatenations [upconv | encoder] exist only as the packed fp16 inputs of the decoder
+            # wgmma path: the skip concatenations [upconv | encoder] exist only as the packed fp16 inputs of the decoder
             # blocks, filled by the epilogues of the two convolutions that produce them
             dec_in = []
             for i, enc in enumerate((self.encoder1, self.encoder2, self.encoder3, self.encoder4)):

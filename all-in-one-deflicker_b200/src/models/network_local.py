@@ -47,7 +47,7 @@ class ResidualBlock(nn.Module):
         return self.conv2.run(self.conv1.run(x, "leaky"), residual=x)
 
     def run_chained(self, x_chain, x, next_chain, tag):
-        """tcgen05 path: `x_chain` is this block's packed input (written by the previous convolution), `x` the same
+        """wgmma path: `x_chain` is this block's packed input (written by the previous convolution), `x` the same
         tensor in fp32 (the residual); conv1's output exists only as conv2's packed input; conv2's output is written in
         fp32 (next residual) and into `next_chain` (the packed input of the next convolution)."""
         n, c, h, w = x.shape
@@ -103,7 +103,7 @@ class TransformNet(nn.Module):
         c2 = torch.empty(n, 4 * nf, h // 2, w // 2, dtype=torch.float32, device=dev)  # [D2 | E2a]
         e2 = torch.empty(n, 4 * nf, h // 2, w // 2, dtype=torch.float32, device=dev)  # [E2a | E2b]
         chained = K.Chain.available()
-        # tcgen05 path: the last convolution's input [D1 | E1a] (64 channels at full resolution, the largest repack of the
+        # wgmma path: the last convolution's input [D1 | E1a] (64 channels at full resolution, the largest repack of the
         # network) is filled by the epilogues of deconv2 and conv1a
         c1_chain = K.Chain(n, 2 * nf, h, w, (7, 7), 3, dev, tag="tn_c1", pad_mode="reflect") if chained else None
         self.conv1a.run(X, "leaky", in_slice=(0, 6), out=c1, out_c_off=nf, chain_out=c1_chain, chain_c_off=nf)
@@ -112,7 +112,7 @@ class TransformNet(nn.Module):
         self.conv2b.run(e1b, "leaky", out=e2, out_c_off=2 * nf)
         c2[:, 2 * nf:] = e2[:, :2 * nf]
         if K.Chain.available() and prev_state is None:
-            # tcgen05 path: conv3 -> 5 residual blocks -> ConvLSTM gates run as one chain of packed fp16 inputs (the
+            # wgmma path: conv3 -> 5 residual blocks -> ConvLSTM gates run as one chain of packed fp16 inputs (the
             # residuals stay fp32 tensors); eleven fp32 -> fp16 repack kernels less
             hq, wq = rb_shape = (h // 4, w // 4)
             chains = [K.Chain(n, 4 * nf, hq, wq, (3, 3), 1, dev, tag=f"tn_rb{i & 1}", pad_mode="reflect")

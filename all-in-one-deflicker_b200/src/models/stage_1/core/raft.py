@@ -2,7 +2,7 @@
 reference's module tree / state_dict keys and forward signature (src/models/stage_1/core/raft.py:28-148).
 Inference only (the reference never trains it).  `args.mixed_precision` keeps the reference's meaning
 (core/raft.py:99,110,131: encoders and update block under fp16 autocast, correlation in fp32): the
-convolutions of those three sub-networks then run on the tcgen05 path (fp16 operands, fp32 accumulation,
+convolutions of those three sub-networks then run on the wgmma path (fp16 operands, fp32 accumulation,
 fp32 tensors between layers); without it every convolution is the fp32 CUDA-core kernel."""
 import contextlib
 

@@ -2,7 +2,7 @@
 (src/models/stage_1/core/update.py:6-136): BasicMotionEncoder, SepConvGRU, FlowHead, mask head.
 Parameters live in nn.Conv2d modules (for checkpoints); arithmetic runs in b200_conv2d / b200_gru_gate.
 The reference runs this block under fp16 autocast; the convolution arithmetic here follows
-b200.nn.conv_precision() (RAFT.forward selects the tcgen05 fp16-operand path when args.mixed_precision)."""
+b200.nn.conv_precision() (RAFT.forward selects the wgmma fp16-operand path when args.mixed_precision)."""
 import torch
 import torch.nn as nn
 
@@ -75,7 +75,7 @@ class BasicMotionEncoder(nn.Module):
     def forward(self, flow, corr):
         n, _, h, w = flow.shape
         if K.Chain.available():
-            # tcgen05 path: each convolution's epilogue writes the packed fp16 input of the next one (the 192 + 64
+            # wgmma path: each convolution's epilogue writes the packed fp16 input of the next one (the 192 + 64
             # channel concat included) — three fp32 intermediates and three repack kernels less per iteration
             dev = flow.device
             c2 = K.Chain(n, 256, h, w, (3, 3), 1, dev, tag="convc2")

@@ -26,7 +26,7 @@ parser.add_argument("--ckpt_local", default="./pretrained_weights/local_refineme
 parser.add_argument("--fps", default=10, type=int)
 parser.add_argument("--video_name", default=None, type=str)
 parser.add_argument('--gpu', type=int, default=0)
-# not in the reference: convolution arithmetic.  "tc" = tcgen05 with fp16 operands / fp32 accumulation — the same
+# not in the reference: convolution arithmetic.  "tc" = wgmma with fp16 operands / fp32 accumulation — the same
 # operand width as the TF32 cuDNN convolutions the reference runs by default; "fp32" = CUDA-core FFMA.
 parser.add_argument('--conv_precision', choices=["tc", "fp32"], default="tc")
 

@@ -1,13 +1,12 @@
 #!/usr/bin/env python
 """Throughput of the stage-1 neural-atlas loop (BASELINE.json metric: atlas iters/sec, 80 frames
-768x432, 10 000 points per iteration) on N B200s of one node.
+768x432, 10 000 points per iteration) on N H100s of one node.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--precision tc|fp32]
-                    [--workload atlas|raft|stage2|seg]
+                    [--workload atlas|raft|stage2|seg] [--dump-outputs DIR]
 
 One "step" = one loop trip of src/stage1_neural_atlas.py:151-231 (sampling, 7 mapping + 3 atlas
-evaluations, 4 losses, backward, Adam).  Prints ONE JSON line on rank 0.  Keys beyond the driver's
-contract:
+evaluations, 4 losses, backward, Adam).  Prints ONE JSON line on rank 0.  Keys beyond the metric itself:
   roofline      every tagged launch site of the step is timed live with CUDA events (a second captured
                 graph that carries the event records, so the headline region is not perturbed); the site
                 with the largest time is reported as `kernel`, its algorithmic FLOPs come from SURVEY.md
@@ -19,6 +18,10 @@ contract:
   e2e           same metric through AtlasTrainer.step_host: pinned H2D of the index batch + D2H of
                 the loss vector + sync every step
   pretrain_steps_per_s, render_s   the two other loops of a stage-1 run (pre_train_mapping, full render)
+--dump-outputs DIR writes what the last timed step left for its caller (atlas workload of --impl b200 only; other
+workloads refuse the flag; rank 0): DIR/losses.npy (the
+loss vector) and DIR/params.npy (the flat parameters after its Adam update), float32.  Inputs are seeded, so two builds
+run with the same arguments can be compared output for output.
 `--workload raft|stage2` times BASELINE.json configs[3]/[4] (1080p) with the same line format; `--workload seg` the
 segmentation variant of the stage-1 loop (SURVEY §8 f3) at the headline geometry.
 """
@@ -39,7 +42,7 @@ sys.path.insert(0, os.path.join(ROOT, "all-in-one-deflicker_b200"))
 
 H, W, T, BATCH = 432, 768, 80, 10000          # BASELINE.json configs[1]
 MAC_MAP, MAC_ATLAS = 263424, 414584           # SURVEY.md §8: MACs per row
-CPU_THREADS = 32      # the oracle gets SLOWER beyond this on the B200 hosts (128 threads: 0.03-0.08 it/s, measured)
+CPU_THREADS = 32      # the oracle's torch CPU ops stop scaling beyond this many threads
 TAGS = {1: "map_fwd", 2: "map_bwd", 3: "atlas_fwd", 4: "atlas_bwd", 5: "wgrad", 6: "adam"}
 
 
@@ -72,7 +75,8 @@ def measured_peaks():
         with open(path) as f:
             d = json.load(f)
         return d, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # H100 SXM data sheet (700 W board): 3.35 TB/s HBM3, 989 TFLOP/s dense fp16 / bf16 — never reached, an upper bound
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "data sheet"
 
 
 class ClockSampler(threading.Thread):
@@ -179,7 +183,7 @@ ATLAS_CONFIG = {"workload": "stage-1 atlas loop, 80 frames 768x432, 10000 sample
                 "frames": T, "height": H, "width": W, "samples_batch": BATCH,
                 "regime": "first half of the timed steps with the global rigidity term (i<=5000), second half without",
                 "l2": "per-step working set (~1 GB of activation images + random gathers from 1.7 GB of pixel "
-                      "records) exceeds the 126 MB L2; no explicit flush"}
+                      "records) exceeds the 50 MB L2; no explicit flush"}
 
 
 def reference_arm(args, rank):
@@ -226,10 +230,14 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-ref-gpu", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the pre-training / render side measurements")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32)")
     ap.add_argument("--emulate-world", type=int, default=0,
                     help="profiling aid: ONE process does the work of rank 0 of an N-GPU run (frame shard 0, no "
                          "collective), so that ncu can list the per-rank kernels of the sharded step")
     args = ap.parse_args()
+    if args.dump_outputs and (args.workload != "atlas" or args.impl != "b200"):
+        ap.error("--dump-outputs covers the atlas workload of the native implementation (--workload atlas --impl b200)")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
@@ -241,7 +249,7 @@ def main():
     K, Wm = args.steps, max(args.warmup, 3)
     from b200 import synth
 
-    # ------------------------------------------------------------------ B200 arm
+    # ------------------------------------------------------------------ GPU arm
     import torch.distributed as dist
     from b200 import _native as N
     from b200 import atlas as A
@@ -319,6 +327,10 @@ def main():
                    "without (i > 5000)": {"steps": K - n_with, "it_per_s": (K - n_with) / (mid.elapsed_time(stop) / 1000.0)},
                    "note": "this rank's device time; the headline value is all K steps"}
     losses_last = trainer.losses.cpu().numpy().copy()
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "losses.npy"), losses_last.astype(np.float32))
+        np.save(os.path.join(args.dump_outputs, "params.npy"), trainer.params.detach().float().cpu().numpy())
     if world > 1:
         tms = torch.tensor([ms], device=dev)
         dist.all_reduce(tms, op=dist.ReduceOp.MAX)
@@ -403,19 +415,12 @@ def main():
                         wgrad_image_bytes(r_map(False, n_f, n_b)) / world / kernels["wgrad"]["ms_without"]) / 1e6
             roof["hbm"] = {"kernel": "tc_wgrad_kernel", "achieved": bw, "peak": hbm_gbs, "unit": "GB/s",
                            "frac": bw / hbm_gbs, "bytes": "algorithmic: both fp16-term images of every dW = dZ^T H operand"}
-        traffic_path = os.path.join(ROOT, "profiles", "r2_ncu_traffic.json")
-        roof["traffic"] = None
-        if os.path.exists(traffic_path) and dom:
-            with open(traffic_path) as f:
-                tr = json.load(f)
-            roof["traffic"] = tr.get(names[dom])           # dram read+write bytes per launch from the committed ncu capture
-            roof["traffic_source"] = "profiles/r2_ncu_traffic.json (ncu --set full, with-global regime)"
         roof.update(kernels=kernels, step_algorithmic_gflop=flop_step / 1e9, step_tflops=flop_step * value / 1e12,
                     step_frac=flop_step * value / 1e12 / peak_tf, rows={"n_f": n_f, "n_b": n_b})
         line = {"metric": "atlas_iters_per_sec", "value": value, "unit": "it/s", "n_gpus": world, "steps": K,
                 "warmup": Wm, "ms_per_step": ms / K, "higher_is_better": True, "scaling": "strong",
                 "vs_baseline": None,
-                "dtype": "fp32" if precision == N.PREC_FP32 else "fp32 (2-term fp16 split on tcgen05, fp32 accumulate)",
+                "dtype": "fp32" if precision == N.PREC_FP32 else "fp32 (2-term fp16 split on wgmma, fp32 accumulate)",
                 "data": "synthetic", "config": dict(ATLAS_CONFIG, parallelism=f"frame-sharded dp{world}" if args.emulate_world < 2
                                                     else f"PROFILING AID: rank 0 of an emulated dp{args.emulate_world} run, no collective",
                                                     precision=prec, cuda_graph=True),

@@ -119,7 +119,8 @@ def _peaks():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         return json.load(open(path)), "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # H100 SXM data sheet (700 W board): 3.35 TB/s HBM3, 989 TFLOP/s dense fp16 / bf16 — never reached, an upper bound
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "data sheet"
 
 
 def _event_ms(fn, iters, warm, world=1, dev=None):
@@ -203,7 +204,7 @@ def seg_line(args, rank, world, local):
     config = {"workload": "stage-1 atlas loop, segmentation variant (two mappings + alpha + atlas), 80 frames 768x432, "
                           "10000 samples/iter, config_flow_100.json coefficients", "frames": T, "height": H, "width": W,
               "samples_batch": B, "regime": "first half of the timed steps with the global rigidity terms, second half without",
-              "l2": "per-step working set (~2 GB of activations) exceeds the 126 MB L2"}
+              "l2": "per-step working set (~2 GB of activations) exceeds the 50 MB L2"}
     metric, unit = "seg_iterations_per_sec", "it/s"
     data = synth.throughput_set(H, W, T, seed=0)
     gm = torch.Generator().manual_seed(2)
@@ -269,7 +270,7 @@ def seg_line(args, rank, world, local):
                     steps, 2)
     out = {"metric": metric, "value": 1000.0 / ms, "unit": unit, "n_gpus": 1, "steps": steps, "warmup": warm,
            "ms_per_step": ms, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
-           "dtype": ("mapping1 + atlas: 2-term fp16 split operands / fp32 accumulate (tcgen05); mapping2 + alpha: fp32 CUDA cores"
+           "dtype": ("mapping1 + atlas: 2-term fp16 split operands / fp32 accumulate (wgmma); mapping2 + alpha: fp32 CUDA cores"
                      if prec == N.PREC_TC else "fp32"), "data": "synthetic", "config": config,
            "e2e": {"value": 1000.0 / ems, "unit": unit, "h2d_bytes_per_step": B * 8, "d2h_bytes_per_step": N.SEG_LOSS_FLOATS * 4},
            "gpu_launches": int(round(n_launch * steps)), "launches_per_step": n_launch,
@@ -392,7 +393,7 @@ def driver_line(args, rank, world, local):
                               "(1080p padded to /32), random-init weights (BASELINE.json configs[4])",
                   "note": "the refinement chain is sequential over frames; with N GPUs each rank filters its own video "
                           "(replicas)", "l2": "per-layer activations (up to 267 MB) exceed L2"}
-        dtype = "fp16 operands / fp32 accumulate (tcgen05), the operand width of the reference's TF32 cuDNN convolutions"
+        dtype = "fp16 operands / fp32 accumulate (wgmma), the operand width of the reference's TF32 cuDNN convolutions"
     if rank == 0:
         print(json.dumps({"metric": metric, "value": value, "unit": unit, "n_gpus": world, "steps": steps, "warmup": warm,
                           "ms_per_step": ms, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,

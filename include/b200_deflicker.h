@@ -1,6 +1,6 @@
 /* b200_deflicker.h — C ABI of libb200deflicker.so
  *
- * B200-native (sm_100a) replacement for the stage-1 neural-atlas hot path of
+ * H100-native (sm_90a) replacement for the stage-1 neural-atlas hot path of
  * ChenyangLEI/All-In-One-Deflicker.  The reference has no FFI layer of its own: its operator
  * boundary for this path is the Python surface listed beside each entry point below (paths
  * relative to the reference root).  The Python mirror of that surface lives in
@@ -19,8 +19,8 @@
  *     descriptor encoder) are not synchronised;
  *   - floating point is fp32 in memory everywhere.  `precision` selects how the 256-wide Linear
  *     layers are contracted: B200_PREC_FP32 = CUDA-core FFMA (bit-for-bit an fp32 GEMM),
- *     B200_PREC_TC = tcgen05 tensor cores on a 2-term fp16 split of both operands (22-bit
- *     significands, fp32 accumulation in TMEM; DESIGN.md §numerics).
+ *     B200_PREC_TC = wgmma tensor cores on a 2-term fp16 split of both operands (22-bit
+ *     significands, fp32 accumulation in registers; DESIGN.md §numerics).
  */
 #ifndef B200_DEFLICKER_H
 #define B200_DEFLICKER_H
@@ -35,7 +35,7 @@ extern "C" {
 #define B200_ERR_INVALID 1      /* bad argument (shape, null pointer, unsupported size)   */
 #define B200_ERR_CUDA 2         /* a CUDA runtime call failed                               */
 #define B200_ERR_WORKSPACE 3    /* workspace too small                                      */
-#define B200_ERR_UNSUPPORTED 4  /* valid request this build cannot serve (e.g. no sm_100a)  */
+#define B200_ERR_UNSUPPORTED 4  /* valid request this build cannot serve (e.g. no sm_90a)   */
 
 #define B200_PREC_FP32 0
 #define B200_PREC_TC 1
@@ -45,7 +45,7 @@ extern "C" {
 
 const char* b200_last_error(void);
 int b200_version(void);
-/* 1 if the current device is compute capability 10.x (tcgen05 path usable), else 0 */
+/* 1 if the current device is compute capability 9.x (wgmma path usable), else 0 */
 int b200_device_supports_tc(void);
 
 /* Diagnostics (no reference counterpart).  b200_launch_count: kernels this library has launched
@@ -375,7 +375,7 @@ int b200_corr_build(const float* fmap1, const float* fmap2, int32_t dim, int32_t
 /* CorrBlock.__call__ (corr.py:33-54): coords [1][2][H8][W8] (x, y) -> out [1][4*(2r+1)^2][H8][W8] */
 /* levels 1..3 from level 0 (2x2 average pooling over the target image, corr.py:22-25); called by both builders */
 int b200_corr_pool_levels(float* pyramid, int32_t H8, int32_t W8, void* stream);
-/* Tensor-core builder: level 0 on tcgen05 with both feature maps split into (hi, lo) fp16 pairs (3 products per
+/* Tensor-core builder: level 0 on wgmma with both feature maps split into (hi, lo) fp16 pairs (3 products per
  * element, fp32 accumulation: fp32-grade like the reference's fp32 matmul), operands fed by TMA; then the pooling.
  * workspace: b200_corr_build_tc_workspace_bytes(dim, H8, W8) bytes. */
 int64_t b200_corr_build_tc_workspace_bytes(int32_t dim, int32_t H8, int32_t W8);
@@ -415,7 +415,7 @@ typedef struct B200ConvDesc {
 } B200ConvDesc;
 int b200_conv2d(const B200ConvDesc* d, const float* x, const float* w, const float* bias,
                 const float* residual, float* y, void* stream);
-/* Tensor-core (tcgen05, fp16 operands / fp32 accumulate) variant of b200_conv2d for the layers the reference
+/* Tensor-core (wgmma, fp16 operands / fp32 accumulate) variant of b200_conv2d for the layers the reference
  * itself runs with 10-bit-mantissa operands (RAFT under fp16 autocast, core/raft.py:131; stage-2 cuDNN
  * convolutions with TF32 allowed).  Weights are first packed into K-major swizzled fp16 images:
  *   bytes = b200_conv_weight_image_bytes(d);  b200_conv_weight_images(d, w, images, stream);
@@ -426,7 +426,7 @@ int b200_conv2d_tc(const B200ConvDesc* d, const float* x, const void* w_images, 
                    const float* residual, float* y, void* stream);
 /* TMA-fed variant (preferred): the input slice is first repacked to fp16 with padding / upsampling / stride
  * phases materialised (workspace of b200_conv_tma_workspace_bytes(d) bytes), then every filter tap is a tiled
- * TMA box load feeding tcgen05.mma directly — no im2col gather.  stride 1 or 2.  Weight images have their own
+ * TMA box load feeding wgmma directly — no im2col gather.  stride 1 or 2.  Weight images have their own
  * layout (tap-major):  b200_conv_tma_weight_image_bytes / b200_conv_tma_weight_images. */
 int64_t b200_conv_tma_workspace_bytes(const B200ConvDesc* d);
 int64_t b200_conv_tma_weight_image_bytes(const B200ConvDesc* d);

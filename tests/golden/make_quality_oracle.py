@@ -8,7 +8,7 @@ texture, exact flows, consistency masks), the reference's whole stage-1 schedule
 `pre_train_mapping` (100 sweeps x 80 frames, unwrap_utils.py:176-198), 10 001 loop trips with 10 000
 samples each, then the render of every frame (evaluate.py:640-708) and PSNR against the input video
 (evaluate.py:740-743).  The index streams come from torch's global CPU generator in the reference's order,
-so the repo's B200 run (tests/perf/quality_vs_oracle.py) consumes the *same* batches.
+so the repo's GPU run (tests/perf/quality_vs_oracle.py) consumes the *same* batches.
 
 What is frozen into tests/golden/quality_oracle.npz: per-frame and mean PSNR, the loss terms every 50 trips,
 the final parameters of both networks (2.7 MB — every rendered frame can be regenerated from them by the oracle

@@ -2,7 +2,7 @@
 
 The oracle ran the reference's WHOLE stage-1 schedule on the CPU (tests/golden/make_quality_oracle.py: quality set
 80 x 432 x 768, pre_train_mapping 100 x 80 steps, 10 001 loop trips, render, PSNR) and its results are frozen in
-tests/golden/quality_oracle.npz.  This script runs the same schedule on the B200 through the product path (tensor-core
+tests/golden/quality_oracle.npz.  This script runs the same schedule on the GPU through the product path (tensor-core
 step, CUDA graphs, tensor-core render) from the same seed — identical initial weights and identical index batches,
 drawn from torch's CPU generator in the reference's order — and reports
 
@@ -10,7 +10,7 @@ drawn from torch's CPU generator in the reference's order — and reports
     the loss curves side by side        (every 50 trips)
     PSNR between the two reconstructions (the oracle's frames are re-rendered from its final parameters)
 
-    python tests/perf/quality_vs_oracle.py [--iters 10001] [--pre-sweeps 100] > profiles/r2_quality_vs_oracle.json
+    python tests/perf/quality_vs_oracle.py [--iters 10001] [--pre-sweeps 100] > quality_vs_oracle.json
 """
 import argparse
 import json

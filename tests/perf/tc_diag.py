@@ -1,4 +1,4 @@
-"""Stage-by-stage check of the tcgen05 path against the oracle / the fp32 path (run on the GPU box)."""
+"""Stage-by-stage check of the wgmma path against the oracle / the fp32 path (run on the GPU box)."""
 import os, sys, json, time
 import numpy as np
 import torch

@@ -238,7 +238,7 @@ def test_five_step_trajectory_with_graph_replay(golden_dir):
             # normalised update differs, so single entries may be off by a fraction of one step;
             # the bulk must agree to fp32 rounding
             d = (v.cpu() - r.detach()).abs()
-            # 5 Adam steps of lr 1e-4.  Measured on B200 (tests/perf/parity_diag.py): max 1.1e-4 (a component
+            # 5 Adam steps of lr 1e-4.  Calibrated with tests/perf/parity_diag.py: max 1.1e-4 (a component
             # whose gradient is summation noise flips the sign of one normalised update), mean <= 7e-7,
             # <= 0.05 % of a tensor's entries beyond 2e-5 (run-to-run variation from the fp32 atomics).  Bounds = measured x 10-40 for
             # mean / median / tail fraction (the theoretical maximum
@@ -406,7 +406,7 @@ def test_eval_maps_match_reference_fixture(golden_dir, precision):
     uv 2e-6; rigidity / flow error 2e-3 relative + small absolute floor (differences of nearby uv values times
     resx / 2: the uv error is amplified by ~L/2 = 20)."""
     if precision == N.PREC_TC and not N.lib().b200_device_supports_tc():
-        pytest.skip("needs sm_100")
+        pytest.skip("needs sm_90")
     z = np.load(os.path.join(golden_dir, "eval_maps.npz"))
     data, _ = _golden_video(golden_dir)
     vid = A.DeviceVideo.from_reference_layout(data, DEV)

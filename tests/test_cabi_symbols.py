@@ -76,7 +76,8 @@ def _conv_desc(n, cin, h, w, cout, kh, kw, stride=1, pad=(0, 0), pad_mode=0, ups
 def test_conv_tma_geometry_host_side():
     """Workspace / weight-image sizes of the TMA convolution are closed-form functions of the descriptor
     (conv_tma.cu tma_geometry): fp16 NHWC repack with channels padded to 64, padding / upsampling / stride-2
-    phases materialised; images = cout tiles x chunks x n_tile rows x 128 B."""
+    phases materialised; images = cout tiles x chunks x n_tile rows x 128 B, n_tile the wgmma N shape (64, 128 or
+    256) that holds a cout tile."""
     lib = N.lib()
     # 3x3, pad 1, 128 -> 128 at 24x40: HP=26, WP=42, Cp=128; chunks = 3*3*2, n_tile = 128
     d = _conv_desc(1, 128, 24, 40, 128, 3, 3, pad=(1, 1))
@@ -86,13 +87,14 @@ def test_conv_tma_geometry_host_side():
     d = _conv_desc(1, 32, 30, 44, 64, 3, 3, stride=2, pad=(1, 1), pad_mode=1)
     assert lib.b200_conv_tma_workspace_bytes(C.byref(d)) == 4 * 16 * 23 * 64 * 2 + 256
     assert lib.b200_conv_tma_weight_image_bytes(C.byref(d)) == 9 * 64 * 128
-    # narrow input, 7x7: x taps folded into the channels (8 per tap): packed width = OW, one chunk per filter row
+    # narrow input, 7x7: x taps folded into the channels (8 per tap): packed width = OW, one chunk per filter row;
+    # 32 output channels occupy an n_tile of 64
     d = _conv_desc(2, 6, 33, 47, 32, 7, 7, pad=(3, 3), pad_mode=1)
     assert lib.b200_conv_tma_workspace_bytes(C.byref(d)) == 2 * 39 * 47 * 64 * 2 + 256
-    assert lib.b200_conv_tma_weight_image_bytes(C.byref(d)) == 7 * 32 * 128
-    # Cout 576 -> 3 cout tiles of 192; x2 nearest upsampling doubles the repacked extent
+    assert lib.b200_conv_tma_weight_image_bytes(C.byref(d)) == 7 * 64 * 128
+    # Cout 576 -> 3 cout tiles of 192 channels, each an n_tile of 256; x2 nearest upsampling doubles the repacked extent
     d = _conv_desc(1, 256, 16, 24, 576, 1, 1)
-    assert lib.b200_conv_tma_weight_image_bytes(C.byref(d)) == 3 * 4 * 192 * 128
+    assert lib.b200_conv_tma_weight_image_bytes(C.byref(d)) == 3 * 4 * 256 * 128
     d = _conv_desc(1, 64, 20, 28, 32, 3, 3, pad=(1, 1), pad_mode=1, upsample=2)
     assert lib.b200_conv_tma_workspace_bytes(C.byref(d)) == 42 * 58 * 64 * 2 + 256
     # invalid descriptors are refused on the host

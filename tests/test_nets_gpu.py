@@ -26,7 +26,7 @@ def test_corr_build_and_lookup(golden_dir):
     got = blk.pyramid.cpu()
     assert got.numel() == flat.numel()
     assert (got - flat).abs().max() <= 1e-4 * flat.abs().max()
-    # both builders (tcgen05 with split fp16 operands = default, fp32 CUDA-core GEMM) to the same fp32-grade bound
+    # both builders (wgmma with split fp16 operands = default, fp32 CUDA-core GEMM) to the same fp32-grade bound
     for impl in ("tc", "simt"):
         alt = K.corr_build(f1.to(DEV), f2.to(DEV), impl=impl).cpu()
         err = ((alt - flat).abs().max() / flat.abs().max()).item()
@@ -93,7 +93,7 @@ def test_full_raft_against_reference_fixture(golden_dir, mixed):
     """Whole RAFT (encoders with instance / folded batch norm, correlation, 3 update iterations, convex
     upsampling) against outputs of the reference model frozen by make_golden_nets.py (reference on CPU = fp32).
     mixed_precision=False: fp32 CUDA-core convolutions, 2e-3 * max|flow|.  mixed_precision=True: the
-    reference's fp16-autocast regime -> tcgen05 convolutions with fp16 operands, 2e-3 * max|flow| as well
+    reference's fp16-autocast regime -> wgmma convolutions with fp16 operands, 2e-3 * max|flow| as well
     (measured 1.5e-4; the reference's own autocast execution is not bit-comparable with its fp32 one either)."""
     import argparse
     from src.models.stage_1.core.raft import RAFT
@@ -112,7 +112,7 @@ def test_full_raft_against_reference_fixture(golden_dir, mixed):
 
 
 # ------------------------------------------------------------------------------------------------
-# tcgen05 convolution (fp16 operands, fp32 accumulation): the operand precision the reference runs these
+# wgmma convolution (fp16 operands, fp32 accumulation): the operand precision the reference runs these
 # layers in (fp16 autocast for RAFT, TF32 cuDNN for stage 2).  Per-layer tolerance 4e-3 * max|y| against an
 # fp64 convolution of the same fp32 inputs (operand rounding 2^-11 each, fp32 accumulation); whole-network
 # tolerances are stated per test.
@@ -184,7 +184,7 @@ def test_conv_tc_slices_residual_and_scale():
 
 
 def test_networks_with_tc_convolutions(golden_dir):
-    """Update block, UNet and TransformNet with every convolution on tcgen05: 2e-2 * max|oracle output|
+    """Update block, UNet and TransformNet with every convolution on wgmma: 2e-2 * max|oracle output|
     (several dozen fp16-operand layers deep; the reference's own fp16/TF32 execution differs from an fp32
     oracle by the same order)."""
     from b200 import nn as K
@@ -227,7 +227,7 @@ def test_networks_with_tc_convolutions(golden_dir):
 
 def test_conv_tc_fused_bilinear_upsample():
     """nn.Upsample(scale_factor=2, mode='bilinear', align_corners=True) + Conv2d (UNet upconv, network_filter.py:22):
-    fused into the fp16 repack on the tcgen05 path, explicit kernel + fp32 convolution otherwise."""
+    fused into the fp16 repack on the wgmma path, explicit kernel + fp32 convolution otherwise."""
     from b200 import nn as K
     import torch.nn.functional as F
     g = torch.Generator().manual_seed(11)
@@ -262,7 +262,7 @@ def test_raft_both_directions_share_the_encoder(golden_dir):
 
 def test_chained_convolutions_equal_unchained():
     """conv -> conv with the intermediate written by the first epilogue straight into the second one's packed fp16 input
-    (b200_conv2d_tma_chain) against the same two tcgen05 convolutions with an fp32 tensor + repack in between: the
+    (b200_conv2d_tma_chain) against the same two wgmma convolutions with an fp32 tensor + repack in between: the
     consumer sees the same fp16 operands, so the results are bit-identical.  Also a two-producer concat (192 + 64
     channels, RAFT motion encoder) and an odd width (ragged last tile)."""
     from b200 import nn as K
@@ -303,7 +303,7 @@ def test_chained_convolutions_equal_unchained():
 
 def test_chained_reflection_padded_convolution():
     """A chained consumer with nn.ReflectionPad2d: the consumer call mirrors the interior of the packed buffer into its
-    halo before the convolution (7x7 / pad 3 and 3x3 / pad 1): bit-identical with the unchained tcgen05 pair."""
+    halo before the convolution (7x7 / pad 3 and 3x3 / pad 1): bit-identical with the unchained wgmma pair."""
     from b200 import nn as K
     g = torch.Generator().manual_seed(32)
     prev = K.set_conv_precision("tc")

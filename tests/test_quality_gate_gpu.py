@@ -1,15 +1,12 @@
 """Quality gate (BASELINE north_star: "output PSNR within 0.1 dB of reference"): the WHOLE stage-1 schedule —
-pre-training, 10 001 loop trips, render of all 80 frames at 768x432 — on the B200 through the product path, against the
+pre-training, 10 001 loop trips, render of all 80 frames at 768x432 — on the GPU through the product path, against the
 oracle's frozen CPU run of the same schedule from the same seed (tests/golden/quality_oracle.npz, produced by
-tests/golden/make_quality_oracle.py).  The run takes ~20 s on a B200.
+tests/golden/make_quality_oracle.py).
 
-Measured (profiles/r2_quality_runs.json).  The oracle itself, run twice on the CPU from the same seed and index stream
-with 4, 8, 6 and 7 threads (only the summation order of its fp32 matrix products differs): 27.273, 27.150, 27.275 and
-27.264 dB, i.e.
-the reference arithmetic reproduces its own PSNR to 0.124 dB (per frame up to 1.47 dB, loss curves 0.9 % median / 9.5 %
-max apart).  Eleven runs of the tensor-core path on the B200: 27.103 ... 27.248 dB, mean 27.188 dB = -0.085 dB against the
-first oracle run, +0.038 dB against the second, -0.052 dB against the mean of the four; one run of the fp32 CUDA-core path:
-27.145 dB.  All of it is the chaotic amplification of fp32 summation order over 10 001 steps, not arithmetic precision.
+The oracle itself, run four times on the CPU from the same seed and index stream with 4, 8, 6 and 7 threads (only the
+summation order of its fp32 matrix products differs), gave 27.273, 27.150, 27.275 and 27.264 dB: the reference
+arithmetic reproduces its own PSNR only to 0.124 dB, the chaotic amplification of fp32 summation order over 10 001
+steps, not arithmetic precision.
 
 Bounds for ONE run: |mean PSNR - mean of the two oracle runs| <= 0.2 dB and within 0.25 dB of the first run; per frame
 within 0.8 dB of the first oracle run where its PSNR is below 36 dB and within 2 dB elsewhere (the two oracle runs differ

@@ -25,7 +25,7 @@ DEV = "cuda"
 
 def test_seg_trip_at_benchmark_size_matches_oracle():
     if not N.lib().b200_device_supports_tc():
-        pytest.skip("needs sm_100")
+        pytest.skip("needs sm_90")
     T, H, W, B = 80, 432, 768, 10000
     data = synth.throughput_set(H, W, T, seed=0)
     masks = (torch.rand(H, W, T, generator=torch.Generator().manual_seed(2)) < 0.4).float()

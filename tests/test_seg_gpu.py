@@ -4,7 +4,7 @@ from the reference's own functions (tests/golden/seg_iteration.npz).  Needs a GP
 Tolerances:
   fp32 path (every network on the CUDA-core kernels): losses rtol 2e-4; parameter gradients |err| <= 1e-3 max|grad|
   per tensor (+ a network-scale floor for near-cancelling bias gradients); network outputs 2e-5.
-  tensor-core path (all four networks on tcgen05, 2-term fp16 split operands): losses rtol 2e-3;
+  tensor-core path (all four networks on wgmma, 2-term fp16 split operands): losses rtol 2e-3;
   gradients 1.5e-2 max|grad| per tensor (the bound of the stand-alone tensor-core IMLP tests).
 """
 import numpy as np

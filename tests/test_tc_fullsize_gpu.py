@@ -40,7 +40,7 @@ KEYS = ("total", "rgb", "gradient", "rigidity", "rigidity_global", "flow")
 
 def _need_tc():
     if not N.lib().b200_device_supports_tc():
-        pytest.skip("no sm_100 device")
+        pytest.skip("no sm_90 device")
 
 
 def _params(golden_dir):

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""A few single convolutions at stage-2 sizes on the tcgen05 path (for ncu captures)."""
+"""A few single convolutions at stage-2 sizes on the wgmma path (for ncu captures)."""
 import os
 import sys
 

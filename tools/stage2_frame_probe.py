@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""A few stage-2 frames (UNet + TransformNet at 1088x1920, tcgen05 convolutions) — for launch lists."""
+"""A few stage-2 frames (UNet + TransformNet at 1088x1920, wgmma convolutions) — for launch lists."""
 import os
 import sys
 import types
