@@ -25,7 +25,6 @@
 // Restates nn.Linear/ReLU/tanh/skip-concat forward+autograd of
 //   src/models/stage_1/implicit_neural_networks.py:62-81 for the two networks of
 //   src/stage1_neural_atlas.py:112-128.
-#include <memory>
 #include <mutex>
 #include <vector>
 
@@ -72,25 +71,33 @@ struct NetImages {
 
 struct TcLayout { NetImages map, atl; };
 
+static char* align_tc(char* base) { return reinterpret_cast<char*>(round_up(reinterpret_cast<int64_t>(base), 1024)); }
 static char* carve_tc(char*& p, int64_t bytes) { char* r = p; p += round_up(bytes, 1024); return r; }
 
-static void plan_net(const MlpShape& s, int64_t rows, bool is_atlas, char*& p, NetImages* n) {
-  const int64_t tiles = rows / TM;
-  n->rows = rows;
+// forward weight images only: all a forward without activation images (the render) needs
+static void plan_fwd_weights(const MlpShape& s, TcNet net, char*& p, NetImages* n) {
+  const bool pe = tc_pe_first(net);
   int64_t off = 0;
   for (int l = 0; l < s.L; ++l) {
     int chunks = 0;
-    const bool tc_layer = is_atlas ? (l <= s.L - 2) : (l >= 1 && l <= s.L - 2);
-    if (tc_layer) chunks = (l == 0 ? 0 : HID / 64) + ((l == 0 || s.skip[l]) && is_atlas ? 1 : 0);
+    const bool tc_layer = pe ? (l <= s.L - 2) : (l >= 1 && l <= s.L - 2);
+    if (tc_layer) chunks = (l == 0 ? 0 : HID / 64) + ((l == 0 || s.skip[l]) && pe ? 1 : 0);
     n->n_chunks_fwd[l] = chunks;
     n->w_fwd_layer[l] = off;
     off += (int64_t)chunks * 2 * STAGE_BYTES;
   }
   n->w_fwd = carve_tc(p, off);
-  off = 0;
+}
+
+static void plan_net(const MlpShape& s, int64_t rows, TcNet net, char*& p, NetImages* n) {
+  const int64_t tiles = rows / TM;
+  const bool pe = tc_pe_first(net);
+  n->rows = rows;
+  plan_fwd_weights(s, net, p, n);
+  int64_t off = 0;
   for (int l = 0; l < s.L; ++l) {
     n->w_bwd_layer[l] = off;
-    const bool used = l <= s.L - 2 && (is_atlas || l >= 1);
+    const bool used = l <= s.L - 2 && (pe || l >= 1);
     if (used) off += (int64_t)(HID / 64) * 2 * STAGE_BYTES;
   }
   n->w_bwd = carve_tc(p, off);
@@ -99,26 +106,26 @@ static void plan_net(const MlpShape& s, int64_t rows, bool is_atlas, char*& p, N
   n->act = carve_tc(p, (int64_t)(s.L - 1) * n->slot_stride);
   n->dz = carve_tc(p, (int64_t)(s.L - 1) * n->slot_stride);
   n->w64_term_stride = tiles * ATOM_BYTES;
-  n->pe = is_atlas ? carve_tc(p, 2 * n->w64_term_stride) : nullptr;
+  n->pe = pe ? carve_tc(p, 2 * n->w64_term_stride) : nullptr;
   n->dzl = carve_tc(p, 2 * n->w64_term_stride);
   n->bits = reinterpret_cast<uint32_t*>(carve_tc(p, (int64_t)(s.L - 1) * rows * 32));
 }
 
 int64_t tc_plan(const MlpShape& ms, const MlpShape& as, int64_t rows_map, int64_t rows_atlas, char* base,
                 TcPlan* out) {
-  char* p = reinterpret_cast<char*>(round_up(reinterpret_cast<int64_t>(base), 1024));
+  char* p = align_tc(base);
   TcLayout lay{};
-  plan_net(ms, rows_map, false, p, &lay.map);
-  plan_net(as, rows_atlas, true, p, &lay.atl);
+  plan_net(ms, rows_map, TcNet::Mapping6, p, &lay.map);
+  plan_net(as, rows_atlas, TcNet::Atlas, p, &lay.atl);
   if (out) { out->base = base; out->bytes = p - base; out->rows_map = rows_map; out->rows_atlas = rows_atlas; }
   return p - base;
 }
 
 static TcLayout layout_of(const TcStep& s) {
-  char* p = reinterpret_cast<char*>(round_up(reinterpret_cast<int64_t>(s.plan->base), 1024));
+  char* p = align_tc(s.plan->base);
   TcLayout lay{};
-  plan_net(*s.ms, s.plan->rows_map, false, p, &lay.map);
-  plan_net(*s.as, s.plan->rows_atlas, true, p, &lay.atl);
+  plan_net(*s.ms, s.plan->rows_map, TcNet::Mapping6, p, &lay.map);
+  plan_net(*s.as, s.plan->rows_atlas, TcNet::Atlas, p, &lay.atl);
   return lay;
 }
 
@@ -1048,6 +1055,29 @@ static int sm_count() {
   return g_sm_count;
 }
 
+TcNet tc_net_of(const MlpShape& s) {
+  if (s.hidden != HID) return TcNet::None;
+  bool skips_4_7 = true, no_skips = true;
+  for (int l = 1; l < s.L; ++l) {
+    skips_4_7 = skips_4_7 && s.skip[l] == (l == 4 || l == 7);
+    no_skips = no_skips && !s.skip[l];
+  }
+  if (s.L == 6 && s.pe == 0 && s.in_dim == 3 && s.out_dim == 2 && no_skips) return TcNet::Mapping6;
+  if (s.L == 4 && s.pe == 0 && s.in_dim == 3 && s.out_dim == 2 && no_skips) return TcNet::Mapping4;
+  if (s.L == 8 && s.pe == 10 && s.in_dim == 2 && s.out_dim == 3 && skips_4_7) return TcNet::Atlas;
+  if (s.L == 8 && s.pe == 5 && s.in_dim == 3 && s.out_dim == 1 && no_skips) return TcNet::Alpha;
+  return TcNet::None;
+}
+
+// The kernel instantiations of each network, indexed by TcNet - 1.
+struct NetKernels { void (*fwd)(FwdParams); void (*bwd)(BwdParams); int fwd_smem, bwd_smem; };
+static const NetKernels g_kernels[] = {
+    {tc_fwd_kernel<false, 6>, tc_bwd_kernel<false, 6>, KCfg<false, false>::SMEM, KCfg<false, true>::SMEM},
+    {tc_fwd_kernel<false, 4>, tc_bwd_kernel<false, 4>, KCfg<false, false>::SMEM, KCfg<false, true>::SMEM},
+    {tc_fwd_kernel<true, 8, 0>, tc_bwd_kernel<true, 8, 0>, KCfg<true, false>::SMEM, KCfg<true, true>::SMEM},
+    {tc_fwd_kernel<true, 8, 1>, tc_bwd_kernel<true, 8, 1>, KCfg<true, false>::SMEM, KCfg<true, true>::SMEM},
+};
+
 static int ensure_attrs() {
   // cudaFuncSetAttribute is per device: remember which devices of this process have been configured
   static bool done_dev[64] = {};
@@ -1056,79 +1086,76 @@ static int ensure_attrs() {
   B200_REQUIRE(dev >= 0 && dev < 64, "device ordinal %d out of range", dev);
   bool& done = done_dev[dev];
   if (done) return B200_OK;
-  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<false, false>::SMEM));
-  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<true, false>::SMEM));
-  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<false, true>::SMEM));
-  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<true, true>::SMEM));
-  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_fwd_kernel<false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<false, false>::SMEM));
-  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_bwd_kernel<false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<false, true>::SMEM));
-  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_fwd_kernel<true, 8, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<true, false>::SMEM));
-  B200_CHECK_CUDA(cudaFuncSetAttribute(tc_bwd_kernel<true, 8, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, KCfg<true, true>::SMEM));
+  for (const NetKernels& k : g_kernels) {
+    B200_CHECK_CUDA(cudaFuncSetAttribute(k.fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, k.fwd_smem));
+    B200_CHECK_CUDA(cudaFuncSetAttribute(k.bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, k.bwd_smem));
+  }
   B200_CHECK_CUDA(cudaFuncSetAttribute(tc_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM));
   done = true;
   return B200_OK;
 }
 
-// Job / item tables depend only on pointers and geometry: built by one eager call per (workspace, row
-// geometry, parameter buffers), kept in device memory, reused inside captured graphs.
-struct HostTables {
-  int key_dev = -1;
-  const void* key_base = nullptr; int key_cap = 0, key_groups = 0; const void* key_params = nullptr;
-  const void* key_grads = nullptr; bool key_atlas = false; int key_flow = 0;
-  PrepJobs* d_prep = nullptr; WgradItems* d_wg = nullptr;
-  int n_wg = 0, n_prep = 0;
-};
-// Captured graphs bake a slot's device pointers in, so a slot is NEVER recycled: the list only grows (each entry
-// is ~50 KB of device memory; one entry per (device, workspace, row geometry, parameter buffers)).
-constexpr int MAX_TABLES = 4096;
-static std::vector<HostTables*> g_tabs;
-static std::mutex g_tabs_mutex;
-
-static int current_device() { int d = 0; cudaGetDevice(&d); return d; }
-
-static HostTables* find_tables(const TcStep& s) {
-  const bool atlas = s.y_atlas != nullptr;
-  const int dev = current_device();
-  std::lock_guard<std::mutex> lock(g_tabs_mutex);
-  for (size_t i = 0; i < g_tabs.size(); ++i) {
-    HostTables& t = *g_tabs[i];
-    if (t.key_dev == dev && t.key_base == s.plan->base && t.key_cap == s.cap && t.key_groups == s.n_groups && t.key_params == s.params &&
-        t.key_grads == s.grads && t.key_atlas == atlas && t.key_flow == s.flow_groups)
-      return &t;
-  }
-  return nullptr;
+static int launch_fwd(TcNet net, const FwdParams& P, int tiles, cudaStream_t st) {
+  const NetKernels& k = g_kernels[(int)net - 1];
+  k.fwd<<<min(sm_count(), tiles), TC_THREADS, k.fwd_smem, st>>>(P);
+  B200_CHECK_LAUNCH();
+  return B200_OK;
 }
 
+static int launch_bwd(TcNet net, const BwdParams& P, int tiles, cudaStream_t st) {
+  const NetKernels& k = g_kernels[(int)net - 1];
+  k.bwd<<<min(sm_count(), tiles), TC_THREADS, k.bwd_smem, st>>>(P);
+  B200_CHECK_LAUNCH();
+  return B200_OK;
+}
+
+// Parameter blocks as the fused step uses them; other callers override the fields that differ.
+static FwdParams fill_fwd(const MlpShape& sh, const NetImages& im, const float* x, float* y, const float* params, int cap,
+                          int groups, const int* n_valid) {
+  FwdParams P{};
+  P.x = x; P.y = y; P.params = params; P.img = im; P.cap = cap; P.n_groups = groups; P.n_valid = n_valid;
+  P.in_scale = 0.5f; P.in_shift = 0.5f; P.store_images = 1; P.tanh_out = 1; P.flow_groups = 0;
+  for (int l = 0; l < sh.L; ++l) { P.w_off[l] = sh.w_off[l]; P.b_off[l] = sh.b_off[l]; }
+  return P;
+}
+
+static BwdParams fill_bwd(const MlpShape& sh, const NetImages& im, const float* dy, const float* y, const float* x,
+                          float* d_in, const float* params, float* grads, int cap, int groups, const int* n_valid,
+                          int* gmax_bits) {
+  BwdParams P{};
+  P.dy = dy; P.y = y; P.x = x; P.d_in = d_in; P.params = params; P.grads = grads; P.img = im;
+  P.cap = cap; P.n_groups = groups; P.n_valid = n_valid; P.gmax_bits = gmax_bits;
+  P.in_scale = 0.5f; P.d_in_accumulate = 1; P.tanh_out = 1; P.flow_groups = 0;
+  for (int l = 0; l < sh.L; ++l) { P.w_off[l] = sh.w_off[l]; P.b_off[l] = sh.b_off[l]; }
+  return P;
+}
+
+// ---- job tables: PrepJobs for tc_prep_kernel, WgradItems for tc_wgrad_kernel
 static void add_prep(PrepJobs& pj, const float* W, int ldw, int n_rows, int k0, int k_cnt, int transpose, char* dst) {
   PrepJob& j = pj.j[pj.n++];
   j.W = W; j.ldw = ldw; j.n_rows = n_rows; j.k0 = k0; j.k_cnt = k_cnt; j.transpose = transpose;
   j.hi = dst; j.lo = dst + STAGE_BYTES;
 }
 
-
-// ---- table builders shared by the cached (training loop) and the ephemeral (stand-alone IMLP) paths
-// the atlas network back-propagates to its input (uv) through the positional encoding; the alpha network's inputs
-// are pixel coordinates
-static bool net_has_dpe(const MlpShape& sh, bool is_atlas) { return is_atlas && sh.in_dim == 2; }
-
-static void prep_jobs_for_net(PrepJobs& pj, const MlpShape& sh, const NetImages& im, const float* pp, bool is_atlas,
+static void prep_jobs_for_net(PrepJobs& pj, const MlpShape& sh, const NetImages& im, const float* pp, TcNet net,
                               bool with_bwd) {
+  const bool pe = tc_pe_first(net);
   for (int l = 0; l < sh.L; ++l) {
     char* dst = im.w_fwd + im.w_fwd_layer[l];
     if (im.n_chunks_fwd[l] == 0) continue;
     const float* W = pp + sh.w_off[l];
     int item = 0;
     if (l > 0) for (int kc = 0; kc < 4; ++kc) add_prep(pj, W, sh.K[l], 256, kc * 64, 64, 0, dst + (int64_t)(item++) * 2 * STAGE_BYTES);
-    if (is_atlas && (l == 0 || sh.skip[l]))
+    if (pe && (l == 0 || sh.skip[l]))
       add_prep(pj, W, sh.K[l], 256, l == 0 ? 0 : 256, sh.enc, 0, dst + (int64_t)(item++) * 2 * STAGE_BYTES);
   }
   if (!with_bwd) return;
   for (int l = 0; l < sh.L - 1; ++l) {
-    if (l < 1 && !net_has_dpe(sh, is_atlas)) continue;
+    if (l < 1 && !tc_net_has_dpe(net)) continue;
     char* dst = im.w_bwd + im.w_bwd_layer[l];
     const float* W = pp + sh.w_off[l];
     // image rows = input index k of layer l (256, or 40 for atlas layer 0), chunk over the output index n
-    const int rows = (is_atlas && l == 0) ? sh.enc : 256;
+    const int rows = (pe && l == 0) ? sh.enc : 256;
     for (int kc = 0; kc < 4; ++kc) add_prep(pj, W, sh.K[l], rows, kc * 64, 64, 1, dst + (int64_t)kc * 2 * STAGE_BYTES);
   }
 }
@@ -1145,19 +1172,20 @@ static double step_cost(int a_cols, int b_cols) {
 struct WgProto { const char* a; int64_t a_term; int a_cols; const char* b; int64_t b_term; int b_cols;
                  float* out; int ld; int n_rows, n_cols, groups; double bytes; int mapping; };
 
-static void protos_for_net(WgProto* protos, int& np, const MlpShape& sh, const NetImages& im, float* g, bool is_atlas,
+static void protos_for_net(WgProto* protos, int& np, const MlpShape& sh, const NetImages& im, float* g, TcNet net,
                            int groups) {
+  const bool pe = tc_pe_first(net);
   auto add = [&](const char* a, int64_t a_term, int a_cols, const char* b, int64_t b_term, int b_cols, float* out, int ld,
                  int n_rows, int n_cols) {
     protos[np++] = WgProto{a, a_term, a_cols, b, b_term, b_cols, out, ld, n_rows, n_cols, groups,
-                           (double)groups * step_cost(a_cols, b_cols), is_atlas ? 0 : 1};
+                           (double)groups * step_cost(a_cols, b_cols), pe ? 0 : 1};
   };
   for (int l = 1; l <= sh.L - 2; ++l)
     add(im.dz + (int64_t)l * im.slot_stride, im.term_stride, 256, im.act + (int64_t)(l - 1) * im.slot_stride,
         im.term_stride, 256, g + sh.w_off[l], sh.K[l], 256, 256);
   add(im.dzl, im.w64_term_stride, 64, im.act + (int64_t)(sh.L - 2) * im.slot_stride, im.term_stride, 256,
       g + sh.w_off[sh.L - 1], sh.K[sh.L - 1], sh.out_dim, 256);
-  if (is_atlas) {
+  if (pe) {
     // positional-encoding parts: layer 0 and the skip layers; output layer's skip part
     add(im.dz, im.term_stride, 256, im.pe, im.w64_term_stride, 64, g + sh.w_off[0], sh.K[0], 256, sh.enc);
     for (int l = 1; l <= sh.L - 2; ++l)
@@ -1210,57 +1238,62 @@ static void apportion_items(WgradItems& wi, const WgProto* protos, int np, int c
   }
 }
 
-static int build_tables(const TcStep& s, const TcLayout& lay, cudaStream_t st, HostTables** out) {
-  if (HostTables* t = find_tables(s)) { *out = t; return B200_OK; }
+// The tables depend only on pointers and geometry.  Callers that keep their workspace and parameter / gradient buffers
+// across calls (the fused step; stand-alone calls on a persistent workspace, such as the segmentation step) take them
+// from a process-wide cache: built by one eager call, kept in their own device allocations, reused inside captured
+// graphs.  The render and ephemeral stand-alone calls (the IMLP class: a fresh workspace per call) upload them into
+// their workspace on every call, so a recycled workspace is harmless and the cache does not grow with every call.
+struct TabKey {
+  int dev; const void* ws; TcNet net;   // fused step: net = Atlas (mapping + atlas) or Mapping6 (pre-training)
+  bool step, with_bwd; int cap, groups, flow;
+  const void* params; const void* grads;   // grads null: a stand-alone forward, served by the entry of its backward
+};
+struct TcTables { TabKey key; PrepJobs* d_prep = nullptr; int n_prep = -1; WgradItems* d_wg = nullptr; int n_wg = -1; };
+// Captured graphs bake an entry's device pointers in, so an entry is NEVER recycled: the list only grows (each entry
+// is ~75 KB of device memory; one entry per (device, workspace, row geometry, parameter buffers)).
+constexpr int MAX_TABLES = 4096;
+static std::vector<TcTables*> g_tabs;
+static std::mutex g_tabs_mutex;
+static thread_local PrepJobs g_pj;        // host side of the table being built
+static thread_local WgradItems g_wi;
+
+static int current_device() { int d = 0; cudaGetDevice(&d); return d; }
+
+// The entry of `k`, or null.  `add`: a missing entry is added with no tables yet.  An entry without gradient buffer
+// (made by a stand-alone forward) adopts the first one a backward brings.
+static TcTables* find_tables(const TabKey& k, bool add) {
+  std::lock_guard<std::mutex> lock(g_tabs_mutex);
+  for (TcTables* t : g_tabs) {
+    TabKey& e = t->key;
+    if (e.dev == k.dev && e.ws == k.ws && e.net == k.net && e.step == k.step && e.with_bwd == k.with_bwd &&
+        e.cap == k.cap && e.groups == k.groups && e.flow == k.flow && e.params == k.params &&
+        (!k.grads || !e.grads || e.grads == k.grads)) {
+      if (!e.grads) e.grads = k.grads;
+      return t;
+    }
+  }
+  if (!add || (int)g_tabs.size() >= MAX_TABLES) return nullptr;
+  g_tabs.push_back(new TcTables{k});
+  return g_tabs.back();
+}
+
+// Copies a host table to *dst: a new allocation of a cache entry (`own`) or a slot of the caller's workspace.  Either
+// way it is a pageable copy made outside graph capture.  A cached table is read later from any stream, so the upload
+// completes before the call returns.
+template <class T> static int upload(const T& host, T** dst, bool own, cudaStream_t st) {
   cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
   cudaStreamIsCapturing(st, &cs);
-  if (cs == cudaStreamCaptureStatusActive) {
-    set_error("tensor-core tables must be built by one eager call before graph capture");
-    return B200_ERR_INVALID;
-  }
-  B200_REQUIRE(s.as->L == 8 && s.ms->L == 6 && s.as->skip[4] && s.as->skip[7] && s.as->pe == 10 && s.ms->pe == 0 &&
-               s.as->hidden == HID && s.ms->hidden == HID, "tensor-core path is specialised to the two stage-1 networks");
-  {
-    std::lock_guard<std::mutex> lock(g_tabs_mutex);
-    B200_REQUIRE((int)g_tabs.size() < MAX_TABLES, "too many distinct tensor-core workspaces in one process (%d)",
-                 MAX_TABLES);
-  }
-  std::unique_ptr<HostTables> tab_owner(new HostTables());
-  HostTables& tab = *tab_owner;
-  B200_CHECK_CUDA(cudaMalloc(&tab.d_prep, sizeof(PrepJobs)));
-  B200_CHECK_CUDA(cudaMalloc(&tab.d_wg, sizeof(WgradItems)));
-  std::unique_ptr<PrepJobs> pj_owner(new PrepJobs()); std::unique_ptr<WgradItems> wi_owner(new WgradItems());
-  PrepJobs& pj = *pj_owner; WgradItems& wi = *wi_owner;
-  pj.n = 0; wi.n = 0;
-  const bool atlas = s.y_atlas != nullptr;
-  // ---- forward / dgrad weight images (the atlas network only where it is evaluated: not in pre-training)
-  prep_jobs_for_net(pj, *s.ms, lay.map, s.params, false, true);
-  if (atlas) prep_jobs_for_net(pj, *s.as, lay.atl, s.params + s.ms->total, true, true);
-  // ---- wgrad items
-  WgProto protos[32]; int np = 0;
-  protos_for_net(protos, np, *s.ms, lay.map, s.grads, false, s.n_groups);
-  if (atlas) protos_for_net(protos, np, *s.as, lay.atl, s.grads + s.ms->total, true, 3);
-  apportion_items(wi, protos, np, s.cap, s.flow_groups);
-  if (pj.n > MAX_PREP_JOBS) { set_error("table overflow"); return B200_ERR_INVALID; }
-  B200_CHECK_CUDA(cudaMemcpyAsync(tab.d_prep, &pj, sizeof(PrepJobs), cudaMemcpyHostToDevice, st));
-  B200_CHECK_CUDA(cudaMemcpyAsync(tab.d_wg, &wi, sizeof(WgradItems), cudaMemcpyHostToDevice, st));
-  B200_CHECK_CUDA(cudaStreamSynchronize(st));
-  tab.n_wg = wi.n; tab.n_prep = pj.n;
-  tab.key_base = s.plan->base; tab.key_cap = s.cap; tab.key_groups = s.n_groups; tab.key_params = s.params;
-  tab.key_grads = s.grads; tab.key_atlas = atlas; tab.key_dev = current_device(); tab.key_flow = s.flow_groups;
-  {
-    std::lock_guard<std::mutex> lock(g_tabs_mutex);
-    g_tabs.push_back(tab_owner.release());
-    *out = g_tabs.back();
-  }
+  B200_REQUIRE(cs != cudaStreamCaptureStatusActive, "tensor-core job tables are uploaded by an eager call: run the same "
+               "call once outside graph capture first (persistent workspaces only; the render is not capturable)");
+  if (own) B200_CHECK_CUDA(cudaMalloc(dst, sizeof(T)));
+  B200_CHECK_CUDA(cudaMemcpyAsync(*dst, &host, sizeof(T), cudaMemcpyHostToDevice, st));
+  if (own) B200_CHECK_CUDA(cudaStreamSynchronize(st));
   return B200_OK;
 }
 
-static void fill_fwd(FwdParams& P, const MlpShape& sh, const NetImages& im, const float* x, float* y,
-                     const float* params, int cap, int groups, const int* n_valid) {
-  P.x = x; P.y = y; P.params = params; P.img = im; P.cap = cap; P.n_groups = groups; P.n_valid = n_valid;
-  P.in_scale = 0.5f; P.in_shift = 0.5f; P.store_images = 1; P.tanh_out = 1; P.flow_groups = 0;
-  for (int l = 0; l < sh.L; ++l) { P.w_off[l] = sh.w_off[l]; P.b_off[l] = sh.b_off[l]; }
+static TabKey step_key(const TcStep& s) {
+  return TabKey{current_device(), s.plan->base, s.y_atlas ? TcNet::Atlas : TcNet::Mapping6, true, true, s.cap, s.n_groups,
+                s.flow_groups, s.params, s.grads};
 }
 
 // The weight images depend only on the parameters, so their preparation runs on a side stream, forked from the
@@ -1271,9 +1304,28 @@ static SideStream g_side[64];
 
 int tc_begin_step(const TcStep& s, cudaStream_t st) {
   B200_PROPAGATE(ensure_attrs());
-  const TcLayout lay = layout_of(s);
-  HostTables* tab = nullptr;
-  B200_PROPAGATE(build_tables(s, lay, st, &tab));
+  TcTables* tab = find_tables(step_key(s), true);
+  B200_REQUIRE(tab, "too many distinct tensor-core workspaces in one process (%d)", MAX_TABLES);
+  if (tab->n_wg < 0) {
+    B200_REQUIRE(tc_net_of(*s.ms) == TcNet::Mapping6 && tc_net_of(*s.as) == TcNet::Atlas,
+                 "tensor-core path is specialised to the two stage-1 networks");
+    const TcLayout lay = layout_of(s);
+    const bool atlas = s.y_atlas != nullptr;
+    // ---- forward / dgrad weight images (the atlas network only where it is evaluated: not in pre-training)
+    g_pj.n = 0;
+    prep_jobs_for_net(g_pj, *s.ms, lay.map, s.params, TcNet::Mapping6, true);
+    if (atlas) prep_jobs_for_net(g_pj, *s.as, lay.atl, s.params + s.ms->total, TcNet::Atlas, true);
+    if (g_pj.n > MAX_PREP_JOBS) { set_error("table overflow"); return B200_ERR_INVALID; }
+    // ---- wgrad items
+    WgProto protos[32]; int np = 0;
+    protos_for_net(protos, np, *s.ms, lay.map, s.grads, TcNet::Mapping6, s.n_groups);
+    if (atlas) protos_for_net(protos, np, *s.as, lay.atl, s.grads + s.ms->total, TcNet::Atlas, 3);
+    g_wi.n = 0;
+    apportion_items(g_wi, protos, np, s.cap, s.flow_groups);
+    B200_PROPAGATE(upload(g_pj, &tab->d_prep, true, st));
+    B200_PROPAGATE(upload(g_wi, &tab->d_wg, true, st));
+    tab->n_prep = g_pj.n; tab->n_wg = g_wi.n;
+  }
   SideStream& sd = g_side[current_device()];
   if (!sd.stream) {
     B200_CHECK_CUDA(cudaStreamCreateWithFlags(&sd.stream, cudaStreamNonBlocking));
@@ -1290,27 +1342,22 @@ int tc_begin_step(const TcStep& s, cudaStream_t st) {
   return B200_OK;
 }
 
-static int run_forward(const TcStep& s, bool with_atlas, cudaStream_t st) {
+int tc_step_forward(const TcStep& s, cudaStream_t st) {
   const TcLayout lay = layout_of(s);
   SideStream& sd = g_side[current_device()];
   if (!sd.pending) B200_PROPAGATE(tc_begin_step(s, st));     // callers that did not fork earlier
   B200_CHECK_CUDA(cudaStreamWaitEvent(st, sd.join, 0));
   sd.pending = false;
-  const int tiles_map = s.n_groups * (s.cap / TM);
-  FwdParams pm{};
-  fill_fwd(pm, *s.ms, lay.map, s.x_map, s.uv, s.params, s.cap, s.n_groups, s.counters);
+  FwdParams pm = fill_fwd(*s.ms, lay.map, s.x_map, s.uv, s.params, s.cap, s.n_groups, s.counters);
   pm.flow_groups = s.flow_groups;
   timer_begin(TAG_MAP_FWD, st);
-  tc_fwd_kernel<false><<<min(sm_count(), tiles_map), TC_THREADS, KCfg<false, false>::SMEM, st>>>(pm);
+  B200_PROPAGATE(launch_fwd(TcNet::Mapping6, pm, s.n_groups * (s.cap / TM), st));
   timer_end(TAG_MAP_FWD, st);
-  B200_CHECK_LAUNCH();
-  if (with_atlas) {
-    FwdParams pa{};
-    fill_fwd(pa, *s.as, lay.atl, s.uv, s.y_atlas, s.params + s.ms->total, s.cap, 3, s.counters);
+  if (s.y_atlas) {
+    const FwdParams pa = fill_fwd(*s.as, lay.atl, s.uv, s.y_atlas, s.params + s.ms->total, s.cap, 3, s.counters);
     timer_begin(TAG_ATLAS_FWD, st);
-    tc_fwd_kernel<true><<<min(sm_count(), 3 * (s.cap / TM)), TC_THREADS, KCfg<true, false>::SMEM, st>>>(pa);
+    B200_PROPAGATE(launch_fwd(TcNet::Atlas, pa, 3 * (s.cap / TM), st));
     timer_end(TAG_ATLAS_FWD, st);
-    B200_CHECK_LAUNCH();
   }
   return B200_OK;
 }
@@ -1331,34 +1378,24 @@ int tc_debug_wgrad(long long* cycles, int* shapes, int max_ctas) {
   return n;
 }
 
-static int run_backward(const TcStep& s, bool with_atlas, cudaStream_t st) {
+int tc_step_backward(const TcStep& s, cudaStream_t st) {
   const TcLayout lay = layout_of(s);
-  HostTables* tab = find_tables(s);
-  if (!tab) { set_error("tensor-core backward called before forward"); return B200_ERR_INVALID; }
+  const TcTables* tab = find_tables(step_key(s), false);
+  B200_REQUIRE(tab && tab->n_wg >= 0, "tensor-core backward called before forward");
   int* gmax = const_cast<int*>(s.counters) + 3;
-  auto fill = [&](BwdParams& P, const MlpShape& sh, const NetImages& im, const float* dy, const float* y,
-                  const float* x, float* d_in, const float* params, float* grads, int groups) {
-    P.dy = dy; P.y = y; P.x = x; P.d_in = d_in; P.params = params; P.grads = grads; P.img = im;
-    P.cap = s.cap; P.n_groups = groups; P.n_valid = s.counters; P.gmax_bits = gmax;
-    P.in_scale = 0.5f; P.d_in_accumulate = 1; P.tanh_out = 1; P.flow_groups = 0;
-    for (int l = 0; l < sh.L; ++l) { P.w_off[l] = sh.w_off[l]; P.b_off[l] = sh.b_off[l]; }
-  };
-  if (with_atlas) {
-    BwdParams pa{};
-    fill(pa, *s.as, lay.atl, s.d_y, s.y_atlas, nullptr, const_cast<float*>(s.d_uv), s.params + s.ms->total,
-         s.grads + s.ms->total, 3);
+  if (s.y_atlas) {
+    const BwdParams pa = fill_bwd(*s.as, lay.atl, s.d_y, s.y_atlas, nullptr, const_cast<float*>(s.d_uv),
+                                  s.params + s.ms->total, s.grads + s.ms->total, s.cap, 3, s.counters, gmax);
     timer_begin(TAG_ATLAS_BWD, st);
-    tc_bwd_kernel<true><<<min(sm_count(), 3 * (s.cap / TM)), TC_THREADS, KCfg<true, true>::SMEM, st>>>(pa);
+    B200_PROPAGATE(launch_bwd(TcNet::Atlas, pa, 3 * (s.cap / TM), st));
     timer_end(TAG_ATLAS_BWD, st);
-    B200_CHECK_LAUNCH();
   }
-  BwdParams pm{};
-  fill(pm, *s.ms, lay.map, s.d_uv, s.uv, s.x_map, nullptr, s.params, s.grads, s.n_groups);
+  BwdParams pm = fill_bwd(*s.ms, lay.map, s.d_uv, s.uv, s.x_map, nullptr, s.params, s.grads, s.cap, s.n_groups,
+                          s.counters, gmax);
   pm.flow_groups = s.flow_groups;
   timer_begin(TAG_MAP_BWD, st);
-  tc_bwd_kernel<false><<<min(sm_count(), s.n_groups * (s.cap / TM)), TC_THREADS, KCfg<false, true>::SMEM, st>>>(pm);
+  B200_PROPAGATE(launch_bwd(TcNet::Mapping6, pm, s.n_groups * (s.cap / TM), st));
   timer_end(TAG_MAP_BWD, st);
-  B200_CHECK_LAUNCH();
   timer_begin(TAG_WGRAD, st);
   g_last_wg = tab->d_wg; g_last_wg_n = min(tab->n_wg, sm_count());
   tc_wgrad_kernel<<<min(tab->n_wg, sm_count()), WG_THREADS, WG_SMEM, st>>>(tab->d_wg, s.counters, gmax);
@@ -1373,234 +1410,129 @@ static int run_backward(const TcStep& s, bool with_atlas, cudaStream_t st) {
 // evaluate.py:640-708).  Workspace: [PrepJobs table][forward weight images of both networks].
 // ---------------------------------------------------------------------------------------------
 
-static void plan_infer(const MlpShape& ms, const MlpShape& as, char* base, NetImages* im_map, NetImages* im_atl,
-                       PrepJobs** d_prep, int64_t* bytes) {
-  char* p = reinterpret_cast<char*>(round_up(reinterpret_cast<int64_t>(base), 1024));
+static int64_t plan_infer(const MlpShape& ms, const MlpShape& as, char* base, NetImages* im_map, NetImages* im_atl,
+                          PrepJobs** d_prep) {
+  char* p = align_tc(base);
   *d_prep = reinterpret_cast<PrepJobs*>(carve_tc(p, sizeof(PrepJobs)));
-  for (int net = 0; net < 2; ++net) {
-    const MlpShape& s = net ? as : ms;
-    NetImages* n = net ? im_atl : im_map;
-    *n = NetImages{};
-    int64_t off = 0;
-    for (int l = 0; l < s.L; ++l) {
-      int chunks = 0;
-      const bool tc_layer = net ? (l <= s.L - 2) : (l >= 1 && l <= s.L - 2);
-      if (tc_layer) chunks = (l == 0 ? 0 : HID / 64) + ((l == 0 || s.skip[l]) && net ? 1 : 0);
-      n->n_chunks_fwd[l] = chunks;
-      n->w_fwd_layer[l] = off;
-      off += (int64_t)chunks * 2 * STAGE_BYTES;
-    }
-    n->w_fwd = carve_tc(p, off);
-  }
-  *bytes = p - base;
+  *im_map = NetImages{}; *im_atl = NetImages{};
+  plan_fwd_weights(ms, TcNet::Mapping6, p, im_map);
+  plan_fwd_weights(as, TcNet::Atlas, p, im_atl);
+  return p - base;
 }
 
 int64_t tc_infer_workspace_bytes(const MlpShape& ms, const MlpShape& as) {
-  NetImages a, b; PrepJobs* d; int64_t bytes = 0;
-  plan_infer(ms, as, nullptr, &a, &b, &d, &bytes);
-  return bytes + 2048;
+  NetImages a, b; PrepJobs* d;
+  return plan_infer(ms, as, nullptr, &a, &b, &d) + 2048;
 }
 
 int tc_infer_forward(const MlpShape& ms, const MlpShape& as, const float* params, const float* x_map, float* uv,
                      float* y, int64_t rows, char* ws, cudaStream_t st) {
   B200_PROPAGATE(ensure_attrs());
-  B200_REQUIRE(as.L == 8 && ms.L == 6 && as.skip[4] && as.skip[7] && as.pe == 10 && ms.pe == 0 && as.hidden == HID &&
-               ms.hidden == HID, "tensor-core path is specialised to the two stage-1 networks");
+  B200_REQUIRE(tc_net_of(ms) == TcNet::Mapping6 && tc_net_of(as) == TcNet::Atlas,
+               "tensor-core path is specialised to the two stage-1 networks");
   B200_REQUIRE(rows > 0 && rows % TM == 0 && rows / TM < (1 << 24), "rows must be a positive multiple of %d", TM);
-  NetImages im_map, im_atl; PrepJobs* d_prep; int64_t bytes;
-  plan_infer(ms, as, ws, &im_map, &im_atl, &d_prep, &bytes);
-  // The job table lives in the caller's workspace and is rebuilt on every call (4 KB, pageable copy: the call is
-  // not graph-capturable, which a render does not need) — nothing is cached, so a recycled workspace is harmless.
-  {
-    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-    cudaStreamIsCapturing(st, &cs);
-    B200_REQUIRE(cs != cudaStreamCaptureStatusActive, "the tensor-core render is not graph-capturable");
-  }
-  static thread_local PrepJobs pj_host;
-  PrepJobs* pj = &pj_host;
-  pj->n = 0;
-  prep_jobs_for_net(*pj, ms, im_map, params, false, false);
-  prep_jobs_for_net(*pj, as, im_atl, params + ms.total, true, false);
-  B200_CHECK_CUDA(cudaMemcpyAsync(d_prep, pj, sizeof(PrepJobs), cudaMemcpyHostToDevice, st));
-  tc_prep_kernel<<<pj->n * 4, 128, 0, st>>>(d_prep);
+  NetImages im_map, im_atl; PrepJobs* d_prep;
+  plan_infer(ms, as, ws, &im_map, &im_atl, &d_prep);
+  // one prep launch for both networks; the job table is rebuilt in the workspace on every call (4 KB)
+  g_pj.n = 0;
+  prep_jobs_for_net(g_pj, ms, im_map, params, TcNet::Mapping6, false);
+  prep_jobs_for_net(g_pj, as, im_atl, params + ms.total, TcNet::Atlas, false);
+  B200_PROPAGATE(upload(g_pj, &d_prep, false, st));
+  tc_prep_kernel<<<g_pj.n * 4, 128, 0, st>>>(d_prep);
   B200_CHECK_LAUNCH();
   const int tiles = (int)(rows / TM);
-  FwdParams pm{};
-  fill_fwd(pm, ms, im_map, x_map, uv, params, (int)rows, 1, nullptr);
+  FwdParams pm = fill_fwd(ms, im_map, x_map, uv, params, (int)rows, 1, nullptr);
   pm.store_images = 0;
-  tc_fwd_kernel<false><<<min(sm_count(), tiles), TC_THREADS, KCfg<false, false>::SMEM, st>>>(pm);
-  B200_CHECK_LAUNCH();
-  FwdParams pa{};
-  fill_fwd(pa, as, im_atl, uv, y, params + ms.total, (int)rows, 1, nullptr);
+  B200_PROPAGATE(launch_fwd(TcNet::Mapping6, pm, tiles, st));
+  FwdParams pa = fill_fwd(as, im_atl, uv, y, params + ms.total, (int)rows, 1, nullptr);
   pa.store_images = 0;
-  tc_fwd_kernel<true><<<min(sm_count(), tiles), TC_THREADS, KCfg<true, false>::SMEM, st>>>(pa);
-  B200_CHECK_LAUNCH();
-  return B200_OK;
+  return launch_fwd(TcNet::Atlas, pa, tiles, st);
 }
 
 // ---------------------------------------------------------------------------------------------
-// stand-alone evaluation of ONE of the two networks with autograd support: what the `IMLP` class needs
-// (implicit_neural_networks.py:62-81 forward + the autograd of its Linear/ReLU/tanh/skip stack).  Tables are
-// rebuilt into the caller's workspace on every call (pageable copies; not graph-capturable): no process-wide cache.
-// Workspace: [PrepJobs][WgradItems][images of the network].
+// stand-alone evaluation of ONE of the networks with autograd support: what the `IMLP` class needs
+// (implicit_neural_networks.py:62-81 forward + the autograd of its Linear/ReLU/tanh/skip stack).
+// Workspace: [PrepJobs][WgradItems][images of the network]; the two table slots serve ephemeral callers.
 // ---------------------------------------------------------------------------------------------
 struct SinglePlan { PrepJobs* d_prep; WgradItems* d_wg; NetImages im; int64_t bytes; };
 
-static void plan_single(const MlpShape& sh, bool is_atlas, int64_t rows, char* base, SinglePlan* out) {
-  char* p = reinterpret_cast<char*>(round_up(reinterpret_cast<int64_t>(base), 1024));
+static void plan_single(const MlpShape& sh, TcNet net, int64_t rows, char* base, SinglePlan* out) {
+  char* p = align_tc(base);
   out->d_prep = reinterpret_cast<PrepJobs*>(carve_tc(p, sizeof(PrepJobs)));
   out->d_wg = reinterpret_cast<WgradItems*>(carve_tc(p, sizeof(WgradItems)));
-  plan_net(sh, rows, is_atlas, p, &out->im);
+  plan_net(sh, rows, net, p, &out->im);
   out->bytes = p - base;
 }
 
-int64_t tc_single_workspace_bytes(const MlpShape& sh, bool is_atlas, int64_t rows) {
-  SinglePlan pl;
-  plan_single(sh, is_atlas, rows, nullptr, &pl);
+int64_t tc_single_workspace_bytes(const MlpShape& sh, TcNet net, int64_t rows) {
+  SinglePlan pl{};
+  plan_single(sh, net, rows, nullptr, &pl);
   return pl.bytes + 2048;
 }
 
-static int check_single(const MlpShape& sh, bool is_atlas, int64_t rows, cudaStream_t st) {
+static int check_single(const MlpShape& sh, TcNet net, int64_t rows) {
   B200_PROPAGATE(ensure_attrs());
-  if (is_atlas) {
-    bool no_skips = true;
-    for (int l = 1; l < sh.L; ++l) no_skips = no_skips && !sh.skip[l];
-    const bool atlas = sh.L == 8 && sh.skip[4] && sh.skip[7] && sh.pe == 10 && sh.hidden == HID && sh.in_dim == 2 && sh.out_dim == 3;
-    const bool alpha = sh.L == 8 && no_skips && sh.pe == 5 && sh.hidden == HID && sh.in_dim == 3 && sh.out_dim == 1;
-    B200_REQUIRE(atlas || alpha, "tensor-core IMLP: neither the atlas (2-PE10-256x6-3, skips 4,7) nor the alpha "
-                 "(3-PE5-256x6-1) architecture");
-  }
-  else {
-    bool plain = (sh.L == 6 || sh.L == 4) && sh.pe == 0 && sh.hidden == HID && sh.in_dim == 3 && sh.out_dim == 2;
-    for (int l = 1; plain && l < sh.L; ++l) plain = !sh.skip[l];
-    B200_REQUIRE(plain, "tensor-core IMLP: not a mapping architecture (3 -> 256 x {2,4} -> 2, no encoding, no skips)");
-  }
+  B200_REQUIRE(net != TcNet::None && tc_net_of(sh) == net, "tensor-core IMLP: the shape is not the network it is "
+               "called for (mapping 3-256x{4,2}-2, atlas 2-PE10-256x6-3 with skips 4, 7, alpha 3-PE5-256x6-1)");
   B200_REQUIRE(rows > 0 && rows % TM == 0 && rows / TM < (1 << 20), "rows must be a positive multiple of %d", TM);
   return B200_OK;
 }
 
-static bool stream_is_capturing(cudaStream_t st) {
-  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-  cudaStreamIsCapturing(st, &cs);
-  return cs == cudaStreamCaptureStatusActive;
-}
-
-// Job tables of stand-alone calls whose caller keeps ONE workspace and ONE set of parameter / gradient buffers alive
-// across calls (the segmentation step): like the fused loop's tables they are a pure function of pointers and geometry,
-// live in their own device allocations (never recycled) and are uploaded by the first eager call, after which the
-// calls are graph-capturable.  Ephemeral callers (the IMLP class: a fresh workspace per call) keep their tables
-// inside the workspace and upload them on every call.
-struct SingleTab {
-  int dev; const void* ws; int64_t rows; const void* params; const void* grads; bool is_atlas; int L, pe, in_dim; bool training;
-  PrepJobs* d_prep = nullptr; WgradItems* d_wg = nullptr; int n_prep = -1, n_wg = -1;
-};
-static std::vector<SingleTab*> g_single_tabs;
-
-static SingleTab* single_tab(const MlpShape& sh, bool is_atlas, const void* ws, int64_t rows, const void* params,
-                             const void* grads, bool training) {
-  const int dev = current_device();
-  std::lock_guard<std::mutex> lock(g_tabs_mutex);
-  for (SingleTab* t : g_single_tabs)
-    if (t->dev == dev && t->ws == ws && t->rows == rows && t->params == params && t->is_atlas == is_atlas && t->L == sh.L &&
-        t->pe == sh.pe && t->in_dim == sh.in_dim && t->training == training && (grads == nullptr || t->grads == nullptr || t->grads == grads)) {
-      if (grads && !t->grads) t->grads = grads;
-      return t;
-    }
-  if ((int)g_single_tabs.size() >= MAX_TABLES) return nullptr;
-  SingleTab* t = new SingleTab{dev, ws, rows, params, grads, is_atlas, sh.L, sh.pe, sh.in_dim, training};
-  g_single_tabs.push_back(t);
-  return t;
+// The tables of a stand-alone call: the cache entry of a persistent workspace, else the workspace's own slots.
+static TcTables* single_tables(TcTables& eph, TcNet net, const char* ws, int64_t rows, const float* params,
+                               const float* grads, bool training, bool persistent) {
+  if (!persistent) return &eph;
+  return find_tables(TabKey{current_device(), ws, net, false, training, (int)rows, 1, 0, params, grads}, true);
 }
 
 // x: mapping [rows][4], atlas [rows][2] (network input itself).  y: [rows][out_dim].
-int tc_single_forward(const MlpShape& sh, bool is_atlas, const float* params, const float* x, float* y, int64_t rows,
+int tc_single_forward(const MlpShape& sh, TcNet net, const float* params, const float* x, float* y, int64_t rows,
                       bool training, char* ws, bool persistent, cudaStream_t st) {
-  B200_PROPAGATE(check_single(sh, is_atlas, rows, st));
-  SinglePlan pl;
-  plan_single(sh, is_atlas, rows, ws, &pl);
-  static thread_local PrepJobs pj;
-  PrepJobs* d_prep = pl.d_prep;
-  int n_prep = 0;
-  SingleTab* tab = persistent ? single_tab(sh, is_atlas, ws, rows, params, nullptr, training) : nullptr;
-  if (tab && tab->n_prep >= 0) {
-    d_prep = tab->d_prep; n_prep = tab->n_prep;
-  } else {
-    B200_REQUIRE(!stream_is_capturing(st), "stand-alone tensor-core IMLP call under stream capture before its job tables "
-                 "exist: run the same call once eagerly first (persistent workspaces only)");
-    pj.n = 0;
-    prep_jobs_for_net(pj, sh, pl.im, params, is_atlas, training);
-    n_prep = pj.n;
-    if (tab) {
-      B200_CHECK_CUDA(cudaMalloc(&tab->d_prep, sizeof(PrepJobs)));
-      B200_CHECK_CUDA(cudaMemcpy(tab->d_prep, &pj, sizeof(PrepJobs), cudaMemcpyHostToDevice));
-      tab->n_prep = n_prep; d_prep = tab->d_prep;
-    } else {
-      B200_CHECK_CUDA(cudaMemcpyAsync(pl.d_prep, &pj, sizeof(PrepJobs), cudaMemcpyHostToDevice, st));
-    }
+  B200_PROPAGATE(check_single(sh, net, rows));
+  SinglePlan pl{};
+  plan_single(sh, net, rows, ws, &pl);
+  TcTables eph{}; eph.d_prep = pl.d_prep;
+  TcTables* tab = single_tables(eph, net, ws, rows, params, nullptr, training, persistent);
+  B200_REQUIRE(tab, "too many distinct tensor-core workspaces in one process (%d)", MAX_TABLES);
+  if (tab->n_prep < 0) {
+    g_pj.n = 0;
+    prep_jobs_for_net(g_pj, sh, pl.im, params, net, training);
+    B200_PROPAGATE(upload(g_pj, &tab->d_prep, persistent, st));
+    tab->n_prep = g_pj.n;
   }
-  tc_prep_kernel<<<n_prep * 4, 128, 0, st>>>(d_prep);
+  tc_prep_kernel<<<tab->n_prep * 4, 128, 0, st>>>(tab->d_prep);
   B200_CHECK_LAUNCH();
-  FwdParams P{};
-  fill_fwd(P, sh, pl.im, x, y, params, (int)rows, 1, nullptr);
+  FwdParams P = fill_fwd(sh, pl.im, x, y, params, (int)rows, 1, nullptr);
   P.in_scale = 1.0f; P.in_shift = 0.0f; P.store_images = training ? 1 : 0; P.tanh_out = sh.tanh_out ? 1 : 0;
-  const int grid = min(sm_count(), (int)(rows / TM));
-  if (is_atlas && sh.in_dim == 3) tc_fwd_kernel<true, 8, 1><<<grid, TC_THREADS, KCfg<true, false>::SMEM, st>>>(P);
-  else if (is_atlas) tc_fwd_kernel<true><<<grid, TC_THREADS, KCfg<true, false>::SMEM, st>>>(P);
-  else if (sh.L == 4) tc_fwd_kernel<false, 4><<<grid, TC_THREADS, KCfg<false, false>::SMEM, st>>>(P);
-  else tc_fwd_kernel<false><<<grid, TC_THREADS, KCfg<false, false>::SMEM, st>>>(P);
-  B200_CHECK_LAUNCH();
-  return B200_OK;
+  return launch_fwd(net, P, (int)(rows / TM), st);
 }
 
 // after tc_single_forward(training) on the same workspace.  y: the saved outputs, dy [rows][out_dim] (zero in padding
 // rows), gmax: device int holding the bits of max|dy| (>= 0), d_in: atlas only, [rows][2] or null.
-int tc_single_backward(const MlpShape& sh, bool is_atlas, const float* params, float* grads, const float* x,
+int tc_single_backward(const MlpShape& sh, TcNet net, const float* params, float* grads, const float* x,
                        const float* y, const float* dy, float* d_in, int* gmax2, int64_t rows, char* ws,
                        bool persistent, cudaStream_t st) {
-  B200_PROPAGATE(check_single(sh, is_atlas, rows, st));
-  SinglePlan pl;
-  plan_single(sh, is_atlas, rows, ws, &pl);
-  static thread_local WgradItems wi;
-  WgradItems* d_wg = pl.d_wg;
-  int n_wg = 0;
-  SingleTab* tab = persistent ? single_tab(sh, is_atlas, ws, rows, params, grads, true) : nullptr;
-  if (tab && tab->n_wg >= 0) {
-    d_wg = tab->d_wg; n_wg = tab->n_wg;
-  } else {
-    B200_REQUIRE(!stream_is_capturing(st), "stand-alone tensor-core IMLP backward under stream capture before its job "
-                 "tables exist: run the same call once eagerly first (persistent workspaces only)");
-    wi.n = 0;
-    WgProto protos[16]; int np = 0;
-    protos_for_net(protos, np, sh, pl.im, grads, is_atlas, 1);
-    apportion_items(wi, protos, np, (int)rows, 0);
-    n_wg = wi.n;
-    if (tab) {
-      B200_CHECK_CUDA(cudaMalloc(&tab->d_wg, sizeof(WgradItems)));
-      B200_CHECK_CUDA(cudaMemcpy(tab->d_wg, &wi, sizeof(WgradItems), cudaMemcpyHostToDevice));
-      tab->n_wg = n_wg; d_wg = tab->d_wg;
-    } else {
-      B200_CHECK_CUDA(cudaMemcpyAsync(pl.d_wg, &wi, sizeof(WgradItems), cudaMemcpyHostToDevice, st));
-    }
+  B200_PROPAGATE(check_single(sh, net, rows));
+  SinglePlan pl{};
+  plan_single(sh, net, rows, ws, &pl);
+  TcTables eph{}; eph.d_wg = pl.d_wg;
+  TcTables* tab = single_tables(eph, net, ws, rows, params, grads, true, persistent);
+  B200_REQUIRE(tab, "too many distinct tensor-core workspaces in one process (%d)", MAX_TABLES);
+  if (tab->n_wg < 0) {
+    WgProto protos[32]; int np = 0;
+    protos_for_net(protos, np, sh, pl.im, grads, net, 1);
+    g_wi.n = 0;
+    apportion_items(g_wi, protos, np, (int)rows, 0);
+    B200_PROPAGATE(upload(g_wi, &tab->d_wg, persistent, st));
+    tab->n_wg = g_wi.n;
   }
-  BwdParams P{};
-  P.dy = dy; P.y = y; P.x = x; P.d_in = d_in; P.params = params; P.grads = grads; P.img = pl.im;
-  P.cap = (int)rows; P.n_groups = 1; P.n_valid = nullptr; P.gmax_bits = gmax2;      // [0] atlas scale, [1] mapping scale
-  P.in_scale = 1.0f; P.d_in_accumulate = 0; P.tanh_out = sh.tanh_out ? 1 : 0; P.flow_groups = 0;
-  for (int l = 0; l < sh.L; ++l) { P.w_off[l] = sh.w_off[l]; P.b_off[l] = sh.b_off[l]; }
-  const int grid = min(sm_count(), (int)(rows / TM));
-  if (is_atlas && sh.in_dim == 3) tc_bwd_kernel<true, 8, 1><<<grid, TC_THREADS, KCfg<true, true>::SMEM, st>>>(P);
-  else if (is_atlas) tc_bwd_kernel<true><<<grid, TC_THREADS, KCfg<true, true>::SMEM, st>>>(P);
-  else if (sh.L == 4) tc_bwd_kernel<false, 4><<<grid, TC_THREADS, KCfg<false, true>::SMEM, st>>>(P);
-  else tc_bwd_kernel<false><<<grid, TC_THREADS, KCfg<false, true>::SMEM, st>>>(P);
-  B200_CHECK_LAUNCH();
-  tc_wgrad_kernel<<<min(n_wg, sm_count()), WG_THREADS, WG_SMEM, st>>>(d_wg, nullptr, gmax2);
+  // gmax2: [0] atlas scale, [1] mapping scale
+  BwdParams P = fill_bwd(sh, pl.im, dy, y, x, d_in, params, grads, (int)rows, 1, nullptr, gmax2);
+  P.in_scale = 1.0f; P.d_in_accumulate = 0; P.tanh_out = sh.tanh_out ? 1 : 0;
+  B200_PROPAGATE(launch_bwd(net, P, (int)(rows / TM), st));
+  tc_wgrad_kernel<<<min(tab->n_wg, sm_count()), WG_THREADS, WG_SMEM, st>>>(tab->d_wg, nullptr, gmax2);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
-
-int tc_atlas_forward(const TcStep& s, cudaStream_t st) { return run_forward(s, true, st); }
-int tc_atlas_backward(const TcStep& s, cudaStream_t st) { return run_backward(s, true, st); }
-int tc_mapping_forward(const TcStep& s, cudaStream_t st) { return run_forward(s, false, st); }
-int tc_mapping_backward(const TcStep& s, cudaStream_t st) { return run_backward(s, false, st); }
 
 }  // namespace b200

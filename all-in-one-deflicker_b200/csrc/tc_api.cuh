@@ -4,6 +4,16 @@
 
 namespace b200 {
 
+// The networks the tensor-core kernels are instantiated for: the stage-1 mapping (3-256x4-2), the background mapping of
+// the segmentation variant (3-256x2-2), the atlas (2-PE10-256x6-3, skips 4, 7) and the alpha network of the
+// segmentation variant (3-PE5-256x6-1).
+enum class TcNet { None, Mapping6, Mapping4, Atlas, Alpha };
+TcNet tc_net_of(const MlpShape& s);
+// atlas and alpha: the positional encoding feeds layer 0, which runs on the tensor cores
+inline bool tc_pe_first(TcNet n) { return n == TcNet::Atlas || n == TcNet::Alpha; }
+// the atlas back-propagates to its input (uv) through the encoding; the other networks' inputs are pixel coordinates
+inline bool tc_net_has_dpe(TcNet n) { return n == TcNet::Atlas; }
+
 // Buffers of the tensor-core path, carved from the caller's workspace (see mlp_tc.cu).
 struct TcPlan {
   char* base = nullptr;
@@ -17,7 +27,7 @@ struct TcStep {
   const float* params; float* grads;
   const float* x_map;        // [n_groups*cap][4]
   float* uv;                 // [n_groups*cap][2]  mapping output
-  float* y_atlas;            // [3*cap][3]         atlas output
+  float* y_atlas;            // [3*cap][3]         atlas output; null: pre-training (mapping only)
   const float* d_uv;         // [n_groups*cap][2]  direct gradient of the loss head
   const float* d_y;          // [3*cap][3]
   int cap, n_groups;
@@ -27,11 +37,9 @@ struct TcStep {
 
 int64_t tc_plan(const MlpShape& ms, const MlpShape& as, int64_t rows_map, int64_t rows_atlas, char* base,
                 TcPlan* out);
-int tc_begin_step(const TcStep& s, cudaStream_t st);       // optional: start the weight-image preparation early (side stream)
-int tc_atlas_forward(const TcStep& s, cudaStream_t st);    // mapping on all groups, atlas on groups 0..2
-int tc_atlas_backward(const TcStep& s, cudaStream_t st);   // all parameter gradients
-int tc_mapping_forward(const TcStep& s, cudaStream_t st);  // pre-training: mapping only
-int tc_mapping_backward(const TcStep& s, cudaStream_t st);
+int tc_begin_step(const TcStep& s, cudaStream_t st);      // optional: start the weight-image preparation early (side stream)
+int tc_step_forward(const TcStep& s, cudaStream_t st);    // mapping on all groups, atlas on groups 0..2
+int tc_step_backward(const TcStep& s, cudaStream_t st);   // all parameter gradients
 
 // inference (render): x_map [rows][4] -> uv [rows][2] -> y [rows][3]; rows a multiple of 128; ws >= tc_infer_workspace_bytes
 int64_t tc_infer_workspace_bytes(const MlpShape& ms, const MlpShape& as);
@@ -39,12 +47,12 @@ int tc_infer_forward(const MlpShape& ms, const MlpShape& as, const float* params
                      float* y, int64_t rows, char* ws, cudaStream_t st);
 
 // stand-alone IMLP (one network, autograd): see mlp_tc.cu
-int64_t tc_single_workspace_bytes(const MlpShape& sh, bool is_atlas, int64_t rows);
+int64_t tc_single_workspace_bytes(const MlpShape& sh, TcNet net, int64_t rows);
 // persistent: the caller keeps this workspace and these parameter / gradient buffers across calls -> job tables are
 // cached in their own device allocations and the calls become graph-capturable after one eager call
-int tc_single_forward(const MlpShape& sh, bool is_atlas, const float* params, const float* x, float* y, int64_t rows,
+int tc_single_forward(const MlpShape& sh, TcNet net, const float* params, const float* x, float* y, int64_t rows,
                       bool training, char* ws, bool persistent, cudaStream_t st);
-int tc_single_backward(const MlpShape& sh, bool is_atlas, const float* params, float* grads, const float* x,
+int tc_single_backward(const MlpShape& sh, TcNet net, const float* params, float* grads, const float* x,
                        const float* y, const float* dy, float* d_in, int* gmax2, int64_t rows, char* ws, bool persistent,
                        cudaStream_t st);
 
