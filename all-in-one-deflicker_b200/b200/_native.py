@@ -98,6 +98,16 @@ SIGNATURES = {
     "b200_atlas_workspace_offsets": (C.c_int, [C.POINTER(AtlasConfig), _P, C.POINTER(_I64)]),
     "b200_atlas_loss_grad": (C.c_int, [C.POINTER(AtlasConfig), C.POINTER(Video), _P, _P, _P, _P, _P, _I64, _P]),
     "b200_pretrain_loss_grad": (C.c_int, [C.POINTER(AtlasConfig), _I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _I64, _P]),
+    "b200_atlas_param_floats_for": (_I64, [C.POINTER(MlpDesc)]),
+    "b200_atlas_workspace_bytes_for": (_I64, [C.POINTER(AtlasConfig), C.POINTER(MlpDesc)]),
+    "b200_atlas_workspace_offsets_for": (C.c_int, [C.POINTER(AtlasConfig), C.POINTER(MlpDesc), _P, C.POINTER(_I64)]),
+    "b200_atlas_loss_grad_for": (C.c_int, [C.POINTER(AtlasConfig), C.POINTER(MlpDesc), C.POINTER(Video), _P, _P, _P, _P,
+                                           _P, _I64, _P]),
+    "b200_pretrain_loss_grad_for": (C.c_int, [C.POINTER(AtlasConfig), C.POINTER(MlpDesc), _I32, _I32, _I32, _P, _P, _P,
+                                              _P, _P, _P, _I64, _P]),
+    "b200_render_workspace_bytes_for": (_I64, [C.POINTER(MlpDesc), _I64]),
+    "b200_render_for": (C.c_int, [C.POINTER(MlpDesc), _P, _I32, _I32, _I32, _I32, _I64, _I64, _P, _P, C.c_int, _P, _I64,
+                                  _P]),
     "b200_adam_step": (C.c_int, [_P, _P, _P, _P, _I64, C.c_double, C.c_double, C.c_double, C.c_double, _F, _P, _P]),
     "b200_gradient_loss_head": (C.c_int, [_P] * 5 + [_I64] + [_P] * 5),
     "b200_rigidity_loss_head": (C.c_int, [_P, _P, _I64, _F, _F, _F, _P, _P, _P, _P, _P]),

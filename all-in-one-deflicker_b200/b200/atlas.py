@@ -189,13 +189,30 @@ DeviceVideo.from_files = classmethod(_from_files)
 # the segmentation trainer, which takes any IMLP shape)
 FUSED_ARCHITECTURE = dict(number_of_layers_mapping1=6, number_of_channels_mapping1=256, use_positional_encoding_mapping1=False,
                           number_of_layers_atlas=8, number_of_channels_atlas=256, positional_encoding_num_atlas=10)
+# ... or a mapping on the positional encoding of (x, y, t): use_positional_encoding_mapping1 with
+# number_of_positional_encoding_mapping1 frequencies (the tensor-core kernels keep the 6 P columns in one 64-column chunk)
+MAPPING_PE_FREQS = range(1, 11)
+
+
+def mapping_pe_freqs(config: Optional[dict]) -> int:
+    """Frequencies of the mapping's positional encoding the config asks for (0: none)."""
+    if not config or not config.get("use_positional_encoding_mapping1", False):
+        return 0
+    return config["number_of_positional_encoding_mapping1"]
 
 
 def check_architecture(config: dict):
     """Raise instead of silently training a different model than the config describes."""
-    bad = {k: config[k] for k, v in FUSED_ARCHITECTURE.items() if k in config and config[k] != v}
+    bad = {k: config[k] for k, v in FUSED_ARCHITECTURE.items()
+           if k in config and config[k] != v and k != "use_positional_encoding_mapping1"}
+    if config.get("use_positional_encoding_mapping1", False) is not False:
+        pe = config.get("number_of_positional_encoding_mapping1")
+        if config["use_positional_encoding_mapping1"] is not True or type(pe) is not int or pe not in MAPPING_PE_FREQS:
+            bad["use_positional_encoding_mapping1"] = config["use_positional_encoding_mapping1"]
+            bad["number_of_positional_encoding_mapping1"] = pe
     if bad:
-        raise N.B200Error(f"the fused stage-1 step is built for {FUSED_ARCHITECTURE}; the config asks for {bad}. "
+        raise N.B200Error(f"the fused stage-1 step is built for {FUSED_ARCHITECTURE} (or use_positional_encoding_mapping1 "
+                          f"with number_of_positional_encoding_mapping1 in 1..10); the config asks for {bad}. "
                           "Use the IMLP class + src/models/stage_1/loss_utils.py (any shape) for other architectures.")
 
 
@@ -220,11 +237,12 @@ class AtlasTrainer:
             import torch.distributed as dist
             self.world = dist.get_world_size(process_group)
         self.resx = resx if resx is not None else (video.W if video is not None else 0)
-        self.map_desc = make_desc(**MAPPING_DESC)
+        # the mapping of src/stage1_neural_atlas.py:112-119, with the positional encoding the config may ask for
+        self.map_desc = make_desc(**dict(MAPPING_DESC, pe_freqs=mapping_pe_freqs(config)))
         self.atlas_desc = make_desc(**ATLAS_DESC)
         self.map_w, self.map_b, self.map_total = mlp_layout(self.map_desc)
         self.atl_w, self.atl_b, self.atl_total = mlp_layout(self.atlas_desc)
-        self.n_params = int(self.lib.b200_atlas_param_floats())
+        self.n_params = int(self.lib.b200_atlas_param_floats_for(C.byref(self.map_desc)))
         assert self.n_params == self.map_total + self.atl_total
         dev = self.device
         # gradients + the loss vector share one buffer so that data parallelism needs ONE exchange
@@ -329,10 +347,11 @@ class AtlasTrainer:
     def _workspace(self):
         if self._ws is None:
             cfg = self._config(True)
-            nbytes = int(self.lib.b200_atlas_workspace_bytes(C.byref(cfg)))
+            md = C.byref(self.map_desc)
+            nbytes = int(self.lib.b200_atlas_workspace_bytes_for(C.byref(cfg), md))
             if cfg.batch < 10000:        # pre_train_mapping always draws 10000 pixels (unwrap_utils.py:183)
                 cfg.batch = 10000
-                nbytes = max(nbytes, int(self.lib.b200_atlas_workspace_bytes(C.byref(cfg))))
+                nbytes = max(nbytes, int(self.lib.b200_atlas_workspace_bytes_for(C.byref(cfg), md)))
             if nbytes < 0:
                 raise N.B200Error(self.lib.b200_last_error().decode())
             self._ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
@@ -345,7 +364,8 @@ class AtlasTrainer:
         cfg = self._config(True)
         ws = self._workspace()
         off = (C.c_int64 * 8)()
-        N.check(self.lib.b200_atlas_workspace_offsets(C.byref(cfg), N.ptr(ws), off), "b200_atlas_workspace_offsets")
+        N.check(self.lib.b200_atlas_workspace_offsets_for(C.byref(cfg), C.byref(self.map_desc), N.ptr(ws), off),
+                "b200_atlas_workspace_offsets_for")
         cap = (cfg.batch + 127) // 128 * 128
         f32 = lambda o, n, *shape: ws[o:o + 4 * n].view(torch.float32).view(*shape)
         return dict(cap=cap, counters=ws[off[0]:off[0] + 32].view(torch.int32),
@@ -359,9 +379,10 @@ class AtlasTrainer:
         """sampling -> forward -> losses -> backward for the indices currently in self.indices."""
         cfg = self._config(with_global)
         ws = self._workspace()
-        N.check(self.lib.b200_atlas_loss_grad(C.byref(cfg), C.byref(self.video.struct), N.ptr(self.indices),
-                                              N.ptr(self.params), N.ptr(self.grads), N.ptr(self.losses),
-                                              N.ptr(ws), ws.numel(), N.current_stream()), "b200_atlas_loss_grad")
+        N.check(self.lib.b200_atlas_loss_grad_for(C.byref(cfg), C.byref(self.map_desc), C.byref(self.video.struct),
+                                                  N.ptr(self.indices), N.ptr(self.params), N.ptr(self.grads),
+                                                  N.ptr(self.losses), N.ptr(ws), ws.numel(), N.current_stream()),
+                "b200_atlas_loss_grad_for")
 
     # ------------------------------------------------------------------ data parallelism over NVLink peer memory
     def _setup_fused_dp(self, required: bool):
@@ -499,10 +520,11 @@ class AtlasTrainer:
                 xs = torch.randint(W, (10000, 1), generator=generator)
                 ys_d.copy_(ys.reshape(-1), non_blocking=True)
                 xs_d.copy_(xs.reshape(-1), non_blocking=True)
-                N.check(self.lib.b200_pretrain_loss_grad(C.byref(cfg), larger, T, f, N.ptr(ys_d), N.ptr(xs_d),
-                                                         N.ptr(self.params), N.ptr(self.grads), N.ptr(self.losses),
-                                                         N.ptr(ws), ws.numel(), N.current_stream()),
-                        "b200_pretrain_loss_grad")
+                N.check(self.lib.b200_pretrain_loss_grad_for(C.byref(cfg), C.byref(self.map_desc), larger, T, f,
+                                                             N.ptr(ys_d), N.ptr(xs_d), N.ptr(self.params),
+                                                             N.ptr(self.grads), N.ptr(self.losses), N.ptr(ws),
+                                                             ws.numel(), N.current_stream()),
+                        "b200_pretrain_loss_grad_for")
                 self.adam(self.params, self.grads, m, v, step, n)
                 last = self.losses
             if progress:
@@ -518,15 +540,16 @@ class AtlasTrainer:
         chunk = H * W if chunk is None else min(chunk, H * W)
         rgb = torch.empty(H * W * 3, dtype=torch.float32, device=self.device)
         u8 = torch.empty(H * W * 3, dtype=torch.uint8, device=self.device) if want_u8 else None
-        nbytes = int(self.lib.b200_render_workspace_bytes(chunk))
+        md = C.byref(self.map_desc)
+        nbytes = int(self.lib.b200_render_workspace_bytes_for(md, chunk))
         ws = getattr(self, "_render_ws", None)
         if ws is None or ws.numel() < nbytes:
             ws = self._render_ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
         for p0 in range(0, H * W, chunk):
             p1 = min(H * W, p0 + chunk)
-            N.check(self.lib.b200_render(N.ptr(self.params), H, W, T, f, p0, p1, N.ptr(rgb[p0 * 3:]),
-                                         N.ptr(u8[p0 * 3:]) if want_u8 else None, prec, N.ptr(ws),
-                                         ws.numel(), N.current_stream()), "b200_render")
+            N.check(self.lib.b200_render_for(md, N.ptr(self.params), H, W, T, f, p0, p1, N.ptr(rgb[p0 * 3:]),
+                                             N.ptr(u8[p0 * 3:]) if want_u8 else None, prec, N.ptr(ws),
+                                             ws.numel(), N.current_stream()), "b200_render_for")
         out = rgb.view(H, W, 3)
         return (out, u8.view(H, W, 3)) if want_u8 else out
 

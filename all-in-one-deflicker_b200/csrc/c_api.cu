@@ -107,9 +107,27 @@ struct AtlasPlan {
   int64_t bytes = 0;
 };
 
-static int plan_atlas(const B200AtlasConfig* cfg, char* base, AtlasPlan* pl) {
+// The mapping of the single-layer script: 3 -> 256 x 4 -> 2 with tanh, either on the raw (x, y, t) or on their positional
+// encoding with 1..10 frequencies (use_positional_encoding_mapping1, src/stage1_neural_atlas.py:112-119).
+static int resolve_step_mapping(const B200MlpDesc* d, MlpShape* s) {
+  B200_REQUIRE(d != nullptr, "null mapping descriptor");
+  B200_PROPAGATE(resolve_mlp(d, s));
+  const TcNet net = tc_net_of(*s);
+  B200_REQUIRE((net == TcNet::Mapping6 || net == TcNet::MappingPE6) && s->tanh_out,
+               "the fused stage-1 step takes a 6-layer mapping 3 -> [PE 1..10 ->] 256 x 4 -> 2 with tanh");
+  return B200_OK;
+}
+
+// layer-0 input of a PE mapping on the fp32 path: the encoding of the raw (x, y, t) rows (float4 rows)
+static int mapping_pe_forward(const MlpShape& ms, const float* x_map, const MlpScratch& sc, const RowSpan& span,
+                              cudaStream_t st) {
+  if (ms.pe == 0) return B200_OK;
+  return launch_pe_forward(x_map, 4, 1.f, 0.f, 3, ms.pe, sc.act[0], ms.K[0], nullptr, nullptr, 0, ms.hidden, span, st);
+}
+
+static int plan_atlas(const B200AtlasConfig* cfg, const B200MlpDesc* mapping, char* base, AtlasPlan* pl) {
   B200_REQUIRE(cfg && cfg->batch > 0 && cfg->batch <= 16384, "samples_batch must be in [1, 16384]");
-  B200_PROPAGATE(resolve_mlp(&mapping_desc(), &pl->ms));
+  B200_PROPAGATE(resolve_step_mapping(mapping, &pl->ms));
   B200_PROPAGATE(resolve_mlp(&atlas_desc(), &pl->as));
   pl->cap = (int)round_up(cfg->batch, kTileRows);
   pl->n_groups = G_COUNT;      // buffers always sized for the 9-group regime
@@ -177,7 +195,7 @@ int64_t b200_mlp_layout(const B200MlpDesc* d, int64_t* w_off, int64_t* b_off) {
 }
 
 // which stage-1 architecture a descriptor is (tensor-core kernels are specialised to them): 1 mapping (either depth),
-// 2 atlas, 3 alpha, 0 none
+// 2 atlas, 3 alpha, 4 position-encoded mapping (either depth), 0 none
 int b200_mlp_tc_architecture(const B200MlpDesc* d) {
   MlpShape s;
   if (resolve_mlp(d, &s) != B200_OK) return -1;
@@ -185,6 +203,7 @@ int b200_mlp_tc_architecture(const B200MlpDesc* d) {
     case TcNet::Mapping6: case TcNet::Mapping4: return 1;
     case TcNet::Atlas: return 2;
     case TcNet::Alpha: return 3;
+    case TcNet::MappingPE6: case TcNet::MappingPE4: return 4;
     default: return 0;
   }
 }
@@ -220,8 +239,9 @@ static int tc_call_prepare(const B200MlpDesc* d, int64_t rows, void* ws, int64_t
                            int64_t* rows_pad, TcCallPlan* pl) {
   B200_PROPAGATE(resolve_mlp(d, s));
   *net = tc_net_of(*s);
-  B200_REQUIRE(*net != TcNet::None, "B200_PREC_TC serves the stage-1 architectures (mapping: 3-256x{2,4}-2 without encoding; alpha: 3-PE5-256x6-1; "
-               "atlas: 2-PE10-256x6-3 with skips 4, 7); use B200_PREC_FP32 for other shapes");
+  B200_REQUIRE(*net != TcNet::None, "B200_PREC_TC serves the stage-1 architectures (mapping: 3-256x{2,4}-2 without encoding "
+               "or 3-PE{1..10}-256x{2,4}-2; alpha: 3-PE5-256x6-1; atlas: 2-PE10-256x6-3 with skips 4, 7); use B200_PREC_FP32 "
+               "for other shapes");
   if (!b200_device_supports_tc()) { set_error("B200_PREC_TC needs a compute-capability 9.x device"); return B200_ERR_UNSUPPORTED; }
   B200_REQUIRE(rows > 0 && rows < (1ll << 26), "rows out of range: %lld", (long long)rows);
   B200_REQUIRE(ws != nullptr, "null workspace");
@@ -296,7 +316,7 @@ int b200_mlp_backward(const B200MlpDesc* d, const float* params, const float* x,
                  "(their inputs are pixel coordinates); use B200_PREC_FP32 when x requires grad");
     B200_PROPAGATE(launch_pack_rows(dy, s.out_dim, s.out_dim, pl.dy, s.out_dim, rows, rows_pad, st));
     B200_CHECK_CUDA(cudaMemsetAsync(pl.gmax2, 0, 8, st));
-    B200_PROPAGATE(launch_absmax(pl.dy, rows_pad * s.out_dim, pl.gmax2 + (tc_pe_first(net) ? 0 : 1), st));
+    B200_PROPAGATE(launch_absmax(pl.dy, rows_pad * s.out_dim, pl.gmax2 + (tc_net_is_mapping(net) ? 1 : 0), st));
     B200_PROPAGATE(tc_single_backward(s, net, params, dparams, pl.x, pl.y, pl.dy, (tc_net_has_dpe(net) && dx) ? pl.d_in : nullptr,
                                       pl.gmax2, rows_pad, pl.tc, g_persistent_ws, st));
     if (tc_net_has_dpe(net) && dx) B200_CHECK_CUDA(cudaMemcpyAsync(dx, pl.d_in, (size_t)rows * 8, cudaMemcpyDeviceToDevice, st));
@@ -336,24 +356,35 @@ int b200_video_pack(const float* frames, const float* frames_dx, const float* fr
                            t_end, records, mask_fwd_bits, mask_bwd_bits, reinterpret_cast<cudaStream_t>(stream));
 }
 
-int64_t b200_atlas_param_floats(void) {
+int64_t b200_atlas_param_floats(void) { return b200_atlas_param_floats_for(&mapping_desc()); }
+
+int64_t b200_atlas_param_floats_for(const B200MlpDesc* mapping) {
   MlpShape m, a;
-  resolve_mlp(&mapping_desc(), &m);
+  if (resolve_step_mapping(mapping, &m) != B200_OK) return -1;
   resolve_mlp(&atlas_desc(), &a);
   return m.total + a.total;
 }
 
 int64_t b200_atlas_workspace_bytes(const B200AtlasConfig* cfg) {
+  return b200_atlas_workspace_bytes_for(cfg, &mapping_desc());
+}
+
+int64_t b200_atlas_workspace_bytes_for(const B200AtlasConfig* cfg, const B200MlpDesc* mapping) {
   AtlasPlan pl;
-  if (plan_atlas(cfg, nullptr, &pl) != B200_OK) return -1;
+  if (plan_atlas(cfg, mapping, nullptr, &pl) != B200_OK) return -1;
   return pl.bytes + 256 + 2048;      // slack for the 256 / 1024-byte alignment of the real base address
 }
 
 int b200_atlas_workspace_offsets(const B200AtlasConfig* cfg, const void* ws, int64_t* offsets) {
+  return b200_atlas_workspace_offsets_for(cfg, &mapping_desc(), ws, offsets);
+}
+
+int b200_atlas_workspace_offsets_for(const B200AtlasConfig* cfg, const B200MlpDesc* mapping, const void* ws,
+                                     int64_t* offsets) {
   B200_REQUIRE(cfg && ws && offsets, "null pointer");
   AtlasPlan pl;
   char* base = reinterpret_cast<char*>(round_up(reinterpret_cast<int64_t>(ws), 256));
-  B200_PROPAGATE(plan_atlas(cfg, base, &pl));
+  B200_PROPAGATE(plan_atlas(cfg, mapping, base, &pl));
   const char* w = reinterpret_cast<const char*>(ws);
   offsets[0] = reinterpret_cast<char*>(pl.counters) - w;
   offsets[1] = reinterpret_cast<char*>(pl.list) - w;
@@ -366,10 +397,11 @@ int b200_atlas_workspace_offsets(const B200AtlasConfig* cfg, const void* ws, int
   return B200_OK;
 }
 
-static int atlas_prepare(const B200AtlasConfig* cfg, void* ws, int64_t ws_bytes, AtlasPlan* pl) {
+static int atlas_prepare(const B200AtlasConfig* cfg, const B200MlpDesc* mapping, void* ws, int64_t ws_bytes,
+                         AtlasPlan* pl) {
   B200_REQUIRE(ws != nullptr, "null workspace");
   char* base = reinterpret_cast<char*>(round_up(reinterpret_cast<int64_t>(ws), 256));
-  B200_PROPAGATE(plan_atlas(cfg, base, pl));
+  B200_PROPAGATE(plan_atlas(cfg, mapping, base, pl));
   if (base + pl->bytes > reinterpret_cast<char*>(ws) + ws_bytes) {
     set_error("workspace too small: need %lld bytes", (long long)(pl->bytes + 256));
     return B200_ERR_WORKSPACE;
@@ -386,12 +418,18 @@ static int atlas_prepare(const B200AtlasConfig* cfg, void* ws, int64_t ws_bytes,
 int b200_atlas_loss_grad(const B200AtlasConfig* cfg, const B200Video* video, const int64_t* indices,
                          const float* params, float* grads, float* losses, void* ws, int64_t ws_bytes,
                          void* stream) {
+  return b200_atlas_loss_grad_for(cfg, &mapping_desc(), video, indices, params, grads, losses, ws, ws_bytes, stream);
+}
+
+int b200_atlas_loss_grad_for(const B200AtlasConfig* cfg, const B200MlpDesc* mapping, const B200Video* video,
+                             const int64_t* indices, const float* params, float* grads, float* losses, void* ws,
+                             int64_t ws_bytes, void* stream) {
   B200_REQUIRE(cfg && video && indices && params && grads && losses, "null pointer");
   B200_REQUIRE(video->records && video->mask_fwd_bits && video->mask_bwd_bits, "video not packed");
   B200_REQUIRE(video->H > 0 && video->W > 0 && video->T > 0 && video->t_begin >= 0 && video->t_end <= video->T,
                "bad video extents");
   AtlasPlan pl;
-  B200_PROPAGATE(atlas_prepare(cfg, ws, ws_bytes, &pl));
+  B200_PROPAGATE(atlas_prepare(cfg, mapping, ws, ws_bytes, &pl));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int cap = pl.cap;
   const int ng = cfg->with_global ? G_COUNT : G_YMG;        // 9 or 7 row groups
@@ -437,6 +475,7 @@ int b200_atlas_loss_grad(const B200AtlasConfig* cfg, const B200Video* video, con
   float* g_atl = grads + pl.ms.total;
 
   if (cfg->precision == B200_PREC_FP32) {
+    B200_PROPAGATE(mapping_pe_forward(pl.ms, pl.x_map, pl.map, span_map, st));
     B200_PROPAGATE(simt_mlp_forward(pl.ms, p_map, pl.x_map, 4, span_map, pl.map, pl.map.y, st));
     float* skips[2] = {pl.atlas.act[4], pl.atlas.act[7]};
     int lds[2] = {pl.as.K[4], pl.as.K[7]};
@@ -462,10 +501,17 @@ int b200_atlas_loss_grad(const B200AtlasConfig* cfg, const B200Video* video, con
 int b200_pretrain_loss_grad(const B200AtlasConfig* cfg, int32_t larger_dim, int32_t T, int32_t frame,
                             const int64_t* ys, const int64_t* xs, const float* params, float* grads,
                             float* losses, void* ws, int64_t ws_bytes, void* stream) {
+  return b200_pretrain_loss_grad_for(cfg, &mapping_desc(), larger_dim, T, frame, ys, xs, params, grads, losses, ws,
+                                     ws_bytes, stream);
+}
+
+int b200_pretrain_loss_grad_for(const B200AtlasConfig* cfg, const B200MlpDesc* mapping, int32_t larger_dim, int32_t T,
+                                int32_t frame, const int64_t* ys, const int64_t* xs, const float* params, float* grads,
+                                float* losses, void* ws, int64_t ws_bytes, void* stream) {
   B200_REQUIRE(cfg && ys && xs && params && grads && losses, "null pointer");
   B200_REQUIRE(larger_dim > 0 && T > 0 && frame >= 0, "bad geometry");
   AtlasPlan pl;
-  B200_PROPAGATE(atlas_prepare(cfg, ws, ws_bytes, &pl));
+  B200_PROPAGATE(atlas_prepare(cfg, mapping, ws, ws_bytes, &pl));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int cap = pl.cap;
   B200_CHECK_CUDA(cudaMemsetAsync(grads, 0, (size_t)pl.ms.total * 4, st));
@@ -476,6 +522,7 @@ int b200_pretrain_loss_grad(const B200AtlasConfig* cfg, int32_t larger_dim, int3
                                         pl.counters, st));
   RowSpan span{(int64_t)cap, cap, pl.counters};
   if (cfg->precision == B200_PREC_FP32) {
+    B200_PROPAGATE(mapping_pe_forward(pl.ms, pl.x_map, pl.map, span, st));
     B200_PROPAGATE(simt_mlp_forward(pl.ms, params, pl.x_map, 4, span, pl.map, pl.map.y, st));
     B200_PROPAGATE(launch_pretrain_loss(pl.x_map, pl.map.y, cfg->batch, cap, cfg->uv_mapping_scale, pl.d_uv,
                                         losses, pl.counters, st));
@@ -533,10 +580,12 @@ int b200_dp_adam_step(const B200DpComm* comm, float* exp_avg, float* exp_avg_sq,
                         reinterpret_cast<cudaStream_t>(stream));
 }
 
-int64_t b200_render_workspace_bytes(int64_t pixels) {
+int64_t b200_render_workspace_bytes(int64_t pixels) { return b200_render_workspace_bytes_for(&mapping_desc(), pixels); }
+
+int64_t b200_render_workspace_bytes_for(const B200MlpDesc* mapping, int64_t pixels) {
   if (pixels <= 0) return -1;
   MlpShape m, a;
-  resolve_mlp(&mapping_desc(), &m);
+  if (resolve_step_mapping(mapping, &m) != B200_OK) return -1;
   resolve_mlp(&atlas_desc(), &a);
   const int64_t rows = round_up(pixels, kTileRows);
   const int64_t fp32_path = round_up(rows * 16, 256) + plan_mlp_scratch(m, rows, false, nullptr, nullptr) +
@@ -549,12 +598,21 @@ int64_t b200_render_workspace_bytes(int64_t pixels) {
 int b200_render(const float* params, int32_t H, int32_t W, int32_t T, int32_t frame, int64_t pix_begin,
                 int64_t pix_end, float* rgb, uint8_t* rgb_u8, int precision, void* ws, int64_t ws_bytes,
                 void* stream) {
+  return b200_render_for(&mapping_desc(), params, H, W, T, frame, pix_begin, pix_end, rgb, rgb_u8, precision, ws,
+                         ws_bytes, stream);
+}
+
+int b200_render_for(const B200MlpDesc* mapping, const float* params, int32_t H, int32_t W, int32_t T, int32_t frame,
+                    int64_t pix_begin, int64_t pix_end, float* rgb, uint8_t* rgb_u8, int precision, void* ws,
+                    int64_t ws_bytes, void* stream) {
   B200_REQUIRE(params && ws && (rgb || rgb_u8), "null pointer");
   B200_REQUIRE(H > 0 && W > 0 && T > 0 && frame >= 0 && frame < T && pix_begin >= 0 && pix_end <= (int64_t)H * W &&
                pix_begin < pix_end, "bad render range");
+  MlpShape m, a;
+  B200_PROPAGATE(resolve_step_mapping(mapping, &m));
   const int64_t count = pix_end - pix_begin;
-  if (ws_bytes < b200_render_workspace_bytes(count)) {
-    set_error("workspace too small: need %lld bytes", (long long)b200_render_workspace_bytes(count));
+  if (ws_bytes < b200_render_workspace_bytes_for(mapping, count)) {
+    set_error("workspace too small: need %lld bytes", (long long)b200_render_workspace_bytes_for(mapping, count));
     return B200_ERR_WORKSPACE;
   }
   B200_REQUIRE(precision == B200_PREC_FP32 || precision == B200_PREC_TC, "unknown precision %d", precision);
@@ -562,8 +620,6 @@ int b200_render(const float* params, int32_t H, int32_t W, int32_t T, int32_t fr
     set_error("B200_PREC_TC needs a compute-capability 9.x device");
     return B200_ERR_UNSUPPORTED;
   }
-  MlpShape m, a;
-  B200_PROPAGATE(resolve_mlp(&mapping_desc(), &m));
   B200_PROPAGATE(resolve_mlp(&atlas_desc(), &a));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int64_t rows = round_up(count, kTileRows);
@@ -584,6 +640,7 @@ int b200_render(const float* params, int32_t H, int32_t W, int32_t T, int32_t fr
   p += plan_mlp_scratch(m, rows, false, p, &sm);
   p += plan_mlp_scratch(a, rows, false, p, &sa);
   RowSpan span{rows, 0, nullptr};
+  B200_PROPAGATE(mapping_pe_forward(m, x_map, sm, span, st));
   B200_PROPAGATE(simt_mlp_forward(m, params, x_map, 4, span, sm, sm.y, st));
   float* skips[2] = {sa.act[4], sa.act[7]};
   int lds[2] = {a.K[4], a.K[7]};

@@ -22,6 +22,9 @@
 //   tc_wgrad_kernel  dW = dZ^T * H as wgmma with both operands MN-major straight from the images
 //                    the two kernels above left in HBM; split over rows, fp32 vector reductions
 //
+// Networks (TcNet, one row of g_kernels each): the plain mappings (6 / 4 layers), the atlas, the alpha network and the
+// position-encoded mappings (3 -> PE 1..10 -> 256 x {4,2} -> 2, use_positional_encoding_mapping1/2).
+//
 // Restates nn.Linear/ReLU/tanh/skip-concat forward+autograd of
 //   src/models/stage_1/implicit_neural_networks.py:62-81 for the two networks of
 //   src/stage1_neural_atlas.py:112-128.
@@ -115,7 +118,7 @@ int64_t tc_plan(const MlpShape& ms, const MlpShape& as, int64_t rows_map, int64_
                 TcPlan* out) {
   char* p = align_tc(base);
   TcLayout lay{};
-  plan_net(ms, rows_map, TcNet::Mapping6, p, &lay.map);
+  plan_net(ms, rows_map, tc_net_of(ms), p, &lay.map);
   plan_net(as, rows_atlas, TcNet::Atlas, p, &lay.atl);
   if (out) { out->base = base; out->bytes = p - base; out->rows_map = rows_map; out->rows_atlas = rows_atlas; }
   return p - base;
@@ -124,7 +127,7 @@ int64_t tc_plan(const MlpShape& ms, const MlpShape& as, int64_t rows_map, int64_
 static TcLayout layout_of(const TcStep& s) {
   char* p = align_tc(s.plan->base);
   TcLayout lay{};
-  plan_net(*s.ms, s.plan->rows_map, TcNet::Mapping6, p, &lay.map);
+  plan_net(*s.ms, s.plan->rows_map, tc_net_of(*s.ms), p, &lay.map);
   plan_net(*s.as, s.plan->rows_atlas, TcNet::Atlas, p, &lay.atl);
   return lay;
 }
@@ -376,6 +379,7 @@ struct FwdParams {
   float in_scale, in_shift;  // atlas: network input = x * in_scale + in_shift (0.5, 0.5 inside the loop: uv -> [0,1])
   int store_images;          // 0: inference (render / IMLP.forward without grad): no activation images, no flags
   int tanh_out;
+  int pe_freqs;              // 3-input PE-first networks: frequencies of the encoding (1..10, 6 columns each)
 };
 
 // =============================================================================================
@@ -384,8 +388,10 @@ struct FwdParams {
 // One 128-row tile walks through all layers on chip.  Per layer each consumer warpgroup runs the MMAs of its 64 rows
 // (A tile in shared memory, weight items from the ring), then its epilogue turns the accumulator registers into the next
 // layer's A operand (bias + ReLU + flag bits + 2-term split) in place and bulk-stores those rows to the activation image.
-// VAR (with ATLAS = true): 0 = the atlas network (2 inputs, 10 frequencies, skips at 4 and 7, 3 outputs), 1 = the alpha
-// network of the segmentation variant (3 inputs, 5 frequencies, no skips, 1 output, no input gradient)
+// ATLAS = true: the positional encoding feeds layer 0, which runs on the tensor cores.  VAR = 0: the atlas network (2
+// inputs, 10 frequencies, skips at 4 and 7, 3 outputs).  VAR > 0: the 3-input family (3 inputs, P.pe_freqs frequencies
+// in one 64-column chunk, no skips, VAR outputs, no input gradient): the alpha network of the segmentation variant
+// (NL = 8, VAR = 1, 5 frequencies) and the position-encoded mappings (NL = 6 or 4, VAR = 2).
 template <bool ATLAS, int NL = (ATLAS ? 8 : 6), int VAR = 0>
 __global__ void __launch_bounds__(TC_THREADS, 1) tc_fwd_kernel(const __grid_constant__ FwdParams P) {
   extern __shared__ __align__(1024) char smem_raw[];
@@ -395,10 +401,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_fwd_kernel(const __grid_cons
   constexpr int L = NL;                                   // mapping-shaped networks: 6 (stage-1 script) or 4 layers
   constexpr int FIRST_TC = ATLAS ? 0 : 1;
   constexpr int LAST_TC = L - 2;
-  constexpr bool ALPHA = ATLAS && VAR == 1;
-  constexpr bool SKIPS = ATLAS && !ALPHA;                 // PE chunk concatenated at layers 4 and L-1
-  constexpr int OUT = ATLAS ? (ALPHA ? 1 : 3) : 2;
+  constexpr bool PE3 = ATLAS && VAR > 0;                  // the 3-input family
+  constexpr bool SKIPS = ATLAS && !PE3;                   // PE chunk concatenated at layers 4 and L-1
+  constexpr int OUT = ATLAS ? (PE3 ? VAR : 3) : 2;
   constexpr int KLAST = SKIPS ? 296 : 256;
+  // real encoding columns of the 3-input family; the alpha network's 5 frequencies are part of its identity (tc_net_of)
+  const int pe_cols = VAR == 1 ? 30 : 6 * P.pe_freqs;
   setup_cta(sm);
   TileIter ti; ti.init(P.cap, P.n_groups, P.n_valid, P.flow_groups);
 
@@ -458,7 +466,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_fwd_kernel(const __grid_cons
         const int m = 64 * c.g + (task & 63), c8 = task >> 6;
         const int64_t row = (int64_t)gt * TM + m;
         float in[3] = {0.f, 0.f, 0.f};
-        if (ALPHA) {                                     // rows padded to 4 floats, like the mapping's
+        if (PE3) {                                       // rows padded to 4 floats, like the mapping's
           const float4 xv = *reinterpret_cast<const float4*>(P.x + row * 4);
           in[0] = xv.x * P.in_scale + P.in_shift; in[1] = xv.y * P.in_scale + P.in_shift; in[2] = xv.z * P.in_scale + P.in_shift;
         } else {
@@ -466,13 +474,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_fwd_kernel(const __grid_cons
           in[0] = uv.x * P.in_scale + P.in_shift; in[1] = uv.y * P.in_scale + P.in_shift;
         }
         float vals[8];
-        if (ALPHA) {
-          // column c = k*6 + r: r < 3 -> sin(x_r b_k), else cos(x_{r-3} b_k); 30 real columns
+        if (PE3) {
+          // column c = k*6 + r: r < 3 -> sin(x_r b_k), else cos(x_{r-3} b_k); pe_cols real columns
 #pragma unroll
           for (int i = 0; i < 8; ++i) {
             const int cc = c8 * 8 + i;
             float v = 0.f;
-            if (cc < 30) {
+            if (cc < pe_cols) {
               const int k = cc / 6, r = cc - k * 6;
               const float a = in[r < 3 ? r : r - 3] * pe_freq(k);
               v = r < 3 ? sinf(a) : cosf(a);
@@ -645,12 +653,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_bwd_kernel(const __grid_cons
   SmemMap<NST> sm; sm.init(smem_raw, 0, SMEM_BWD_CONST_FLOATS);
   const int warp = warp_uniform(), lane = threadIdx.x & 31;
   constexpr int L = NL;                                   // mapping-shaped networks: 6 (stage-1 script) or 4 layers
-  constexpr bool ALPHA = ATLAS && VAR == 1;
-  constexpr bool SKIPS = ATLAS && !ALPHA;                 // PE chunk concatenated at layers 4 and L-1
-  constexpr int OUT = ATLAS ? (ALPHA ? 1 : 3) : 2;
+  constexpr bool PE3 = ATLAS && VAR > 0;                  // the 3-input family (see tc_fwd_kernel)
+  constexpr bool SKIPS = ATLAS && !PE3;                   // PE chunk concatenated at layers 4 and L-1
+  constexpr int OUT = ATLAS ? (PE3 ? VAR : 3) : 2;
   constexpr int KLAST = SKIPS ? 296 : 256;
   constexpr int LOW = 1;                                  // dgrad layers L-2 .. 1 (atlas: + the dPE product)
-  constexpr bool HAS_DPE = ATLAS && !ALPHA;               // input gradient through the positional encoding
+  constexpr bool HAS_DPE = ATLAS && !PE3;                 // input gradient through the positional encoding
+  constexpr bool MAPPING = OUT == 2;                      // the 3 -> 2 mappings, with or without encoding
   // shared accumulators: bias gradients of layers 0..L-2; (mapping) dW0
   float* s_bacc = sm.cst;                                // (L-1)*256
   float* s_w0acc = s_bacc + (L - 1) * 256;               // mapping: 768
@@ -658,7 +667,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_bwd_kernel(const __grid_cons
   setup_cta(sm);
   TileIter ti; ti.init(P.cap, P.n_groups, P.n_valid, P.flow_groups);
   float s_g, inv_sg;
-  grad_scales(P.gmax_bits, !ATLAS, s_g, inv_sg);
+  grad_scales(P.gmax_bits, MAPPING, s_g, inv_sg);
 
   if (warp >= CONSUMER_WGS * 4) {
     setmaxnreg_dec<PRODUCER_REGS>();
@@ -1066,6 +1075,10 @@ TcNet tc_net_of(const MlpShape& s) {
   if (s.L == 4 && s.pe == 0 && s.in_dim == 3 && s.out_dim == 2 && no_skips) return TcNet::Mapping4;
   if (s.L == 8 && s.pe == 10 && s.in_dim == 2 && s.out_dim == 3 && skips_4_7) return TcNet::Atlas;
   if (s.L == 8 && s.pe == 5 && s.in_dim == 3 && s.out_dim == 1 && no_skips) return TcNet::Alpha;
+  // the encoding (6 P columns) must fit the one 64-column chunk of layer 0
+  const bool pe_chunk = s.pe >= 1 && s.pe <= 10;
+  if (s.L == 6 && pe_chunk && s.in_dim == 3 && s.out_dim == 2 && no_skips) return TcNet::MappingPE6;
+  if (s.L == 4 && pe_chunk && s.in_dim == 3 && s.out_dim == 2 && no_skips) return TcNet::MappingPE4;
   return TcNet::None;
 }
 
@@ -1076,6 +1089,8 @@ static const NetKernels g_kernels[] = {
     {tc_fwd_kernel<false, 4>, tc_bwd_kernel<false, 4>, KCfg<false, false>::SMEM, KCfg<false, true>::SMEM},
     {tc_fwd_kernel<true, 8, 0>, tc_bwd_kernel<true, 8, 0>, KCfg<true, false>::SMEM, KCfg<true, true>::SMEM},
     {tc_fwd_kernel<true, 8, 1>, tc_bwd_kernel<true, 8, 1>, KCfg<true, false>::SMEM, KCfg<true, true>::SMEM},
+    {tc_fwd_kernel<true, 6, 2>, tc_bwd_kernel<true, 6, 2>, KCfg<true, false>::SMEM, KCfg<true, true>::SMEM},
+    {tc_fwd_kernel<true, 4, 2>, tc_bwd_kernel<true, 4, 2>, KCfg<true, false>::SMEM, KCfg<true, true>::SMEM},
 };
 
 static int ensure_attrs() {
@@ -1114,8 +1129,16 @@ static FwdParams fill_fwd(const MlpShape& sh, const NetImages& im, const float* 
                           int groups, const int* n_valid) {
   FwdParams P{};
   P.x = x; P.y = y; P.params = params; P.img = im; P.cap = cap; P.n_groups = groups; P.n_valid = n_valid;
-  P.in_scale = 0.5f; P.in_shift = 0.5f; P.store_images = 1; P.tanh_out = 1; P.flow_groups = 0;
+  P.in_scale = 0.5f; P.in_shift = 0.5f; P.store_images = 1; P.tanh_out = 1; P.flow_groups = 0; P.pe_freqs = sh.pe;
   for (int l = 0; l < sh.L; ++l) { P.w_off[l] = sh.w_off[l]; P.b_off[l] = sh.b_off[l]; }
+  return P;
+}
+
+// The mapping of the fused step and of the render: a PE mapping encodes the raw (x, y, t) rows.
+static FwdParams fill_fwd_mapping(const MlpShape& sh, const NetImages& im, const float* x, float* y, const float* params,
+                                  int cap, int groups, const int* n_valid) {
+  FwdParams P = fill_fwd(sh, im, x, y, params, cap, groups, n_valid);
+  P.in_scale = 1.0f; P.in_shift = 0.0f;
   return P;
 }
 
@@ -1175,10 +1198,11 @@ struct WgProto { const char* a; int64_t a_term; int a_cols; const char* b; int64
 static void protos_for_net(WgProto* protos, int& np, const MlpShape& sh, const NetImages& im, float* g, TcNet net,
                            int groups) {
   const bool pe = tc_pe_first(net);
+  const int mapping = tc_net_is_mapping(net) ? 1 : 0;
   auto add = [&](const char* a, int64_t a_term, int a_cols, const char* b, int64_t b_term, int b_cols, float* out, int ld,
                  int n_rows, int n_cols) {
     protos[np++] = WgProto{a, a_term, a_cols, b, b_term, b_cols, out, ld, n_rows, n_cols, groups,
-                           (double)groups * step_cost(a_cols, b_cols), pe ? 0 : 1};
+                           (double)groups * step_cost(a_cols, b_cols), mapping};
   };
   for (int l = 1; l <= sh.L - 2; ++l)
     add(im.dz + (int64_t)l * im.slot_stride, im.term_stride, 256, im.act + (int64_t)(l - 1) * im.slot_stride,
@@ -1244,7 +1268,8 @@ static void apportion_items(WgradItems& wi, const WgProto* protos, int np, int c
 // graphs.  The render and ephemeral stand-alone calls (the IMLP class: a fresh workspace per call) upload them into
 // their workspace on every call, so a recycled workspace is harmless and the cache does not grow with every call.
 struct TabKey {
-  int dev; const void* ws; TcNet net;   // fused step: net = Atlas (mapping + atlas) or Mapping6 (pre-training)
+  int dev; const void* ws; TcNet net;   // fused step: net = Atlas (mapping + atlas) or the mapping's (pre-training)
+  int pe;                               // encoding frequencies of the (mapping) network: its tables depend on them
   bool step, with_bwd; int cap, groups, flow;
   const void* params; const void* grads;   // grads null: a stand-alone forward, served by the entry of its backward
 };
@@ -1265,7 +1290,7 @@ static TcTables* find_tables(const TabKey& k, bool add) {
   std::lock_guard<std::mutex> lock(g_tabs_mutex);
   for (TcTables* t : g_tabs) {
     TabKey& e = t->key;
-    if (e.dev == k.dev && e.ws == k.ws && e.net == k.net && e.step == k.step && e.with_bwd == k.with_bwd &&
+    if (e.dev == k.dev && e.ws == k.ws && e.net == k.net && e.pe == k.pe && e.step == k.step && e.with_bwd == k.with_bwd &&
         e.cap == k.cap && e.groups == k.groups && e.flow == k.flow && e.params == k.params &&
         (!k.grads || !e.grads || e.grads == k.grads)) {
       if (!e.grads) e.grads = k.grads;
@@ -1292,8 +1317,13 @@ template <class T> static int upload(const T& host, T** dst, bool own, cudaStrea
 }
 
 static TabKey step_key(const TcStep& s) {
-  return TabKey{current_device(), s.plan->base, s.y_atlas ? TcNet::Atlas : TcNet::Mapping6, true, true, s.cap, s.n_groups,
-                s.flow_groups, s.params, s.grads};
+  return TabKey{current_device(), s.plan->base, s.y_atlas ? TcNet::Atlas : tc_net_of(*s.ms), s.ms->pe, true, true, s.cap,
+                s.n_groups, s.flow_groups, s.params, s.grads};
+}
+
+static bool step_shapes_ok(const TcStep& s) {
+  const TcNet m = tc_net_of(*s.ms);
+  return (m == TcNet::Mapping6 || m == TcNet::MappingPE6) && tc_net_of(*s.as) == TcNet::Atlas;
 }
 
 // The weight images depend only on the parameters, so their preparation runs on a side stream, forked from the
@@ -1307,18 +1337,19 @@ int tc_begin_step(const TcStep& s, cudaStream_t st) {
   TcTables* tab = find_tables(step_key(s), true);
   B200_REQUIRE(tab, "too many distinct tensor-core workspaces in one process (%d)", MAX_TABLES);
   if (tab->n_wg < 0) {
-    B200_REQUIRE(tc_net_of(*s.ms) == TcNet::Mapping6 && tc_net_of(*s.as) == TcNet::Atlas,
-                 "tensor-core path is specialised to the two stage-1 networks");
+    B200_REQUIRE(step_shapes_ok(s), "tensor-core path is specialised to the two stage-1 networks (6-layer mapping, "
+                 "with or without positional encoding, and the atlas)");
     const TcLayout lay = layout_of(s);
+    const TcNet mnet = tc_net_of(*s.ms);
     const bool atlas = s.y_atlas != nullptr;
     // ---- forward / dgrad weight images (the atlas network only where it is evaluated: not in pre-training)
     g_pj.n = 0;
-    prep_jobs_for_net(g_pj, *s.ms, lay.map, s.params, TcNet::Mapping6, true);
+    prep_jobs_for_net(g_pj, *s.ms, lay.map, s.params, mnet, true);
     if (atlas) prep_jobs_for_net(g_pj, *s.as, lay.atl, s.params + s.ms->total, TcNet::Atlas, true);
     if (g_pj.n > MAX_PREP_JOBS) { set_error("table overflow"); return B200_ERR_INVALID; }
     // ---- wgrad items
     WgProto protos[32]; int np = 0;
-    protos_for_net(protos, np, *s.ms, lay.map, s.grads, TcNet::Mapping6, s.n_groups);
+    protos_for_net(protos, np, *s.ms, lay.map, s.grads, mnet, s.n_groups);
     if (atlas) protos_for_net(protos, np, *s.as, lay.atl, s.grads + s.ms->total, TcNet::Atlas, 3);
     g_wi.n = 0;
     apportion_items(g_wi, protos, np, s.cap, s.flow_groups);
@@ -1348,10 +1379,10 @@ int tc_step_forward(const TcStep& s, cudaStream_t st) {
   if (!sd.pending) B200_PROPAGATE(tc_begin_step(s, st));     // callers that did not fork earlier
   B200_CHECK_CUDA(cudaStreamWaitEvent(st, sd.join, 0));
   sd.pending = false;
-  FwdParams pm = fill_fwd(*s.ms, lay.map, s.x_map, s.uv, s.params, s.cap, s.n_groups, s.counters);
+  FwdParams pm = fill_fwd_mapping(*s.ms, lay.map, s.x_map, s.uv, s.params, s.cap, s.n_groups, s.counters);
   pm.flow_groups = s.flow_groups;
   timer_begin(TAG_MAP_FWD, st);
-  B200_PROPAGATE(launch_fwd(TcNet::Mapping6, pm, s.n_groups * (s.cap / TM), st));
+  B200_PROPAGATE(launch_fwd(tc_net_of(*s.ms), pm, s.n_groups * (s.cap / TM), st));
   timer_end(TAG_MAP_FWD, st);
   if (s.y_atlas) {
     const FwdParams pa = fill_fwd(*s.as, lay.atl, s.uv, s.y_atlas, s.params + s.ms->total, s.cap, 3, s.counters);
@@ -1394,7 +1425,7 @@ int tc_step_backward(const TcStep& s, cudaStream_t st) {
                           s.counters, gmax);
   pm.flow_groups = s.flow_groups;
   timer_begin(TAG_MAP_BWD, st);
-  B200_PROPAGATE(launch_bwd(TcNet::Mapping6, pm, s.n_groups * (s.cap / TM), st));
+  B200_PROPAGATE(launch_bwd(tc_net_of(*s.ms), pm, s.n_groups * (s.cap / TM), st));
   timer_end(TAG_MAP_BWD, st);
   timer_begin(TAG_WGRAD, st);
   g_last_wg = tab->d_wg; g_last_wg_n = min(tab->n_wg, sm_count());
@@ -1415,7 +1446,7 @@ static int64_t plan_infer(const MlpShape& ms, const MlpShape& as, char* base, Ne
   char* p = align_tc(base);
   *d_prep = reinterpret_cast<PrepJobs*>(carve_tc(p, sizeof(PrepJobs)));
   *im_map = NetImages{}; *im_atl = NetImages{};
-  plan_fwd_weights(ms, TcNet::Mapping6, p, im_map);
+  plan_fwd_weights(ms, tc_net_of(ms), p, im_map);
   plan_fwd_weights(as, TcNet::Atlas, p, im_atl);
   return p - base;
 }
@@ -1428,22 +1459,23 @@ int64_t tc_infer_workspace_bytes(const MlpShape& ms, const MlpShape& as) {
 int tc_infer_forward(const MlpShape& ms, const MlpShape& as, const float* params, const float* x_map, float* uv,
                      float* y, int64_t rows, char* ws, cudaStream_t st) {
   B200_PROPAGATE(ensure_attrs());
-  B200_REQUIRE(tc_net_of(ms) == TcNet::Mapping6 && tc_net_of(as) == TcNet::Atlas,
+  const TcNet mnet = tc_net_of(ms);
+  B200_REQUIRE((mnet == TcNet::Mapping6 || mnet == TcNet::MappingPE6) && tc_net_of(as) == TcNet::Atlas,
                "tensor-core path is specialised to the two stage-1 networks");
   B200_REQUIRE(rows > 0 && rows % TM == 0 && rows / TM < (1 << 24), "rows must be a positive multiple of %d", TM);
   NetImages im_map, im_atl; PrepJobs* d_prep;
   plan_infer(ms, as, ws, &im_map, &im_atl, &d_prep);
   // one prep launch for both networks; the job table is rebuilt in the workspace on every call (4 KB)
   g_pj.n = 0;
-  prep_jobs_for_net(g_pj, ms, im_map, params, TcNet::Mapping6, false);
+  prep_jobs_for_net(g_pj, ms, im_map, params, mnet, false);
   prep_jobs_for_net(g_pj, as, im_atl, params + ms.total, TcNet::Atlas, false);
   B200_PROPAGATE(upload(g_pj, &d_prep, false, st));
   tc_prep_kernel<<<g_pj.n * 4, 128, 0, st>>>(d_prep);
   B200_CHECK_LAUNCH();
   const int tiles = (int)(rows / TM);
-  FwdParams pm = fill_fwd(ms, im_map, x_map, uv, params, (int)rows, 1, nullptr);
+  FwdParams pm = fill_fwd_mapping(ms, im_map, x_map, uv, params, (int)rows, 1, nullptr);
   pm.store_images = 0;
-  B200_PROPAGATE(launch_fwd(TcNet::Mapping6, pm, tiles, st));
+  B200_PROPAGATE(launch_fwd(mnet, pm, tiles, st));
   FwdParams pa = fill_fwd(as, im_atl, uv, y, params + ms.total, (int)rows, 1, nullptr);
   pa.store_images = 0;
   return launch_fwd(TcNet::Atlas, pa, tiles, st);
@@ -1473,16 +1505,17 @@ int64_t tc_single_workspace_bytes(const MlpShape& sh, TcNet net, int64_t rows) {
 static int check_single(const MlpShape& sh, TcNet net, int64_t rows) {
   B200_PROPAGATE(ensure_attrs());
   B200_REQUIRE(net != TcNet::None && tc_net_of(sh) == net, "tensor-core IMLP: the shape is not the network it is "
-               "called for (mapping 3-256x{4,2}-2, atlas 2-PE10-256x6-3 with skips 4, 7, alpha 3-PE5-256x6-1)");
+               "called for (mapping 3-256x{4,2}-2, atlas 2-PE10-256x6-3 with skips 4, 7, alpha 3-PE5-256x6-1, "
+               "PE mapping 3-PE{1..10}-256x{4,2}-2)");
   B200_REQUIRE(rows > 0 && rows % TM == 0 && rows / TM < (1 << 20), "rows must be a positive multiple of %d", TM);
   return B200_OK;
 }
 
 // The tables of a stand-alone call: the cache entry of a persistent workspace, else the workspace's own slots.
-static TcTables* single_tables(TcTables& eph, TcNet net, const char* ws, int64_t rows, const float* params,
+static TcTables* single_tables(TcTables& eph, const MlpShape& sh, TcNet net, const char* ws, int64_t rows, const float* params,
                                const float* grads, bool training, bool persistent) {
   if (!persistent) return &eph;
-  return find_tables(TabKey{current_device(), ws, net, false, training, (int)rows, 1, 0, params, grads}, true);
+  return find_tables(TabKey{current_device(), ws, net, sh.pe, false, training, (int)rows, 1, 0, params, grads}, true);
 }
 
 // x: mapping [rows][4], atlas [rows][2] (network input itself).  y: [rows][out_dim].
@@ -1492,7 +1525,7 @@ int tc_single_forward(const MlpShape& sh, TcNet net, const float* params, const 
   SinglePlan pl{};
   plan_single(sh, net, rows, ws, &pl);
   TcTables eph{}; eph.d_prep = pl.d_prep;
-  TcTables* tab = single_tables(eph, net, ws, rows, params, nullptr, training, persistent);
+  TcTables* tab = single_tables(eph, sh, net, ws, rows, params, nullptr, training, persistent);
   B200_REQUIRE(tab, "too many distinct tensor-core workspaces in one process (%d)", MAX_TABLES);
   if (tab->n_prep < 0) {
     g_pj.n = 0;
@@ -1516,7 +1549,7 @@ int tc_single_backward(const MlpShape& sh, TcNet net, const float* params, float
   SinglePlan pl{};
   plan_single(sh, net, rows, ws, &pl);
   TcTables eph{}; eph.d_wg = pl.d_wg;
-  TcTables* tab = single_tables(eph, net, ws, rows, params, grads, true, persistent);
+  TcTables* tab = single_tables(eph, sh, net, ws, rows, params, grads, true, persistent);
   B200_REQUIRE(tab, "too many distinct tensor-core workspaces in one process (%d)", MAX_TABLES);
   if (tab->n_wg < 0) {
     WgProto protos[32]; int np = 0;

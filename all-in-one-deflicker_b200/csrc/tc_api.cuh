@@ -5,14 +5,21 @@
 namespace b200 {
 
 // The networks the tensor-core kernels are instantiated for: the stage-1 mapping (3-256x4-2), the background mapping of
-// the segmentation variant (3-256x2-2), the atlas (2-PE10-256x6-3, skips 4, 7) and the alpha network of the
-// segmentation variant (3-PE5-256x6-1).
-enum class TcNet { None, Mapping6, Mapping4, Atlas, Alpha };
+// the segmentation variant (3-256x2-2), the atlas (2-PE10-256x6-3, skips 4, 7), the alpha network of the
+// segmentation variant (3-PE5-256x6-1) and the position-encoded mappings (3-PE P-256x{4,2}-2, P = 1..10:
+// use_positional_encoding_mapping1/2 of the scripts' configs).
+enum class TcNet { None, Mapping6, Mapping4, Atlas, Alpha, MappingPE6, MappingPE4 };
 TcNet tc_net_of(const MlpShape& s);
-// atlas and alpha: the positional encoding feeds layer 0, which runs on the tensor cores
-inline bool tc_pe_first(TcNet n) { return n == TcNet::Atlas || n == TcNet::Alpha; }
+// atlas, alpha and the PE mappings: the positional encoding feeds layer 0, which runs on the tensor cores
+inline bool tc_pe_first(TcNet n) {
+  return n == TcNet::Atlas || n == TcNet::Alpha || n == TcNet::MappingPE6 || n == TcNet::MappingPE4;
+}
 // the atlas back-propagates to its input (uv) through the encoding; the other networks' inputs are pixel coordinates
 inline bool tc_net_has_dpe(TcNet n) { return n == TcNet::Atlas; }
+// the 3 -> 2 mappings: their gradients take the second gradient scale (max |dL/duv|)
+inline bool tc_net_is_mapping(TcNet n) {
+  return n == TcNet::Mapping6 || n == TcNet::Mapping4 || n == TcNet::MappingPE6 || n == TcNet::MappingPE4;
+}
 
 // Buffers of the tensor-core path, carved from the caller's workspace (see mlp_tc.cu).
 struct TcPlan {
@@ -21,6 +28,8 @@ struct TcPlan {
   int64_t rows_map = 0, rows_atlas = 0;
 };
 
+// The fused step and the render take the 6-layer mapping, with or without positional encoding (tc_net_of(ms) is
+// Mapping6 or MappingPE6), and the atlas.
 struct TcStep {
   const MlpShape* ms; const MlpShape* as;
   const TcPlan* plan;

@@ -68,7 +68,8 @@ class IMLP(nn.Module):
         self._w_off, self._b_off, self._total = A.mlp_layout(self._desc)
         # architectures of the stage-1 scripts with wgmma kernels (the library decides): 1 = mapping-shaped
         # (3 -> 256 x {2,4} -> 2, no encoding), 2 = atlas (2 -> PE 10 -> 256 x 6 -> 3, skips 4 and 7), 3 = alpha
-        # (3 -> PE 5 -> 256 x 6 -> 1), 0 = fp32 kernels only
+        # (3 -> PE 5 -> 256 x 6 -> 1), 4 = position-encoded mapping (3 -> PE 1..10 -> 256 x {2,4} -> 2), 0 = fp32
+        # kernels only
         self._tc_arch = max(0, int(N.lib().b200_mlp_tc_architecture(C.byref(self._desc))))
         # one flat fp32 buffer in the library's layout; the per-layer tensors are views of it
         self.flat = nn.Parameter(torch.zeros(self._total))
@@ -102,7 +103,7 @@ class IMLP(nn.Module):
     def _precision(self, input_needs_grad: bool) -> int:
         """Tensor cores (B200_PREC_TC: 2-term fp16 operands, fp32 accumulation — DESIGN.md §3) whenever the
         architecture has the fused kernels and the device is sm_90; `B200_IMLP_PRECISION=fp32|tc` overrides.  The
-        mapping / alpha kernels produce no input gradient (their inputs are pixel coordinates)."""
+        mapping (codes 1, 4) / alpha kernels produce no input gradient (their inputs are pixel coordinates)."""
         import os
         want = os.environ.get("B200_IMLP_PRECISION", "auto")
         ok = self._tc_arch != 0 and bool(N.lib().b200_device_supports_tc()) and not (self._tc_arch != 2 and input_needs_grad)

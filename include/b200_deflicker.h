@@ -156,12 +156,25 @@ typedef struct B200AtlasConfig {
 int64_t b200_atlas_param_floats(void);   /* mapping block followed by atlas block, padded */
 int64_t b200_atlas_workspace_bytes(const B200AtlasConfig* cfg);
 
+/* The mapping network of the script is a config choice (src/stage1_neural_atlas.py:112-119):
+ * use_positional_encoding_mapping1 puts a positional encoding of number_of_positional_encoding_mapping1
+ * frequencies in front of it.  Every atlas-step entry point has a `_for` form that takes the mapping
+ * descriptor: 3 -> 256 x 4 -> 2 (6 layers, no skips, tanh), on the raw (x, y, t) (pe_freqs = 0) or on
+ * their encoding (pe_freqs 1..10; b200_mlp_tc_architecture 1 or 4).  The forms without `_for` are the
+ * default mapping (pe_freqs = 0).  The parameter buffer is the mapping block (b200_mlp_layout of
+ * `mapping`) followed by the atlas block; b200_atlas_param_floats_for returns -1 for another mapping. */
+int64_t b200_atlas_param_floats_for(const B200MlpDesc* mapping);
+int64_t b200_atlas_workspace_bytes_for(const B200AtlasConfig* cfg, const B200MlpDesc* mapping);
+
 /* indices: `batch` int64 pixel-table indices n -> (x = n % W, y = (n / W) % H, t = n / (H*W)),
  * identical on every rank; rows whose frame is not resident are skipped.  grads (same layout
  * as params) and losses are overwritten. */
 int b200_atlas_loss_grad(const B200AtlasConfig* cfg, const B200Video* video,
                          const int64_t* indices, const float* params, float* grads,
                          float* losses, void* ws, int64_t ws_bytes, void* stream);
+int b200_atlas_loss_grad_for(const B200AtlasConfig* cfg, const B200MlpDesc* mapping,
+                             const B200Video* video, const int64_t* indices, const float* params,
+                             float* grads, float* losses, void* ws, int64_t ws_bytes, void* stream);
 
 /* Test / debugging aid: byte offsets (from `ws`) of the step's intermediate buffers inside the
  * workspace, for the configuration `cfg`: [0] counters (int32: n_local, n_fwd, n_bwd, ...),
@@ -169,6 +182,8 @@ int b200_atlas_loss_grad(const B200AtlasConfig* cfg, const B200Video* video,
  * [cap][12], [4] d_uv, [5] d_y, [6] mapping output uv [groups][cap][2], [7] atlas output
  * [3][cap][3].  cap = batch rounded up to 128. */
 int b200_atlas_workspace_offsets(const B200AtlasConfig* cfg, const void* ws, int64_t* offsets);
+int b200_atlas_workspace_offsets_for(const B200AtlasConfig* cfg, const B200MlpDesc* mapping,
+                                     const void* ws, int64_t* offsets);
 
 /* One pre_train_mapping step (src/models/stage_1/unwrap_utils.py:182-195): rows ys / columns
  * xs (int64[batch]) of frame `frame`; gradients of the mapping block only; loss -> losses[0]. */
@@ -176,6 +191,10 @@ int b200_pretrain_loss_grad(const B200AtlasConfig* cfg, int32_t larger_dim, int3
                             int32_t frame, const int64_t* ys, const int64_t* xs,
                             const float* params, float* grads, float* losses, void* ws,
                             int64_t ws_bytes, void* stream);
+int b200_pretrain_loss_grad_for(const B200AtlasConfig* cfg, const B200MlpDesc* mapping,
+                                int32_t larger_dim, int32_t T, int32_t frame, const int64_t* ys,
+                                const int64_t* xs, const float* params, float* grads,
+                                float* losses, void* ws, int64_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Input producer on the device — replaces the per-frame / per-pair arithmetic of
@@ -280,6 +299,11 @@ int64_t b200_render_workspace_bytes(int64_t pixels);
 int b200_render(const float* params, int32_t H, int32_t W, int32_t T, int32_t frame,
                 int64_t pix_begin, int64_t pix_end, float* rgb, uint8_t* rgb_u8, int precision,
                 void* ws, int64_t ws_bytes, void* stream);
+/* the same with the mapping of b200_atlas_param_floats_for */
+int64_t b200_render_workspace_bytes_for(const B200MlpDesc* mapping, int64_t pixels);
+int b200_render_for(const B200MlpDesc* mapping, const float* params, int32_t H, int32_t W,
+                    int32_t T, int32_t frame, int64_t pix_begin, int64_t pix_end, float* rgb,
+                    uint8_t* rgb_u8, int precision, void* ws, int64_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Segmentation variant of the loop — replaces src/stage1_neural_atlas_seg.py:207-315 +
@@ -315,8 +339,10 @@ typedef struct B200SegConfig {
 
 /* Which tensor-core kernels serve a network shape: 1 = mapping-shaped (3 -> 256 x {2,4} -> 2, no
  * encoding: both mappings of the scripts), 2 = the atlas network (2 -> PE 10 -> 256 x 6 -> 3, skips 4
- * and 7), 3 = the alpha network of the segmentation variant (3 -> PE 5 -> 256 x 6 -> 1), 0 = any
- * other shape (fp32 kernels only), -1 = invalid descriptor */
+ * and 7), 3 = the alpha network of the segmentation variant (3 -> PE 5 -> 256 x 6 -> 1), 4 = a
+ * position-encoded mapping (3 -> PE P -> 256 x {2,4} -> 2, P = 1..10, no skips: the mappings with
+ * use_positional_encoding_mapping1/2), 0 = any other shape (fp32 kernels only), -1 = invalid
+ * descriptor.  Codes 1 and 4 have no input gradient on the tensor cores. */
 int b200_mlp_tc_architecture(const B200MlpDesc* d);
 
 /* parameters / gradients / Adam moments are ONE flat buffer: the four networks in the order of
