@@ -20,7 +20,8 @@
 //   tc_bwd_kernel    same structure for dL/dz: tanh', last layer on CUDA cores, hidden layers as
 //                    dZ * W (B = W^T images), ReLU mask from 1-bit flags, bias gradients by shuffle column sums
 //   tc_wgrad_kernel  dW = dZ^T * H as wgmma with both operands MN-major straight from the images
-//                    the two kernels above left in HBM; split over rows, fp32 vector reductions
+//                    the two kernels above left in HBM; split over rows, fp32 vector reductions; clusters of two CTAs
+//                    split the 256-wide operand and multicast the other, so each image byte is read once
 //
 // Networks (TcNet, one row of g_kernels each): the plain mappings (6 / 4 layers), the atlas, the alpha network and the
 // position-encoded mappings (3 -> PE 1..10 -> 256 x {4,2} -> 2, use_positional_encoding_mapping1/2).
@@ -881,85 +882,81 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_bwd_kernel(const __grid_cons
 // weight gradients:  dW[n][k] += sum_rows dZ[row][n] * H[row][k]
 // =============================================================================================
 struct WgradItem {
-  const char* a_img;      // dZ image, hi (lo at +a_term): 256 wide [tile][4 atoms][16 KB] or 64 wide [tile][16 KB]
-  const char* b_img;      // input image, hi (lo at +b_term): same two shapes
+  const char* a_img;      // M-side image, hi (lo at +a_term): 256 wide [tile][4 atoms][16 KB] or 64 wide [tile][16 KB]
+  const char* b_img;      // N-side image, hi (lo at +b_term): same two shapes
   int64_t a_term, b_term;
-  float* out; int ld_out; // fp32 dW block [a_cols rows][ld_out], columns [0, n_cols)
-  int a_cols;             // 256: four M=64 blocks;  64: one M=64 block (output-layer gradient, n_rows real rows)
-  int b_cols;             // 256 (four passes of 64 columns) or 64
-  int n_rows, n_cols;     // real rows / columns to write
+  float* out; int ld_out; // fp32 dW block [n_rows][ld_out], columns [0, n_cols)
+  int a_cols;             // 256: 128 columns per CTA of the pair, 64 per consumer warpgroup;  64: the 64x64 shape
+  int b_cols;             // the MMA N: 256 or 64
+  int transposed;         // 1: the M side indexes dW columns (output layer: M = last activation, N = its dZ)
+  int n_rows, n_cols;     // real rows / columns of dW to write
   int cap, n_groups;      // row geometry of the network this item belongs to
-  int split, n_split;     // this CTA's share of the live tiles
+  int split, n_split;     // this cluster's share of the live tiles
   int mapping;            // 1: gradients of the mapping network (second gradient scale)
   int flow_groups;        // row geometry: compacted flow-match groups (mapping batch of the loop)
 };
 constexpr int MAX_WGRAD_ITEMS = 768;
 struct WgradItems { WgradItem it[MAX_WGRAD_ITEMS]; int n; long long cycles[256]; };   // cycles: per-CTA duration (diagnostics)
 
-constexpr int WG_STAGE = 65536;          // 32 rows: A hi 16K | A lo 16K | B hi 16K | B lo 16K, each [atom][4 groups][1 KB]
-constexpr int WG_NSTAGE = 3;
+constexpr int WG_CLUSTER = 2;            // CTAs per cluster: the pair shares (multicasts) the N-side operand
+constexpr int WG_STAGE = 49152;          // 32 rows: A hi 8K | A lo 8K | B hi 16K | B lo 16K, each [atom][4 groups][1 KB]
+constexpr int WG_NSTAGE = 4;
 constexpr int WG_SMEM = WG_NSTAGE * WG_STAGE + 256;
 constexpr int WG_THREADS = TC_THREADS;
+constexpr int WG_EMPTY_ARRIVALS = WG_CLUSTER * EMPTY_ARRIVALS;   // every consumer warp of the pair frees every slot
 
-// MMAs of one 32-row step for this warpgroup's M blocks (MN-major operands: LBO = atom stride, SBO = 8-row group).
-// NMB = 2: a 256-row dW block, warpgroup g owns M blocks 2g, 2g+1;  NMB = 1: a 64-row block (output layer), both
-// warpgroups compute it (keeps the MMA sequence free of warpgroup-dependent branches), warpgroup 0 stores it.
-template <int NB, int NMB>
-__device__ __forceinline__ void wgrad_step(float (&acc)[NMB][NB / 2], uint32_t sb, int g, uint32_t& scale) {
-#pragma unroll
-  for (int ks = 0; ks < 2; ++ks) {                      // 16 rows = 2 groups per MMA
-    const uint64_t b_hi = make_desc(sb + 32768 + ks * 2048, 4096, 1024);
-    const uint64_t b_lo = make_desc(sb + 49152 + ks * 2048, 4096, 1024);
-#pragma unroll
-    for (int mb = 0; mb < NMB; ++mb) {
-      const uint32_t a = sb + (NMB == 2 ? (2 * g + mb) * 4096 : 0) + ks * 2048;
-      const uint64_t a_hi = make_desc(a, 4096, 1024), a_lo = make_desc(a + 16384, 4096, 1024);
-      if constexpr (NB == 128) {
-        wgmma_n128<1, 1>(acc[mb], a_hi, b_hi, scale);
-        wgmma_n128<1, 1>(acc[mb], a_hi, b_lo, 1u);
-        wgmma_n128<1, 1>(acc[mb], a_lo, b_hi, 1u);
-      } else {
-        wgmma_n64<1, 1>(acc[mb], a_hi, b_hi, scale);
-        wgmma_n64<1, 1>(acc[mb], a_hi, b_lo, 1u);
-        wgmma_n64<1, 1>(acc[mb], a_lo, b_hi, 1u);
-      }
-    }
-    scale = 1u;
-  }
-}
-
-template <int NB, int NMB>
-__device__ __forceinline__ void wgrad_pass(const WgradItem& W, int n_steps, int n0, char* stage, uint64_t* full,
-                                           uint64_t* empty, uint32_t& gs, const Consumer& c, float inv) {
-  float acc[NMB][NB / 2];
+// One work unit of this warpgroup: the M block at m0 of dW (or of dW^T), all N columns, accumulated over the unit's
+// 32-row steps, then flushed with fp32 atomics.  MN-major operands: LBO = atom stride, SBO = 8-row group.
+// HALF_K (the 64x64 shape): both warpgroups own the same 64 x 64 block, warpgroup g takes rows 16g..16g+15 of each step,
+// so the MMA sequence has no warpgroup-dependent branch and no MMA is run twice; both flush.
+template <int NB, bool HALF_K>
+__device__ __forceinline__ void wgrad_unit(const WgradItem& W, int n_steps, int m0, char* stage, uint64_t* full,
+                                           uint64_t* empty, uint32_t peer_empty, uint32_t& gs, const Consumer& c,
+                                           float inv) {
+  float acc[NB / 2];
   uint32_t scale = 0u;
   int pending = -1;
   for (int s = 0; s < n_steps; ++s, ++gs) {
     const int slot = gs % WG_NSTAGE;
     mbar_wait(&full[slot], (gs / WG_NSTAGE) & 1);
+    const uint32_t sb = smem_u32(stage + slot * WG_STAGE);
     wgmma_fence();
-    wgrad_step<NB, NMB>(acc, smem_u32(stage + slot * WG_STAGE), c.g, scale);
+#pragma unroll
+    for (int kk = 0; kk < (HALF_K ? 1 : 2); ++kk) {       // 16 rows = 2 groups per MMA
+      const int ks = HALF_K ? c.g : kk;
+      const uint32_t a = sb + (HALF_K ? 0 : c.g * 4096) + ks * 2048;
+      const uint64_t a_hi = make_desc(a, 4096, 1024), a_lo = make_desc(a + 8192, 4096, 1024);
+      const uint64_t b_hi = make_desc(sb + 16384 + ks * 2048, 4096, 1024);
+      const uint64_t b_lo = make_desc(sb + 32768 + ks * 2048, 4096, 1024);
+      if constexpr (NB == 256) {
+        wgmma_n256<1, 1>(acc, a_hi, b_hi, scale);
+        wgmma_n256<1, 1>(acc, a_hi, b_lo, 1u);
+        wgmma_n256<1, 1>(acc, a_lo, b_hi, 1u);
+      } else {
+        wgmma_n64<1, 1>(acc, a_hi, b_hi, scale);
+        wgmma_n64<1, 1>(acc, a_hi, b_lo, 1u);
+        wgmma_n64<1, 1>(acc, a_lo, b_hi, 1u);
+      }
+      scale = 1u;
+    }
     wgmma_commit();
     wgmma_wait<1>();
-    if (pending >= 0 && c.warp_leader) mbar_arrive(&empty[pending]);
+    if (pending >= 0 && c.warp_leader) { mbar_arrive(&empty[pending]); mbar_arrive_remote(peer_empty + pending * 8); }
     pending = slot;
   }
   wgmma_wait<0>();
+  acc_fence(acc);
+  if (pending >= 0 && c.warp_leader) { mbar_arrive(&empty[pending]); mbar_arrive_remote(peer_empty + pending * 8); }
 #pragma unroll
-  for (int mb = 0; mb < NMB; ++mb) acc_fence(acc[mb]);
-  if (pending >= 0 && c.warp_leader) mbar_arrive(&empty[pending]);
-  if (NMB == 1 && c.g != 0) return;
-#pragma unroll
-  for (int mb = 0; mb < NMB; ++mb) {
-#pragma unroll
-    for (int rr = 0; rr < 2; ++rr) {
-      const int n = (NMB == 2 ? (2 * c.g + mb) * 64 : 0) + 16 * c.w4 + (c.lane >> 2) + 8 * rr;   // dW row
-      if (NMB == 1 && n >= W.n_rows) continue;
-      float* orow = W.out + (int64_t)n * W.ld_out;
+  for (int rr = 0; rr < 2; ++rr) {
+    const int m = m0 + 16 * c.w4 + (c.lane >> 2) + 8 * rr;
+    if (!W.transposed) {                                  // dW row m, columns 8i + 2q + {0, 1}
+      if (m >= W.n_rows) continue;
+      float* orow = W.out + (int64_t)m * W.ld_out;
 #pragma unroll
       for (int i = 0; i < NB / 8; ++i) {
-        const int k = n0 + 8 * i + 2 * c.q;
-        const float v0 = acc[mb][4 * i + 2 * rr] * inv, v1 = acc[mb][4 * i + 2 * rr + 1] * inv;
+        const int k = 8 * i + 2 * c.q;
+        const float v0 = acc[4 * i + 2 * rr] * inv, v1 = acc[4 * i + 2 * rr + 1] * inv;
         if (((W.ld_out & 1) == 0) && k + 1 < W.n_cols) {
           atomicAdd(reinterpret_cast<float2*>(orow + k), make_float2(v0, v1));
         } else {
@@ -967,61 +964,91 @@ __device__ __forceinline__ void wgrad_pass(const WgradItem& W, int n_steps, int 
           if (k + 1 < W.n_cols) atomicAdd(orow + k + 1, v1);
         }
       }
+    } else {                                              // dW column m, rows 8i + 2q + {0, 1}
+      if (m >= W.n_cols) continue;
+#pragma unroll
+      for (int i = 0; i < NB / 8; ++i) {
+        const int n = 8 * i + 2 * c.q;
+        if (n < W.n_rows) atomicAdd(W.out + (int64_t)n * W.ld_out + m, acc[4 * i + 2 * rr] * inv);
+        if (n + 1 < W.n_rows) atomicAdd(W.out + (int64_t)(n + 1) * W.ld_out + m, acc[4 * i + 2 * rr + 1] * inv);
+      }
     }
   }
 }
 
-// Work units ("items" = one dW GEMM restricted to a share of the rows) are dealt round-robin: CTA b processes items b,
-// b + grid, b + 2 grid, ... (WG_UNITS_PER_CTA of them; the host builds the list).  A 256-column B operand is covered in
-// four passes of 64 columns, each re-reading A: a wider accumulator leaves too few registers for the asynchronous wgmma
-// pipeline.  The operand ring runs across passes and units; the accumulator is flushed (vector atomics) after every pass.
-__global__ void __launch_bounds__(WG_THREADS, 1)
+// The unit's share [t_begin, t_end) of the live tiles.  32-bit: tiles < 2^21 and n_split <= MAX_WGRAD_ITEMS.
+__device__ __forceinline__ void unit_tiles(const WgradItem& W, const TileIter& ti, int& t_begin, int& t_end) {
+  t_begin = ti.total * W.split / W.n_split;
+  t_end = ti.total * (W.split + 1) / W.n_split;
+}
+
+// Work units ("items" = one dW GEMM restricted to a share of the rows) are dealt round-robin to clusters of two CTAs:
+// cluster b processes items b, b + clusters, ... (WG_UNITS_PER_CLUSTER of them; the host builds the list).  Both CTAs
+// of a cluster run the same rows and each reads its half of the M-side operand; the N-side operand is read once per
+// cluster, each CTA multicasting half of it into both CTAs' rings, so every operand byte leaves HBM once.  The 64x64
+// shape has no 256-wide side to split: the pair splits its row steps instead.  A ring slot is refilled only after the
+// consumers of both CTAs have released it (the partner's producer writes into it), so both CTAs step through the same
+// slot sequence.
+__global__ void __cluster_dims__(WG_CLUSTER, 1, 1) __launch_bounds__(WG_THREADS, 1)
 tc_wgrad_kernel(const WgradItems* __restrict__ items, const int* __restrict__ n_valid, const int* __restrict__ gmax_bits) {
   extern __shared__ __align__(1024) char smem_raw[];
   char* stage = smem_raw;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + WG_NSTAGE * WG_STAGE);
   uint64_t* empty = full + WG_NSTAGE;
   const int warp = warp_uniform(), lane = threadIdx.x & 31;
+  const int rank = (int)cluster_ctarank(), cluster = blockIdx.x / WG_CLUSTER, n_clusters = gridDim.x / WG_CLUSTER;
   if (threadIdx.x == 0) {
     if (smem_u32(stage) & 1023u) __trap();   // the swizzled operand layouts need 1024-byte alignment
-    for (int i = 0; i < WG_NSTAGE; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], EMPTY_ARRIVALS); }
+    for (int i = 0; i < WG_NSTAGE; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], WG_EMPTY_ARRIVALS); }
     fence_barrier_init();
   }
-  __syncthreads();
+  cluster_sync();                            // the partner's barriers are initialised before any remote operation
   const int n_items = items->n;
   const long long t_start = clock64();
 
   if (warp >= CONSUMER_WGS * 4) {
     setmaxnreg_dec<PRODUCER_REGS>();
     if (warp == CONSUMER_WGS * 4 && lane == 0) {
-      uint32_t gs = 0;                                  // running stage counter across units
-      for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
+      uint32_t gs = 0;                                  // running stage counter across units, equal in both CTAs
+      for (int it = cluster; it < n_items; it += n_clusters) {
         const WgradItem W = items->it[it];
         TileIter ti; ti.init(W.cap, W.n_groups, n_valid, W.flow_groups);
-        const int t_begin = (int)((int64_t)ti.total * W.split / W.n_split);
-        const int t_end = (int)((int64_t)ti.total * (W.split + 1) / W.n_split);
+        int t_begin, t_end; unit_tiles(W, ti, t_begin, t_end);
         const int a_atoms = W.a_cols / 64, b_atoms = W.b_cols / 64;
-        const int passes = b_atoms, pass_atoms = 1;     // one 64-column atom of B per pass
-        const int n_steps = (t_end - t_begin) * 4;     // 32-row steps
-        for (int ps = 0; ps < passes; ++ps)
-          for (int s = 0; s < n_steps; ++s, ++gs) {
-            const int slot = gs % WG_NSTAGE;
-            mbar_wait(&empty[slot], ((gs / WG_NSTAGE) & 1) ^ 1);
-            const int gt = ti.global_tile(t_begin + (s >> 2));
-            const int ch = s & 3;                      // 32-row chunk = groups 4ch .. 4ch+3 of every atom block
-            char* dst = stage + slot * WG_STAGE;
-            mbar_expect_tx(&full[slot], 2 * 4096 * (a_atoms + pass_atoms));
-            const char* a = W.a_img + (int64_t)gt * a_atoms * ATOM_BYTES + ch * 4096;
-            for (int j = 0; j < a_atoms; ++j) {
-              bulk_g2s(dst + j * 4096, a + (int64_t)j * ATOM_BYTES, 4096, &full[slot]);
-              bulk_g2s(dst + 16384 + j * 4096, a + W.a_term + (int64_t)j * ATOM_BYTES, 4096, &full[slot]);
-            }
-            const char* b = W.b_img + (int64_t)gt * b_atoms * ATOM_BYTES + ch * 4096 + (int64_t)ps * pass_atoms * ATOM_BYTES;
-            for (int j = 0; j < pass_atoms; ++j) {
-              bulk_g2s(dst + 32768 + j * 4096, b + (int64_t)j * ATOM_BYTES, 4096, &full[slot]);
-              bulk_g2s(dst + 49152 + j * 4096, b + W.b_term + (int64_t)j * ATOM_BYTES, 4096, &full[slot]);
-            }
+        const bool split_rows = W.a_cols == 64;         // 64x64: CTA r takes the r-th half of the 32-row steps
+        const int n_steps = (t_end - t_begin) * 4;     // a multiple of 4: the halves are equal
+        const int s0 = split_rows ? rank * (n_steps / 2) : 0, s1 = split_rows ? s0 + n_steps / 2 : n_steps;
+        const uint32_t tx = split_rows ? 16384 : 16384 + 2 * 4096 * b_atoms;
+        for (int s = s0; s < s1; ++s, ++gs) {
+          const int slot = gs % WG_NSTAGE;
+          mbar_wait(&empty[slot], ((gs / WG_NSTAGE) & 1) ^ 1);
+          const int gt = ti.global_tile(t_begin + (s >> 2));
+          const int ch = s & 3;                        // 32-row chunk = groups 4ch .. 4ch+3 of every atom block
+          char* dst = stage + slot * WG_STAGE;
+          mbar_expect_tx(&full[slot], tx);
+          const char* a = W.a_img + (int64_t)gt * a_atoms * ATOM_BYTES + ch * 4096;
+          const char* b = W.b_img + (int64_t)gt * b_atoms * ATOM_BYTES + ch * 4096;
+          if (split_rows) {
+            bulk_g2s(dst, a, 4096, &full[slot]);
+            bulk_g2s(dst + 8192, a + W.a_term, 4096, &full[slot]);
+            bulk_g2s(dst + 16384, b, 4096, &full[slot]);
+            bulk_g2s(dst + 32768, b + W.b_term, 4096, &full[slot]);
+            continue;
           }
+          for (int j = 0; j < 2; ++j) {                // this CTA's two atoms of A
+            const int64_t off = (int64_t)(2 * rank + j) * ATOM_BYTES;
+            bulk_g2s(dst + j * 4096, a + off, 4096, &full[slot]);
+            bulk_g2s(dst + 8192 + j * 4096, a + W.a_term + off, 4096, &full[slot]);
+          }
+          if (b_atoms == 4) {                          // B: atoms 2r, 2r+1 of both terms, into both CTAs
+            for (int j = 2 * rank; j < 2 * rank + 2; ++j) {
+              bulk_g2s_multicast(dst + 16384 + j * 4096, b + (int64_t)j * ATOM_BYTES, 4096, &full[slot], 0x3);
+              bulk_g2s_multicast(dst + 32768 + j * 4096, b + W.b_term + (int64_t)j * ATOM_BYTES, 4096, &full[slot], 0x3);
+            }
+          } else {                                     // B: one atom, rank 0 sends the hi term, rank 1 the lo term
+            bulk_g2s_multicast(dst + 16384 + rank * 16384, b + rank * W.b_term, 4096, &full[slot], 0x3);
+          }
+        }
       }
     }
   } else {
@@ -1030,24 +1057,24 @@ tc_wgrad_kernel(const WgradItems* __restrict__ items, const int* __restrict__ n_
     float s_gm, inv_gm, s_ga, inv_ga;
     grad_scales(gmax_bits, true, s_gm, inv_gm);
     grad_scales(gmax_bits, false, s_ga, inv_ga);
+    const uint32_t peer_empty = mapa_shared(smem_u32(empty), rank ^ 1);
     uint32_t gs = 0;
-    for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
+    for (int it = cluster; it < n_items; it += n_clusters) {
       const WgradItem W = items->it[it];
       TileIter ti; ti.init(W.cap, W.n_groups, n_valid, W.flow_groups);
-      const int t_begin = (int)((int64_t)ti.total * W.split / W.n_split);
-      const int t_end = (int)((int64_t)ti.total * (W.split + 1) / W.n_split);
+      int t_begin, t_end; unit_tiles(W, ti, t_begin, t_end);
       const int n_steps = (t_end - t_begin) * 4;
       if (n_steps == 0) continue;
       const float inv = (W.mapping ? inv_gm : inv_ga) * (1.0f / S_ACT);
-      // 64 output columns per pass: the accumulator (two 64 x 64 blocks) stays in registers next to the pipeline
-      for (int n0 = 0; n0 < W.b_cols; n0 += 64) {
-        if (W.a_cols == 256) wgrad_pass<64, 2>(W, n_steps, n0, stage, full, empty, gs, c, inv);
-        else wgrad_pass<64, 1>(W, n_steps, n0, stage, full, empty, gs, c, inv);
-      }
+      const int m0 = rank * 128 + c.g * 64;
+      if (W.a_cols == 64) wgrad_unit<64, true>(W, n_steps / 2, 0, stage, full, empty, peer_empty, gs, c, inv);
+      else if (W.b_cols == 256) wgrad_unit<256, false>(W, n_steps, m0, stage, full, empty, peer_empty, gs, c, inv);
+      else wgrad_unit<64, false>(W, n_steps, m0, stage, full, empty, peer_empty, gs, c, inv);
     }
   }
   __syncthreads();
   if (threadIdx.x == 0 && blockIdx.x < 256) const_cast<WgradItems*>(items)->cycles[blockIdx.x] = clock64() - t_start;
+  cluster_sync();                            // no CTA exits while its partner may still arrive on its barriers
 }
 
 // =============================================================================================
@@ -1063,6 +1090,8 @@ static int sm_count() {
   }
   return g_sm_count;
 }
+
+static int current_device() { int d = 0; cudaGetDevice(&d); return d; }
 
 TcNet tc_net_of(const MlpShape& s) {
   if (s.hidden != HID) return TcNet::None;
@@ -1093,6 +1122,9 @@ static const NetKernels g_kernels[] = {
     {tc_fwd_kernel<true, 4, 2>, tc_bwd_kernel<true, 4, 2>, KCfg<true, false>::SMEM, KCfg<true, true>::SMEM},
 };
 
+// Clusters of the weight-gradient kernel that fit on each device at once (set by ensure_attrs)
+static int g_wg_clusters[64];
+
 static int ensure_attrs() {
   // cudaFuncSetAttribute is per device: remember which devices of this process have been configured
   static bool done_dev[64] = {};
@@ -1106,6 +1138,10 @@ static int ensure_attrs() {
     B200_CHECK_CUDA(cudaFuncSetAttribute(k.bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, k.bwd_smem));
   }
   B200_CHECK_CUDA(cudaFuncSetAttribute(tc_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WG_SMEM));
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(WG_CLUSTER); cfg.blockDim = dim3(WG_THREADS); cfg.dynamicSmemBytes = WG_SMEM;
+  B200_CHECK_CUDA(cudaOccupancyMaxActiveClusters(&g_wg_clusters[dev], tc_wgrad_kernel, &cfg));
+  B200_REQUIRE(g_wg_clusters[dev] > 0, "the weight-gradient kernel's %d-CTA clusters do not fit on device %d", WG_CLUSTER, dev);
   done = true;
   return B200_OK;
 }
@@ -1183,16 +1219,18 @@ static void prep_jobs_for_net(PrepJobs& pj, const MlpShape& sh, const NetImages&
   }
 }
 
-// wgrad work list.  CTAs are balanced by a per-32-row-step cost of each GEMM, indexed by the image columns of its two
+// wgrad work list.  Units are balanced by a per-32-row-step cost of each GEMM, indexed by the image columns of its two
 // operands (a_cols + b_cols): narrow steps cost more than their bytes (barrier round trips and M = 64 MMAs do not
-// shrink).  On an H100 (700 W) these weights gave 1.07 ms for the kernel at the benchmark shape; plain loaded-column counts
-// over the 64-column passes gave 1.39 ms.
+// shrink).  The weights are those of the one-CTA-per-SM kernel that re-read A per 64-column pass; kept, they give the same
+// row shares and so the same per-unit sums.  On an H100 at a 400 W power limit the kernel takes 0.51-0.52 ms (with the
+// global rigidity term) and 0.44 ms (without) at the benchmark shape, against 1.11-1.13 / 0.94 ms before; per-cluster
+// busy time spreads from 0.74 to 1.11 of the mean (tools/wgrad_cluster_balance.py).
 static double step_cost(int a_cols, int b_cols) {
   const int cols = a_cols + b_cols;
   return cols >= 512 ? 512.0 : (cols >= 320 ? 416.0 : 340.0);
 }
 
-struct WgProto { const char* a; int64_t a_term; int a_cols; const char* b; int64_t b_term; int b_cols;
+struct WgProto { const char* a; int64_t a_term; int a_cols; const char* b; int64_t b_term; int b_cols; int transposed;
                  float* out; int ld; int n_rows, n_cols, groups; double bytes; int mapping; };
 
 static void protos_for_net(WgProto* protos, int& np, const MlpShape& sh, const NetImages& im, float* g, TcNet net,
@@ -1200,15 +1238,16 @@ static void protos_for_net(WgProto* protos, int& np, const MlpShape& sh, const N
   const bool pe = tc_pe_first(net);
   const int mapping = tc_net_is_mapping(net) ? 1 : 0;
   auto add = [&](const char* a, int64_t a_term, int a_cols, const char* b, int64_t b_term, int b_cols, float* out, int ld,
-                 int n_rows, int n_cols) {
-    protos[np++] = WgProto{a, a_term, a_cols, b, b_term, b_cols, out, ld, n_rows, n_cols, groups,
+                 int n_rows, int n_cols, int transposed = 0) {
+    protos[np++] = WgProto{a, a_term, a_cols, b, b_term, b_cols, transposed, out, ld, n_rows, n_cols, groups,
                            (double)groups * step_cost(a_cols, b_cols), mapping};
   };
   for (int l = 1; l <= sh.L - 2; ++l)
     add(im.dz + (int64_t)l * im.slot_stride, im.term_stride, 256, im.act + (int64_t)(l - 1) * im.slot_stride,
         im.term_stride, 256, g + sh.w_off[l], sh.K[l], 256, 256);
-  add(im.dzl, im.w64_term_stride, 64, im.act + (int64_t)(sh.L - 2) * im.slot_stride, im.term_stride, 256,
-      g + sh.w_off[sh.L - 1], sh.K[sh.L - 1], sh.out_dim, 256);
+  // output layer: the 256-wide activation goes on the M side (split over the pair), dW is written transposed
+  add(im.act + (int64_t)(sh.L - 2) * im.slot_stride, im.term_stride, 256, im.dzl, im.w64_term_stride, 64,
+      g + sh.w_off[sh.L - 1], sh.K[sh.L - 1], sh.out_dim, 256, 1);
   if (pe) {
     // positional-encoding parts: layer 0 and the skip layers; output layer's skip part
     add(im.dz, im.term_stride, 256, im.pe, im.w64_term_stride, 64, g + sh.w_off[0], sh.K[0], 256, sh.enc);
@@ -1222,14 +1261,17 @@ static void protos_for_net(WgProto* protos, int& np, const MlpShape& sh, const N
   }
 }
 
-// One CTA per SM (each CTA needs most of the shared memory); the GEMMs are cut into WG_UNITS_PER_CTA x SMs units of equal
-// cost (largest-remainder apportionment) that the CTAs take round-robin (see tc_wgrad_kernel).  More than one unit
-// per CTA balances any cost-model error but multiplies the accumulator flushes (fp32 vector atomics), so the default is 1.
-constexpr int WG_UNITS_PER_CTA = 1;
+// One CTA per SM (each CTA needs most of the shared memory), in clusters of two; the GEMMs are cut into
+// WG_UNITS_PER_CLUSTER x clusters units of equal cost (largest-remainder apportionment) that the clusters take
+// round-robin (see tc_wgrad_kernel).  Two units per cluster keep the rows summed by one fp32 accumulator at what one
+// CTA per SM summed (wgmma accumulation error grows with that length, and the ill-conditioned mapping gradients show
+// it); on a 132-SM H100 the work list is the same as with one unit per SM.
+constexpr int WG_UNITS_PER_CLUSTER = 2;
+static int wg_clusters() { return g_wg_clusters[current_device()]; }
 static void apportion_items(WgradItems& wi, const WgProto* protos, int np, int cap, int flow_groups) {
   double total_bytes = 0;
   for (int i = 0; i < np; ++i) total_bytes += protos[i].bytes;
-  const int sms = sm_count() * WG_UNITS_PER_CTA;
+  const int sms = wg_clusters() * WG_UNITS_PER_CLUSTER;
   int n_split[32], used = 0;
   double frac[32];
   for (int i = 0; i < np; ++i) {
@@ -1254,7 +1296,7 @@ static void apportion_items(WgradItems& wi, const WgProto* protos, int np, int c
       WgradItem& it = wi.it[wi.n++];
       const WgProto& pr = protos[i];
       it.a_img = pr.a; it.a_term = pr.a_term; it.a_cols = pr.a_cols;
-      it.b_img = pr.b; it.b_term = pr.b_term; it.b_cols = pr.b_cols;
+      it.b_img = pr.b; it.b_term = pr.b_term; it.b_cols = pr.b_cols; it.transposed = pr.transposed;
       it.out = pr.out; it.ld_out = pr.ld; it.n_rows = pr.n_rows; it.n_cols = pr.n_cols;
       it.cap = cap; it.n_groups = pr.groups; it.split = sp; it.n_split = n_split[i]; it.mapping = pr.mapping;
       it.flow_groups = (pr.mapping && flow_groups) ? 1 : 0;
@@ -1281,8 +1323,6 @@ static std::vector<TcTables*> g_tabs;
 static std::mutex g_tabs_mutex;
 static thread_local PrepJobs g_pj;        // host side of the table being built
 static thread_local WgradItems g_wi;
-
-static int current_device() { int d = 0; cudaGetDevice(&d); return d; }
 
 // The entry of `k`, or null.  `add`: a missing entry is added with no tables yet.  An entry without gradient buffer
 // (made by a stand-alone forward) adopts the first one a backward brings.
@@ -1396,18 +1436,24 @@ int tc_step_forward(const TcStep& s, cudaStream_t st) {
 static const WgradItems* g_last_wg = nullptr;
 static int g_last_wg_n = 0;
 
-// diagnostics: per-CTA cycle counts and (a_cols, b_cols, n_split) of the item each CTA ran in the last weight-gradient launch
+// diagnostics: per-CTA cycle counts and the dW shape (rows, columns of its image operands) and n_split of the first item
+// each CTA ran in the last weight-gradient launch; CTAs 2c and 2c + 1 form cluster c
 int tc_debug_wgrad(long long* cycles, int* shapes, int max_ctas) {
   if (!g_last_wg) { set_error("no weight-gradient launch yet"); return -1; }
   static WgradItems host;
   if (cudaMemcpy(&host, g_last_wg, sizeof(WgradItems), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
   const int n = g_last_wg_n < max_ctas ? g_last_wg_n : max_ctas;
   for (int i = 0; i < n; ++i) {
+    const WgradItem& it = host.it[i / WG_CLUSTER];
     cycles[i] = host.cycles[i];
-    shapes[3 * i] = host.it[i].a_cols; shapes[3 * i + 1] = host.it[i].b_cols; shapes[3 * i + 2] = host.it[i].n_split;
+    shapes[3 * i] = it.transposed ? it.b_cols : it.a_cols; shapes[3 * i + 1] = it.transposed ? it.a_cols : it.b_cols;
+    shapes[3 * i + 2] = it.n_split;
   }
   return n;
 }
+
+// grid of a weight-gradient launch: as many clusters as fit on the device at once, at most one per work unit
+static int wgrad_grid(int n_items) { return WG_CLUSTER * min(n_items, wg_clusters()); }
 
 int tc_step_backward(const TcStep& s, cudaStream_t st) {
   const TcLayout lay = layout_of(s);
@@ -1428,8 +1474,8 @@ int tc_step_backward(const TcStep& s, cudaStream_t st) {
   B200_PROPAGATE(launch_bwd(tc_net_of(*s.ms), pm, s.n_groups * (s.cap / TM), st));
   timer_end(TAG_MAP_BWD, st);
   timer_begin(TAG_WGRAD, st);
-  g_last_wg = tab->d_wg; g_last_wg_n = min(tab->n_wg, sm_count());
-  tc_wgrad_kernel<<<min(tab->n_wg, sm_count()), WG_THREADS, WG_SMEM, st>>>(tab->d_wg, s.counters, gmax);
+  g_last_wg = tab->d_wg; g_last_wg_n = wgrad_grid(tab->n_wg);
+  tc_wgrad_kernel<<<wgrad_grid(tab->n_wg), WG_THREADS, WG_SMEM, st>>>(tab->d_wg, s.counters, gmax);
   timer_end(TAG_WGRAD, st);
   B200_CHECK_LAUNCH();
   return B200_OK;
@@ -1563,7 +1609,7 @@ int tc_single_backward(const MlpShape& sh, TcNet net, const float* params, float
   BwdParams P = fill_bwd(sh, pl.im, dy, y, x, d_in, params, grads, (int)rows, 1, nullptr, gmax2);
   P.in_scale = 1.0f; P.d_in_accumulate = 0; P.tanh_out = sh.tanh_out ? 1 : 0;
   B200_PROPAGATE(launch_bwd(net, P, (int)(rows / TM), st));
-  tc_wgrad_kernel<<<min(tab->n_wg, sm_count()), WG_THREADS, WG_SMEM, st>>>(tab->d_wg, nullptr, gmax2);
+  tc_wgrad_kernel<<<wgrad_grid(tab->n_wg), WG_THREADS, WG_SMEM, st>>>(tab->d_wg, nullptr, gmax2);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }

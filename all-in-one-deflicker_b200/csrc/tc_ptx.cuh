@@ -45,6 +45,28 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
+// ------------------------------------------------------------------------------------ thread-block clusters
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// every thread of every CTA of the cluster; orders the shared-memory operations before it cluster-wide
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// the shared::cluster address of the same shared-memory offset in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t mapa_shared(uint32_t smem_addr, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
+  return r;
+}
+// arrive on an mbarrier of another CTA of the cluster (address from mapa_shared).  Default (CTA-scope) release: it
+// frees an operand slot whose reads by wgmma have already completed, so no cluster-wide fence is needed.
+__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
+}
+
 // ------------------------------------------------------------------------------------ bulk copy
 // contiguous global -> shared through the TMA engine (UBLKCP), completion on an mbarrier
 __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, uint32_t bytes, uint64_t* bar) {
@@ -52,6 +74,16 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
                    smem_u32(dst_smem)),
                "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
+}
+// the same copy into the same shared-memory offset of every CTA of the cluster in `cta_mask`; each destination CTA's
+// mbarrier at the offset of `bar` receives the bytes it got
+__device__ __forceinline__ void bulk_g2s_multicast(void* dst_smem, const void* src_gmem, uint32_t bytes, uint64_t* bar,
+                                                   uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(
+          smem_u32(dst_smem)),
+      "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)), "h"(cta_mask)
+      : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
