@@ -13,14 +13,13 @@ ACT = {"none": 0, "relu": 1, "leaky": 2, "sigmoid": 3, "tanh": 4}
 # summation order), "tc" = wgmma with fp16 operands and fp32 accumulation — the operand precision the
 # reference itself uses for these layers (fp16 autocast in RAFT, TF32 cuDNN in stage 2).
 _conv_precision = "fp32"
-_weight_images = {}        # id(weight tensor) -> (weakref to it, {(version, layout): packed fp16 images})
+_weight_images = {}        # id(weight tensor) -> (weakref to it, {(version, stride): packed fp16 images})
 
 
 def set_conv_precision(mode):
-    """'fp32', 'tc' (TMA-fed wgmma; gather variant for strides it does not take) or 'tc_gather'.
-    Returns the previous mode."""
+    """'fp32' or 'tc' (TMA-fed wgmma; stride 1 or 2).  Returns the previous mode."""
     global _conv_precision
-    if mode not in ("fp32", "tc", "tc_gather"):
+    if mode not in ("fp32", "tc"):
         raise N.B200Error(f"unknown convolution precision {mode!r}")
     prev, _conv_precision = _conv_precision, mode
     return prev
@@ -30,7 +29,7 @@ def conv_precision():
     return _conv_precision
 
 
-def _images_for(d, w, tma):
+def _images_for(d, w):
     """Packed weight images, cached per weight TENSOR OBJECT (not per address: a freed tensor's address is reused)
     and per in-place version.  Pass module parameters themselves (conv.weight) to benefit from the cache."""
     key = id(w)
@@ -38,18 +37,16 @@ def _images_for(d, w, tma):
     if ent is None or ent[0]() is not w:
         ent = (weakref.ref(w, lambda _r, k=key: _weight_images.pop(k, None)), {})
         _weight_images[key] = ent
-    sub = (w._version, tma, d.stride)
+    sub = (w._version, d.stride)
     img = ent[1].get(sub)
     if img is None:
         ent[1].clear()
-        L = N.lib()
-        size_fn, pack_fn = ((L.b200_conv_tma_weight_image_bytes, L.b200_conv_tma_weight_images) if tma else
-                            (L.b200_conv_weight_image_bytes, L.b200_conv_weight_images))
-        nbytes = size_fn(C.byref(d))
+        nbytes = N.lib().b200_conv_tma_weight_image_bytes(C.byref(d))
         if nbytes <= 0:
             raise N.B200Error("conv weight image size: invalid descriptor: " + N.last_error())
         img = torch.empty(nbytes, dtype=torch.uint8, device=w.device)
-        N.check(pack_fn(C.byref(d), N.ptr(w), N.ptr(img), N.current_stream()), "conv weight images")
+        N.check(N.lib().b200_conv_tma_weight_images(C.byref(d), N.ptr(w), N.ptr(img), N.current_stream()),
+                "conv weight images")
         ent[1][sub] = img
     return img
 
@@ -104,18 +101,22 @@ def conv2d(x, w, b=None, stride=1, pad=(0, 0), pad_mode="zeros", act="none", ups
     out[:, out_c_off:out_c_off+Cout] (allocated when None).  Restates nn.Conv2d / ReflectionPad2d / Upsample.
     `x` may be a `Chain` (input already packed by its producers); `chain_out` additionally writes the result into the
     consumer's packed input at channel `chain_c_off`, and with keep_fp32=False the fp32 tensor is not produced (returns
-    None)."""
-    if isinstance(x, Chain) or chain_out is not None:
-        return _conv2d_chained(x, w, b, stride, pad, pad_mode, act, upsample, out, out_c_off, in_slice, residual, res_c_off,
-                               out_scale, upsample_mode, chain_out, chain_c_off, keep_fp32)
-    _check(x); _check(w); _check(b); _check(residual)
+    None).  With precision 'tc' (and whenever `x` or `chain_out` is a `Chain`) the convolution runs on the wgmma
+    path, which takes stride 1 or 2 only: any other stride raises B200Error rather than changing the arithmetic."""
+    _check(w); _check(b); _check(residual)
     mode = _conv_precision if precision is None else precision
+    if mode not in ("fp32", "tc"):
+        raise N.B200Error(f"unknown convolution precision {mode!r}")
+    packed_in = isinstance(x, Chain)
+    tc = mode == "tc" or packed_in or chain_out is not None
+    if not packed_in:
+        _check(x)
     bilinear = 0
     if upsample_mode == "bilinear":
         if upsample != 2:
             raise N.B200Error("bilinear upsampling is x2 only")
-        if mode == "tc" and stride in (1, 2):
-            bilinear = 1                                  # fused into the fp16 repack of b200_conv2d_tma
+        if tc:
+            bilinear = 1                                  # fused into the fp16 repack of b200_conv2d_tma_chain
         else:                                             # explicit nn.Upsample kernel, then a plain convolution
             if in_slice is not None:
                 x = x[:, in_slice[0]:in_slice[1]].contiguous()
@@ -123,49 +124,12 @@ def conv2d(x, w, b=None, stride=1, pad=(0, 0), pad_mode="zeros", act="none", ups
             x, upsample = upsample_bilinear2(x), 1
     elif upsample_mode != "nearest":
         raise N.B200Error(f"unknown upsample mode {upsample_mode!r}")
-    n, c_total, h, wd = x.shape
-    c_off, cin = (0, c_total) if in_slice is None else (in_slice[0], in_slice[1] - in_slice[0])
-    cout, cin_w, kh, kw = w.shape
-    if cin_w != cin:
-        raise N.B200Error(f"weight expects {cin_w} input channels, got {cin}")
-    ph, pw = (pad, pad) if isinstance(pad, int) else pad
-    hu, wu = h * upsample, wd * upsample
-    oh, ow = (hu + 2 * ph - kh) // stride + 1, (wu + 2 * pw - kw) // stride + 1
-    if out is None:
-        out = torch.empty(n, cout, oh, ow, dtype=torch.float32, device=x.device)
-    _check(out)
-    d = N.ConvDesc(n, cin, h, wd, c_total, c_off, cout, kh, kw, stride, ph, pw, 1 if pad_mode == "reflect" else 0,
-                   upsample, out.shape[1], out_c_off, ACT[act], float(out_scale),
-                   residual.shape[1] if residual is not None else 0, res_c_off, bilinear)
-    if mode == "tc" and stride in (1, 2):
-        nbytes = N.lib().b200_conv_tma_workspace_bytes(C.byref(d))
-        if nbytes <= 0:
-            raise N.B200Error("b200_conv_tma_workspace_bytes: " + N.last_error())
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
-        N.check(N.lib().b200_conv2d_tma(C.byref(d), N.ptr(x), N.ptr(_images_for(d, w, True)), N.ptr(b), N.ptr(residual),
-                                        N.ptr(out), N.ptr(ws), nbytes, N.current_stream()), "b200_conv2d_tma")
-    elif mode in ("tc", "tc_gather"):
-        N.check(N.lib().b200_conv2d_tc(C.byref(d), N.ptr(x), N.ptr(_images_for(d, w, False)), N.ptr(b), N.ptr(residual),
-                                       N.ptr(out), N.current_stream()), "b200_conv2d_tc")
-    else:
-        N.check(N.lib().b200_conv2d(C.byref(d), N.ptr(x), N.ptr(w), N.ptr(b), N.ptr(residual), N.ptr(out),
-                                    N.current_stream()), "b200_conv2d")
-    return out
-
-
-def _conv2d_chained(x, w, b, stride, pad, pad_mode, act, upsample, out, out_c_off, in_slice, residual, res_c_off, out_scale,
-                    upsample_mode, chain_out, chain_c_off, keep_fp32):
-    """b200_conv2d_tma_chain: packed input and / or packed output (wgmma path, see `Chain`)."""
-    _check(w); _check(b); _check(residual)
-    packed_in = isinstance(x, Chain)
-    bilinear = 1 if upsample_mode == "bilinear" else 0
     if packed_in:
         if in_slice is not None or stride != 1 or upsample != 1 or pad_mode != x.pad_mode:
             raise N.B200Error("a chained input feeds a plain stride-1 convolution of the whole tensor, padded as declared")
         n, c_total, h, wd = x.n, x.cin, x.h, x.w
         dev = x.buf.device
     else:
-        _check(x)
         n, c_total, h, wd = x.shape
         dev = x.device
     c_off, cin = (0, c_total) if in_slice is None else (in_slice[0], in_slice[1] - in_slice[0])
@@ -184,6 +148,10 @@ def _conv2d_chained(x, w, b, stride, pad, pad_mode, act, upsample, out, out_c_of
     d = N.ConvDesc(n, cin, h, wd, c_total, c_off, cout, kh, kw, stride, ph, pw, 1 if pad_mode == "reflect" else 0, upsample,
                    out.shape[1] if out is not None else cout, out_c_off if out is not None else 0, ACT[act], float(out_scale),
                    residual.shape[1] if residual is not None else 0, res_c_off, bilinear)
+    if not tc:
+        N.check(N.lib().b200_conv2d(C.byref(d), N.ptr(x), N.ptr(w), N.ptr(b), N.ptr(residual), N.ptr(out),
+                                    N.current_stream()), "b200_conv2d")
+        return out
     if packed_in and (x.desc.KH, x.desc.KW, x.desc.pad_h, x.desc.pad_w) != (kh, kw, ph, pw):
         raise N.B200Error("the chained input was packed for another filter geometry")
     ws, nbytes = None, 0
@@ -193,7 +161,7 @@ def _conv2d_chained(x, w, b, stride, pad, pad_mode, act, upsample, out, out_c_of
             raise N.B200Error("b200_conv_tma_workspace_bytes: " + N.last_error())
         ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     N.check(N.lib().b200_conv2d_tma_chain(
-        C.byref(d), None if packed_in else N.ptr(x), N.ptr(x.buf) if packed_in else None, N.ptr(_images_for(d, w, True)),
+        C.byref(d), None if packed_in else N.ptr(x), N.ptr(x.buf) if packed_in else None, N.ptr(_images_for(d, w)),
         N.ptr(b), N.ptr(residual), N.ptr(out), N.ptr(chain_out.buf) if chain_out is not None else None,
         C.byref(chain_out.desc) if chain_out is not None else None, int(chain_c_off), N.ptr(ws), nbytes,
         N.current_stream()), "b200_conv2d_tma_chain")

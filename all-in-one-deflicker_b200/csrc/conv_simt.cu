@@ -316,7 +316,7 @@ int b200_add_relu(const float* a, const float* b, float* out, int64_t n, void* s
 
 int b200_conv2d(const B200ConvDesc* d, const float* x, const float* w, const float* bias, const float* residual,
                 float* y, void* stream) {
-  B200_REQUIRE(d && d->upsample_mode == 0, "bilinear upsampling is fused only by b200_conv2d_tma");
+  B200_REQUIRE(d && d->upsample_mode == 0, "bilinear upsampling is fused only by b200_conv2d_tma_chain");
   B200_REQUIRE(d && x && w && y, "null pointer");
   B200_REQUIRE(d->N > 0 && d->Cin > 0 && d->H > 0 && d->W > 0 && d->Cout > 0 && d->KH > 0 && d->KW > 0 && d->stride > 0 &&
                (d->upsample == 1 || d->upsample == 2) && (d->pad_mode == 0 || d->pad_mode == 1) && d->act >= 0 && d->act <= 4,

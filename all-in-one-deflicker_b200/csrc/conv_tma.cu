@@ -429,7 +429,7 @@ static int tma_geometry(const B200ConvDesc* d, TmaGeom* g) {
                (d->stride == 1 || d->stride == 2) && (d->upsample == 1 || d->upsample == 2) &&
                (d->pad_mode == 0 || d->pad_mode == 1) && d->act >= 0 && d->act <= 4 && d->pad_h >= 0 && d->pad_w >= 0 &&
                (d->upsample_mode == 0 || (d->upsample_mode == 1 && d->upsample == 2)),
-               "invalid convolution descriptor (b200_conv2d_tma supports stride 1 and 2)");
+               "invalid convolution descriptor (b200_conv2d_tma_chain supports stride 1 and 2)");
   g->HU = d->H * d->upsample; g->WU = d->W * d->upsample;
   B200_REQUIRE(d->pad_mode == 0 || (d->pad_h < g->HU && d->pad_w < g->WU), "reflection padding larger than the input");
   const int HP = g->HU + 2 * d->pad_h, WP = g->WU + 2 * d->pad_w;
@@ -592,22 +592,6 @@ int b200_conv_tma_weight_images(const B200ConvDesc* d, const float* w, void* ima
   if (int rc = tma_geometry(d, &g)) return rc;
   const int KHW = d->KH * d->KW;
   return launch_weight_images(d, g, w, (int64_t)d->Cin * KHW, KHW, 1, 1.0f, 0, images, reinterpret_cast<cudaStream_t>(stream));
-}
-
-int b200_conv2d_tma(const B200ConvDesc* d, const float* x, const void* w_images, const float* bias,
-                    const float* residual, float* y, void* workspace, int64_t workspace_bytes, void* stream) {
-  B200_REQUIRE(x && w_images && y && workspace, "null pointer");
-  TmaGeom g;
-  if (int rc = tma_geometry(d, &g)) return rc;
-  B200_REQUIRE(d->in_c_off >= 0 && d->in_c_off + d->Cin <= d->in_c_total && d->out_c_off >= 0 &&
-               d->out_c_off + d->Cout <= d->out_c_total, "channel slice out of range");
-  if (!b200_device_supports_tc()) { set_error("b200_conv2d_tma needs a compute-capability 9.x device"); return B200_ERR_UNSUPPORTED; }
-  char* base = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
-  if (base + g.pack_bytes > reinterpret_cast<char*>(workspace) + workspace_bytes) {
-    set_error("b200_conv2d_tma: workspace too small (%lld < %lld)", (long long)workspace_bytes, (long long)(g.pack_bytes + 256));
-    return B200_ERR_WORKSPACE;
-  }
-  return launch_conv_tma(d, g, x, base, w_images, bias, residual, y, 0, 1.0f, reinterpret_cast<cudaStream_t>(stream));
 }
 
 /* A convolution can consume a packed input written by its producers when its packing is the plain one: stride 1, no

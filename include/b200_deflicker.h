@@ -437,36 +437,33 @@ typedef struct B200ConvDesc {
   int32_t res_c_total, res_c_off;  /* residual tensor slice (same spatial size as the output)         */
   int32_t upsample_mode;           /* with upsample == 2: B200_UP_NEAREST or B200_UP_BILINEAR_AC
                                       (nn.Upsample(scale_factor=2, mode='bilinear', align_corners=True),
-                                      network_filter.py:22 — b200_conv2d_tma only)                     */
+                                      network_filter.py:22 — b200_conv2d_tma_chain only)               */
 } B200ConvDesc;
 int b200_conv2d(const B200ConvDesc* d, const float* x, const float* w, const float* bias,
                 const float* residual, float* y, void* stream);
 /* Tensor-core (wgmma, fp16 operands / fp32 accumulate) variant of b200_conv2d for the layers the reference
  * itself runs with 10-bit-mantissa operands (RAFT under fp16 autocast, core/raft.py:131; stage-2 cuDNN
- * convolutions with TF32 allowed).  Weights are first packed into K-major swizzled fp16 images:
- *   bytes = b200_conv_weight_image_bytes(d);  b200_conv_weight_images(d, w, images, stream);
- * then b200_conv2d_tc takes `images` in place of w.  Same descriptor semantics as b200_conv2d. */
-int64_t b200_conv_weight_image_bytes(const B200ConvDesc* d);
-int b200_conv_weight_images(const B200ConvDesc* d, const float* w, void* images, void* stream);
-int b200_conv2d_tc(const B200ConvDesc* d, const float* x, const void* w_images, const float* bias,
-                   const float* residual, float* y, void* stream);
-/* TMA-fed variant (preferred): the input slice is first repacked to fp16 with padding / upsampling / stride
- * phases materialised (workspace of b200_conv_tma_workspace_bytes(d) bytes), then every filter tap is a tiled
- * TMA box load feeding wgmma directly — no im2col gather.  stride 1 or 2.  Weight images have their own
- * layout (tap-major):  b200_conv_tma_weight_image_bytes / b200_conv_tma_weight_images. */
-int64_t b200_conv_tma_workspace_bytes(const B200ConvDesc* d);
-int64_t b200_conv_tma_weight_image_bytes(const B200ConvDesc* d);
-int b200_conv_tma_weight_images(const B200ConvDesc* d, const float* w, void* images, void* stream);
-int b200_conv2d_tma(const B200ConvDesc* d, const float* x, const void* w_images, const float* bias,
-                    const float* residual, float* y, void* workspace, int64_t workspace_bytes, void* stream);
-/* Chained form: the fp16 NHWC repack of a convolution's input is skipped when its producers wrote it directly.
+ * convolutions with TF32 allowed).  Same descriptor semantics as b200_conv2d; stride 1 or 2.  The input slice is
+ * first repacked to fp16 with padding / upsampling / stride phases materialised (workspace of
+ * b200_conv_tma_workspace_bytes(d) bytes), then every filter tap is a tiled TMA box load feeding wgmma directly.
+ * Weights are first packed into tap-major swizzled fp16 images:
+ *   bytes = b200_conv_tma_weight_image_bytes(d);  b200_conv_tma_weight_images(d, w, images, stream);
+ * then b200_conv2d_tma_chain takes `images` in place of w.
+ *
+ * b200_conv2d_tma_chain(d, x, NULL, images, bias, residual, y, NULL, NULL, 0, ws, ws_bytes, stream) is the plain
+ * convolution.  The chained form skips the fp16 NHWC repack of a convolution's input when its producers wrote it directly:
  *   in_packed  (or NULL): the packed input of `d` — b200_conv_tma_workspace_bytes(d) bytes, 256-byte aligned, zeroed once
- *              by the caller (halo and padded channels stay zero), interior written by the producers; x is then ignored
+ *              by the caller (halo and padded channels stay zero), interior written by the producers; x and the
+ *              workspace are then ignored
  *   out_packed (or NULL) + next + next_c_off: ALSO write act(conv) as fp16 into the packed input of the consumer
  *              convolution `next` at its input channel next_c_off (several producers may fill one consumer: concat);
  *              y may then be NULL (no fp32 NCHW output at all)
- * `next` / `d` with a packed input must satisfy b200_conv_tma_chainable: stride 1, no upsampling, zero padding, whole
- * input tensor (no channel slice), Cin * KW > 64. */
+ * `next` / `d` with a packed input must satisfy b200_conv_tma_chainable: stride 1, no upsampling, zero or reflection
+ * padding (a reflection halo is mirrored from the interior by the consumer call), whole input tensor (no channel slice),
+ * Cin * KW > 64. */
+int64_t b200_conv_tma_workspace_bytes(const B200ConvDesc* d);
+int64_t b200_conv_tma_weight_image_bytes(const B200ConvDesc* d);
+int b200_conv_tma_weight_images(const B200ConvDesc* d, const float* w, void* images, void* stream);
 int b200_conv_tma_chainable(const B200ConvDesc* next);
 int b200_conv2d_tma_chain(const B200ConvDesc* d, const float* x, void* in_packed, const void* w_images,
                           const float* bias, const float* residual, float* y, void* out_packed,

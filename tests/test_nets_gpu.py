@@ -146,7 +146,6 @@ def test_conv_tc_single_layer(case):
     b = torch.randn(cout, generator=g)
     xd, wd, bd = x.to(DEV), wt.to(DEV), b.to(DEV)
     y_tc = K.conv2d(xd, wd, bd, stride=stride, pad=pad, pad_mode=mode, act=act, upsample=ups, precision="tc")
-    y_tg = K.conv2d(xd, wd, bd, stride=stride, pad=pad, pad_mode=mode, act=act, upsample=ups, precision="tc_gather")
     y_32 = K.conv2d(xd, wd, bd, stride=stride, pad=pad, pad_mode=mode, act=act, upsample=ups, precision="fp32")
     xx = x.double()
     if ups == 2:
@@ -162,10 +161,10 @@ def test_conv_tc_single_layer(case):
     scale = ref.abs().max().item()
     assert (y_32.cpu().double() - ref).abs().max() <= 2e-5 * scale
     assert (y_tc.cpu().double() - ref).abs().max() <= 4e-3 * scale        # TMA-fed kernel
-    assert (y_tg.cpu().double() - ref).abs().max() <= 4e-3 * scale        # gather kernel
 
 
 def test_conv_tc_slices_residual_and_scale():
+    from b200 import _native as N
     from b200 import nn as K
     g = torch.Generator().manual_seed(5)
     x = torch.randn(1, 96, 20, 28, generator=g).to(DEV)
@@ -181,6 +180,8 @@ def test_conv_tc_slices_residual_and_scale():
     assert torch.equal(outs[1][:, :8], torch.full_like(outs[1][:, :8], 7.0))
     assert torch.equal(outs[1][:, 48:], torch.full_like(outs[1][:, 48:], 7.0))
     assert (outs[0] - outs[1]).abs().max() <= 4e-3 * outs[0][:, 8:48].abs().max()
+    with pytest.raises(N.B200Error, match="stride 1 and 2"):     # no silent fall-back to another arithmetic
+        K.conv2d(x, wt, b, stride=3, pad=1, in_slice=(16, 80), precision="tc")
 
 
 def test_networks_with_tc_convolutions(golden_dir):
