@@ -9,7 +9,7 @@
 // iteration from max|dL/dy|), undone exactly in the epilogues.
 //
 // Kernels
-//   tc_prep_kernel   fp32 parameters -> split fp16 "stage images" (the exact 128B-swizzled smem
+//   tc_prep_kernel   fp32 parameters -> split fp16 weight items (16 KB each, the exact 64B-swizzled smem
 //                    layout a wgmma descriptor reads), W for the forward and W^T for the dgrad
 //   tc_fwd_kernel    persistent; one 128-row tile walks through ALL layers on chip: the A operand lives in
 //                    shared memory in the image layout, weights stream L2->smem through the TMA engine
@@ -41,7 +41,8 @@ using namespace ptx;
 
 constexpr int TM = 128;                 // rows per tile
 constexpr int HID = 256;
-constexpr int STAGE_BYTES = 32768;      // one weight image: 256 rows x 64 k (fp16), 128B swizzle
+constexpr int ITEM_BYTES = 16384;       // one weight item: 256 rows x 32 k (fp16), K-major, 64B swizzle
+constexpr int CHUNK_BYTES = 4 * ITEM_BYTES;   // one 64-wide k chunk of a weight: hi k 0-31, hi k 32-63, lo k 0-31, lo 32-63
 constexpr float S_ACT = 16.0f;          // activation scale before the fp16 split
 constexpr float S_W = 256.0f;           // weight scale
 constexpr int ATOM_BYTES = TM * 128;    // one 64-column block of a tile image, one term: 16 KB
@@ -55,14 +56,19 @@ __host__ __device__ __forceinline__ int atom_off(int m, int k) {          // k i
   const int r = m & 7;
   return (m >> 3) * 1024 + r * 128 + (((k >> 3) ^ r) << 4) + ((k & 7) << 1);
 }
+// Weight item = [32 groups of 8 rows][8 rows x 64 B] with the 16-byte chunks of a row XOR-swizzled by (row / 2) % 4:
+// a K-major SW64 wgmma B operand (N = rows, K = the 32 columns).
+__host__ __device__ __forceinline__ int item_off(int n, int k) {          // k in [0, 32)
+  return (n >> 3) * 512 + (n & 7) * 64 + ((((k >> 3) ^ (n >> 1)) & 3) << 4) + ((k & 7) << 1);
+}
 
 // ---------------------------------------------------------------------------------------------
 // layout of the tensor-core workspace
 // ---------------------------------------------------------------------------------------------
 struct NetImages {
-  // forward weight images, consumption order: per TC layer, per 64-wide k chunk: hi image, lo image
+  // forward weight items, consumption order: per TC layer, per 64-wide k chunk: hi k 0-31, hi k 32-63, lo k 0-31, lo 32-63
   char* w_fwd; int64_t w_fwd_layer[B200_MAX_LAYERS]; int n_chunks_fwd[B200_MAX_LAYERS];
-  // dgrad weight images (W^T): per layer, per 64-wide chunk of the reduction (out) index: hi, lo
+  // dgrad weight items (W^T): per layer, per 64-wide chunk of the reduction (out) index: the same four items
   char* w_bwd; int64_t w_bwd_layer[B200_MAX_LAYERS];
   // activation images h_0..h_{L-2} and dZ images: [slot][term][tile][4 atoms][16 KB]
   char* act; char* dz;
@@ -88,7 +94,7 @@ static void plan_fwd_weights(const MlpShape& s, TcNet net, char*& p, NetImages* 
     if (tc_layer) chunks = (l == 0 ? 0 : HID / 64) + ((l == 0 || s.skip[l]) && pe ? 1 : 0);
     n->n_chunks_fwd[l] = chunks;
     n->w_fwd_layer[l] = off;
-    off += (int64_t)chunks * 2 * STAGE_BYTES;
+    off += (int64_t)chunks * CHUNK_BYTES;
   }
   n->w_fwd = carve_tc(p, off);
 }
@@ -102,7 +108,7 @@ static void plan_net(const MlpShape& s, int64_t rows, TcNet net, char*& p, NetIm
   for (int l = 0; l < s.L; ++l) {
     n->w_bwd_layer[l] = off;
     const bool used = l <= s.L - 2 && (pe || l >= 1);
-    if (used) off += (int64_t)(HID / 64) * 2 * STAGE_BYTES;
+    if (used) off += (int64_t)(HID / 64) * CHUNK_BYTES;
   }
   n->w_bwd = carve_tc(p, off);
   n->term_stride = tiles * TILE_IMG_BYTES;
@@ -140,14 +146,14 @@ struct PrepJob {
   const float* W; int ldw;          // fp32 weight [N][ldw]
   int n_rows, k0, k_cnt;            // valid image rows and the window [k0, k0+k_cnt) of the other index
   int transpose;                    // 0: image(row=n, col=k-k0) = W[n][k];  1: image(row=k, col=n-k0) = W[n][k]
-  char* hi; char* lo;               // destination images (32 KB each, zero padded)
+  char* hi; char* lo;               // destination: two 16 KB items each (k 0-31, k 32-63), zero padded
 };
 constexpr int MAX_PREP_JOBS = 96;
 struct PrepJobs { PrepJob j[MAX_PREP_JOBS]; int n; };
 
 __global__ void tc_prep_kernel(const PrepJobs* __restrict__ jobs_ptr) {
   const PrepJob jb = jobs_ptr->j[blockIdx.x >> 2];
-  // one image = 256 rows x 64 cols; this block does 64 rows; thread handles one 16-byte chunk at a time
+  // one job = 256 rows x 64 cols; this block does 64 rows; thread handles one 16-byte chunk at a time
   for (int e = threadIdx.x; e < 64 * 8; e += blockDim.x) {
     const int row = (blockIdx.x & 3) * 64 + (e >> 3), c8 = (e & 7) * 8;
     float v[8];
@@ -161,7 +167,7 @@ __global__ void tc_prep_kernel(const PrepJobs* __restrict__ jobs_ptr) {
     uint32_t h[4], l[4];
 #pragma unroll
     for (int q = 0; q < 4; ++q) split2_f16(v[2 * q] * S_W, v[2 * q + 1] * S_W, h[q], l[q]);
-    const int off = atom_off(row, c8);
+    const int off = (c8 >> 5) * ITEM_BYTES + item_off(row, c8 & 31);
     *reinterpret_cast<uint4*>(jb.hi + off) = make_uint4(h[0], h[1], h[2], h[3]);
     *reinterpret_cast<uint4*>(jb.lo + off) = make_uint4(l[0], l[1], l[2], l[3]);
   }
@@ -202,12 +208,14 @@ struct TileIter {                    // static round-robin over the live tiles o
   }
 };
 
+// n_items consecutive weight items into the ring; `bytes` < ITEM_BYTES sends only the first rows of each (the n64 dPE
+// product reads 64 of the 256 rows)
 template <int NST>
-__device__ __forceinline__ void produce_items(Pipe<NST>& pp, const char* src, int n_items) {
+__device__ __forceinline__ void produce_items(Pipe<NST>& pp, const char* src, int n_items, uint32_t bytes = ITEM_BYTES) {
   for (int i = 0; i < n_items; ++i) {
     mbar_wait(&pp.empty[pp.slot()], pp.parity() ^ 1);
-    mbar_expect_tx(&pp.full[pp.slot()], STAGE_BYTES);
-    bulk_g2s(pp.stage + pp.slot() * STAGE_BYTES, src + (int64_t)i * STAGE_BYTES, STAGE_BYTES, &pp.full[pp.slot()]);
+    mbar_expect_tx(&pp.full[pp.slot()], bytes);
+    bulk_g2s(pp.stage + pp.slot() * ITEM_BYTES, src + (int64_t)i * ITEM_BYTES, bytes, &pp.full[pp.slot()]);
     ++pp.it;
   }
 }
@@ -242,17 +250,18 @@ struct Consumer {
 // of one tile of an activation / dZ image, so it doubles as the staging buffer of the image's bulk store
 __host__ __device__ __forceinline__ int tile_off(int m, int col) { return (col >> 6) * ATOM_BYTES + atom_off(m, col & 63); }
 
-// One 32 KB weight item (B: 256 rows x 64 k, K-major SW128) against a 64-column A chunk of this warpgroup's rows:
-// D += A_hi * B (+ A_lo * B when with_lo).  The item read before this one is released once its MMAs have completed.
+// One 16 KB weight item (B: 256 rows x 32 k, K-major SW64) against 32 columns of this warpgroup's rows of the A tile
+// (a_hi / a_lo: their first column inside a 64-column atom block): D += A_hi * B (+ A_lo * B when with_lo), one k16
+// step after the other.  The item read before this one is released once its MMAs have completed.
 template <int NST, int NN>
 __device__ __forceinline__ void consume_item(Pipe<NST>& pp, float (&acc)[NN / 2], uint32_t a_hi, uint32_t a_lo, bool with_lo,
                                              uint32_t& scale, int& pending, const Consumer& c) {
   mbar_wait(&pp.full[pp.slot()], pp.parity());
-  const uint32_t sb = smem_u32(pp.stage + pp.slot() * STAGE_BYTES);
+  const uint32_t sb = smem_u32(pp.stage + pp.slot() * ITEM_BYTES);
   wgmma_fence();
 #pragma unroll
-  for (int ks = 0; ks < 4; ++ks) {
-    const uint64_t bd = make_desc(sb + ks * 32, 16, 1024);
+  for (int ks = 0; ks < 2; ++ks) {
+    const uint64_t bd = make_desc_sw64(sb + ks * 32, 512);
     if constexpr (NN == 256) wgmma_n256<0, 0>(*reinterpret_cast<float(*)[128]>(&acc), make_desc(a_hi + ks * 32, 16, 1024), bd, scale);
     else wgmma_n64<0, 0>(*reinterpret_cast<float(*)[32]>(&acc), make_desc(a_hi + ks * 32, 16, 1024), bd, scale);
     scale = 1u;
@@ -267,12 +276,15 @@ __device__ __forceinline__ void consume_item(Pipe<NST>& pp, float (&acc)[NN / 2]
   pending = pp.slot();
   ++pp.it;
 }
-// MMAs of one 64-wide k chunk:  D += A_hi*B_hi + A_lo*B_hi  (B_hi item)  then  D += A_hi*B_lo  (B_lo item)
+// MMAs of one 64-wide k chunk, per k16 step:  D += A_hi*B_hi + A_lo*B_hi  (two B_hi items)  then  D += A_hi*B_lo  (two
+// B_lo items); 64 bytes of an A row are 32 columns
 template <int NST, int NN>
 __device__ __forceinline__ void consume_chunk(Pipe<NST>& pp, float (&acc)[NN / 2], uint32_t a_hi, uint32_t a_lo,
                                               uint32_t& scale, int& pending, const Consumer& c) {
   consume_item<NST, NN>(pp, acc, a_hi, a_lo, true, scale, pending, c);
+  consume_item<NST, NN>(pp, acc, a_hi + 64, a_lo + 64, true, scale, pending, c);
   consume_item<NST, NN>(pp, acc, a_hi, a_lo, false, scale, pending, c);
+  consume_item<NST, NN>(pp, acc, a_hi + 64, a_lo + 64, false, scale, pending, c);
 }
 template <int NST, int R>
 __device__ __forceinline__ void finish_pass(Pipe<NST>& pp, float (&acc)[R], int& pending, const Consumer& c) {
@@ -330,17 +342,22 @@ __device__ __forceinline__ float rows_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 16);
 }
 
-// dynamic shared memory map: [A tile hi 64 KB | lo 64 KB][weight stages][aux tile 32 KB (atlas forward)][consts][barriers]
+// dynamic shared memory map: [A tile hi 64 KB | lo 64 KB][weight ring][aux tile 32 KB (atlas forward)][consts][barriers]
 constexpr int SMEM_A = 2 * TILE_IMG_BYTES;
 constexpr int SMEM_AUX = 2 * ATOM_BYTES;
 constexpr int SMEM_BWD_CONST_FLOATS = 7 * 256 + 768;         // bias-gradient accumulators (+ dW0 of the mapping)
 constexpr int SMEM_BARS = 256;
-// The forward kernels keep as many 32 KB weight stages as the 227 KB of shared memory allow next to the A tile (and the
-// atlas's positional-encoding tile); the backward kernels need room for their gradient accumulators.
+constexpr int SMEM_MAX = 227 * 1024;                         // opt-in shared memory of one sm_90 CTA
+// Every kernel keeps as many 16 KB weight slots as the shared memory allows next to the A tile and, in the atlas
+// forward, the positional-encoding tile (6 mapping forward, 4 atlas forward); the backward kernels also hold their
+// gradient accumulators (5 slots).
 template <bool ATLAS, bool BWD> struct KCfg {
-  static constexpr int NST = (BWD || ATLAS) ? 2 : 3;
-  static constexpr int SMEM = SMEM_A + NST * STAGE_BYTES + (ATLAS && !BWD ? SMEM_AUX : 0) +
+  static constexpr int NST = BWD ? 5 : (ATLAS ? 4 : 6);
+  static constexpr int SMEM = SMEM_A + NST * ITEM_BYTES + (ATLAS && !BWD ? SMEM_AUX : 0) +
                               (BWD ? SMEM_BWD_CONST_FLOATS * 4 : 0) + SMEM_BARS;
+  static_assert(SMEM <= SMEM_MAX, "fused kernel exceeds the shared memory of one CTA");
+  static_assert(SMEM + ITEM_BYTES > SMEM_MAX, "one more weight slot would fit");
+  static_assert(2 * NST * 8 <= SMEM_BARS, "ring barriers exceed their shared-memory slot");
 };
 
 template <int NST>
@@ -350,7 +367,7 @@ struct SmemMap {
   __device__ __forceinline__ void init(char* raw, int aux_bytes, int cst_floats) {
     char* p = raw;                                   // 1024-aligned (checked in setup_cta)
     a_tile = p; p += SMEM_A;
-    stage = p; p += NST * STAGE_BYTES;
+    stage = p; p += NST * ITEM_BYTES;
     aux = p; p += aux_bytes;
     cst = reinterpret_cast<float*>(p); p += cst_floats * 4;
     full = reinterpret_cast<uint64_t*>(p);
@@ -419,9 +436,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_fwd_kernel(const __grid_cons
       for (int t = blockIdx.x; t < ti.total; t += gridDim.x)
         for (int l = FIRST_TC; l <= LAST_TC; ++l) {
           const char* base = P.img.w_fwd + P.img.w_fwd_layer[l];
-          if (ATLAS && l == 0) { produce_items(pp, base, 2); continue; }
-          if (SKIPS && l == 4) produce_items(pp, base + (int64_t)4 * 2 * STAGE_BYTES, 2);      // skip (PE) chunk first
-          produce_items(pp, base, 8);
+          if (ATLAS && l == 0) { produce_items(pp, base, 4); continue; }
+          if (SKIPS && l == 4) produce_items(pp, base + (int64_t)4 * CHUNK_BYTES, 4);      // skip (PE) chunk first
+          produce_items(pp, base, 16);
         }
     }
     return;
@@ -675,7 +692,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_bwd_kernel(const __grid_cons
     if (warp == CONSUMER_WGS * 4 && lane == 0) {
       Pipe<NST> pp{sm.full, sm.empty, sm.stage, 0};
       for (int t = blockIdx.x; t < ti.total; t += gridDim.x)
-        for (int l = L - 2; l >= (HAS_DPE ? 0 : LOW); --l) produce_items(pp, P.img.w_bwd + P.img.w_bwd_layer[l], 8);
+        for (int l = L - 2; l >= (HAS_DPE ? 0 : LOW); --l)
+          produce_items(pp, P.img.w_bwd + P.img.w_bwd_layer[l], 16, l == 0 ? 64 * 64 : ITEM_BYTES);   // dPE: 64 rows
     }
     return;
   }
@@ -818,8 +836,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_bwd_kernel(const __grid_cons
                         P.img.term_stride);
     }
     if (HAS_DPE) {
-      // ---------------- dPE = dZ_0 W_0 (64 columns, 40 real) -> d(in) -> d_in += in_scale * d(in)
-      float acc64[32];
+      // ---------------- dPE = dZ_0 W_0 (64 columns, 40 real) -> d(in) -> d_in += in_scale * d(in); the accumulator is
+      // the first 32 registers of acc (a separate one next to it serialises the kernel's wgmma for lack of registers)
+      float (&acc64)[32] = *reinterpret_cast<float(*)[32]>(&acc);
       uint32_t scale = 0u;
       for (int kc = 0; kc < 4; ++kc)
         consume_chunk<NST, 64>(pp, acc64, a_rows + kc * ATOM_BYTES, a_rows + TILE_IMG_BYTES + kc * ATOM_BYTES, scale,
@@ -1193,7 +1212,7 @@ static BwdParams fill_bwd(const MlpShape& sh, const NetImages& im, const float* 
 static void add_prep(PrepJobs& pj, const float* W, int ldw, int n_rows, int k0, int k_cnt, int transpose, char* dst) {
   PrepJob& j = pj.j[pj.n++];
   j.W = W; j.ldw = ldw; j.n_rows = n_rows; j.k0 = k0; j.k_cnt = k_cnt; j.transpose = transpose;
-  j.hi = dst; j.lo = dst + STAGE_BYTES;
+  j.hi = dst; j.lo = dst + 2 * ITEM_BYTES;
 }
 
 static void prep_jobs_for_net(PrepJobs& pj, const MlpShape& sh, const NetImages& im, const float* pp, TcNet net,
@@ -1203,10 +1222,10 @@ static void prep_jobs_for_net(PrepJobs& pj, const MlpShape& sh, const NetImages&
     char* dst = im.w_fwd + im.w_fwd_layer[l];
     if (im.n_chunks_fwd[l] == 0) continue;
     const float* W = pp + sh.w_off[l];
-    int item = 0;
-    if (l > 0) for (int kc = 0; kc < 4; ++kc) add_prep(pj, W, sh.K[l], 256, kc * 64, 64, 0, dst + (int64_t)(item++) * 2 * STAGE_BYTES);
+    int chunk = 0;
+    if (l > 0) for (int kc = 0; kc < 4; ++kc) add_prep(pj, W, sh.K[l], 256, kc * 64, 64, 0, dst + (int64_t)(chunk++) * CHUNK_BYTES);
     if (pe && (l == 0 || sh.skip[l]))
-      add_prep(pj, W, sh.K[l], 256, l == 0 ? 0 : 256, sh.enc, 0, dst + (int64_t)(item++) * 2 * STAGE_BYTES);
+      add_prep(pj, W, sh.K[l], 256, l == 0 ? 0 : 256, sh.enc, 0, dst + (int64_t)(chunk++) * CHUNK_BYTES);
   }
   if (!with_bwd) return;
   for (int l = 0; l < sh.L - 1; ++l) {
@@ -1215,7 +1234,7 @@ static void prep_jobs_for_net(PrepJobs& pj, const MlpShape& sh, const NetImages&
     const float* W = pp + sh.w_off[l];
     // image rows = input index k of layer l (256, or 40 for atlas layer 0), chunk over the output index n
     const int rows = (pe && l == 0) ? sh.enc : 256;
-    for (int kc = 0; kc < 4; ++kc) add_prep(pj, W, sh.K[l], rows, kc * 64, 64, 1, dst + (int64_t)kc * 2 * STAGE_BYTES);
+    for (int kc = 0; kc < 4; ++kc) add_prep(pj, W, sh.K[l], rows, kc * 64, 64, 1, dst + (int64_t)kc * CHUNK_BYTES);
   }
 }
 

@@ -162,6 +162,16 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_b
   d |= (uint64_t)1 << 62;
   return d;
 }
+// K-major 64-byte swizzle (layout type 2): rows of 64 B (32 fp16 k), 16-byte chunk index XOR-ed with (row / 2) % 4,
+// SBO = stride of 8-row groups (512 B when dense); LBO unused
+__device__ __forceinline__ uint64_t make_desc_sw64(uint32_t smem_addr, uint32_t sbo_bytes) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
+  d |= (uint64_t)2 << 62;
+  return d;
+}
 
 // ------------------------------------------------------------------------------------ fp16 split
 // v -> (hi, lo) with hi = rn_f16(v), lo = rn_f16(v - hi); saturating (no inf).  v must already be scaled.
