@@ -216,6 +216,63 @@ def check_architecture(config: dict):
                           "Use the IMLP class + src/models/stage_1/loss_utils.py (any shape) for other architectures.")
 
 
+class FusedDp:
+    """Symmetric (peer-mapped) allocations for b200_dp_adam_step: the parameters, the [gradients || losses] buffer and
+    the flag words, with the communicator that names every rank's copies.  torch's symmetric-memory allocator does the
+    rendezvous (plumbing); the exchange itself is this library's kernel.  With it a rank keeps the Adam moments of its
+    own slice only (gather_moments assembles them)."""
+
+    def __init__(self, pg, device, n_params: int, n_losses: int):
+        import torch.distributed as dist
+        import torch.distributed._symmetric_memory as symm
+        self.pg, self.world = pg, dist.get_world_size(pg)
+        self.n_params, self.n_total = n_params, n_params + n_losses
+        self.params = symm.empty(n_params, dtype=torch.float32, device=device)
+        self.grad_loss = symm.empty(self.n_total, dtype=torch.float32, device=device)
+        self.flags = symm.empty(2 * N.MAX_RANKS, dtype=torch.int64, device=device)
+        self.params.zero_(); self.grad_loss.zero_(); self.flags.zero_()
+        self.handles = [symm.rendezvous(t, pg) for t in (self.grad_loss, self.params, self.flags)]
+        self.comm = N.DpComm()
+        self.comm.world, self.comm.rank = self.world, dist.get_rank(pg)
+        for j in range(self.world):
+            self.comm.partials[j] = int(self.handles[0].buffer_ptrs[j])
+            self.comm.params[j] = int(self.handles[1].buffer_ptrs[j])
+            self.comm.flags[j] = int(self.handles[2].buffer_ptrs[j])
+        self.epoch = torch.zeros(1, dtype=torch.int64, device=device)
+        torch.cuda.synchronize(device)
+        dist.barrier(pg)
+
+    @classmethod
+    def create(cls, pg, device, n_params: int, n_losses: int, required: bool) -> Optional["FusedDp"]:
+        """The fused optimiser, or None (-> NCCL all-reduce + local Adam) when the allocator is unavailable and
+        `required` is false."""
+        try:
+            return cls(pg, device, n_params, n_losses)
+        except Exception as e:                      # noqa: BLE001 - any allocator / rendezvous failure
+            if required:
+                raise
+            import sys
+            print(f"b200: fused data-parallel optimiser unavailable ({type(e).__name__}: {e}); "
+                  f"using NCCL all-reduce + local Adam", file=sys.stderr)
+            return None
+
+    def adam_step(self, exp_avg, exp_avg_sq, lr: float, step_count):
+        """reduce-scatter + Adam + all-gather in one kernel (b200_dp_adam_step)."""
+        N.check(N.lib().b200_dp_adam_step(C.byref(self.comm), N.ptr(exp_avg), N.ptr(exp_avg_sq), self.n_params,
+                                          self.n_total, lr, 0.9, 0.999, 1e-8, N.ptr(step_count), N.ptr(self.epoch),
+                                          N.current_stream()), "b200_dp_adam_step")
+
+    def gather_moments(self, exp_avg, exp_avg_sq):
+        """Assemble the full Adam moments (checkpoint time) with one all-reduce of the owned slices.  Collective."""
+        import torch.distributed as dist
+        b, c = C.c_int64(), C.c_int64()
+        N.check(N.lib().b200_dp_slice(self.world, self.comm.rank, self.n_total, C.byref(b), C.byref(c)))
+        lo, hi = min(b.value, self.n_params), min(b.value + c.value, self.n_params)
+        for t in (exp_avg, exp_avg_sq):
+            t[:lo].zero_(); t[hi:].zero_()
+            dist.all_reduce(t, group=self.pg)
+
+
 class AtlasTrainer:
     """Flat parameters/optimiser state of (mapping, atlas) + the fused step."""
 
@@ -248,10 +305,12 @@ class AtlasTrainer:
         # gradients + the loss vector share one buffer so that data parallelism needs ONE exchange
         self._dp = None
         if self.world > 1 and dev.type == "cuda" and fused_dp is not False:
-            self._dp = self._setup_fused_dp(required=bool(fused_dp))
+            self._dp = FusedDp.create(process_group, dev, self.n_params, N.LOSS_FLOATS, required=bool(fused_dp))
         if self._dp is None:
             self.params = torch.zeros(self.n_params, dtype=torch.float32, device=dev)
             self.grad_loss = torch.zeros(self.n_params + N.LOSS_FLOATS, dtype=torch.float32, device=dev)
+        else:
+            self.params, self.grad_loss = self._dp.params, self._dp.grad_loss
         self.grads = self.grad_loss[:self.n_params]
         self.losses = self.grad_loss[self.n_params:]
         self.exp_avg = torch.zeros_like(self.params)
@@ -385,58 +444,15 @@ class AtlasTrainer:
                 "b200_atlas_loss_grad_for")
 
     # ------------------------------------------------------------------ data parallelism over NVLink peer memory
-    def _setup_fused_dp(self, required: bool):
-        """Symmetric (peer-mapped) allocations for b200_dp_adam_step: parameters, the [gradients || losses] buffer and
-        the flag words.  torch's symmetric-memory allocator does the rendezvous (plumbing); the exchange itself is
-        this library's kernel.  Returns the communicator struct, or None (-> NCCL all-reduce + local Adam) when the
-        allocator is unavailable."""
-        try:
-            import torch.distributed as dist
-            import torch.distributed._symmetric_memory as symm
-            dev, n = self.device, self.n_params + N.LOSS_FLOATS
-            self.params = symm.empty(self.n_params, dtype=torch.float32, device=dev)
-            self.grad_loss = symm.empty(n, dtype=torch.float32, device=dev)
-            self._dp_flags = symm.empty(2 * N.MAX_RANKS, dtype=torch.int64, device=dev)
-            self.params.zero_(); self.grad_loss.zero_(); self._dp_flags.zero_()
-            handles = [symm.rendezvous(t, self.pg) for t in (self.grad_loss, self.params, self._dp_flags)]
-            comm = N.DpComm()
-            comm.world, comm.rank = self.world, dist.get_rank(self.pg)
-            for j in range(self.world):
-                comm.partials[j] = int(handles[0].buffer_ptrs[j])
-                comm.params[j] = int(handles[1].buffer_ptrs[j])
-                comm.flags[j] = int(handles[2].buffer_ptrs[j])
-            self._dp_handles = handles
-            self._dp_epoch = torch.zeros(1, dtype=torch.int64, device=dev)
-            torch.cuda.synchronize(dev)
-            dist.barrier(self.pg)
-            return comm
-        except Exception as e:                      # noqa: BLE001 - any allocator / rendezvous failure
-            if required:
-                raise
-            import sys
-            print(f"b200: fused data-parallel optimiser unavailable ({type(e).__name__}: {e}); "
-                  f"using NCCL all-reduce + local Adam", file=sys.stderr)
-            return None
-
     def dp_adam(self):
         """reduce-scatter + Adam + all-gather in one kernel (b200_dp_adam_step)."""
-        N.check(self.lib.b200_dp_adam_step(C.byref(self._dp), N.ptr(self.exp_avg), N.ptr(self.exp_avg_sq), self.n_params,
-                                           self.n_params + N.LOSS_FLOATS, self.lr, 0.9, 0.999, 1e-8,
-                                           N.ptr(self.step_count), N.ptr(self._dp_epoch), N.current_stream()),
-                "b200_dp_adam_step")
+        self._dp.adam_step(self.exp_avg, self.exp_avg_sq, self.lr, self.step_count)
 
     def gather_moments(self):
         """With the fused optimiser a rank maintains only the Adam moments of its slice: assemble the full state
         (checkpoint time) with one all-reduce of the owned slices."""
-        if self._dp is None:
-            return
-        import torch.distributed as dist
-        b, c = C.c_int64(), C.c_int64()
-        N.check(self.lib.b200_dp_slice(self.world, self._dp.rank, self.n_params + N.LOSS_FLOATS, C.byref(b), C.byref(c)))
-        lo, hi = min(b.value, self.n_params), min(b.value + c.value, self.n_params)
-        for t in (self.exp_avg, self.exp_avg_sq):
-            t[:lo].zero_(); t[hi:].zero_()
-            dist.all_reduce(t, group=self.pg)
+        if self._dp is not None:
+            self._dp.gather_moments(self.exp_avg, self.exp_avg_sq)
 
     def all_reduce(self):
         if self.pg is not None and self.world > 1:

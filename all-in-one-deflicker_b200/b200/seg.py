@@ -17,7 +17,7 @@ import numpy as np
 import torch
 
 from . import _native as N
-from .atlas import DeviceVideo, layer_dims, make_desc, mlp_layout
+from .atlas import DeviceVideo, FusedDp, layer_dims, make_desc, mlp_layout
 
 # hyper-parameters of src/config/config_flow_100.json that the seg loop reads
 SEG_DEFAULTS = dict(
@@ -51,17 +51,27 @@ def seg_descs(c: dict) -> Dict[str, N.MlpDesc]:
                         int(c["positional_encoding_num_atlas"]), (4, 7)))
 
 
-def pack_mask_frames(mask_frames: torch.Tensor, device) -> torch.Tensor:
-    """(H, W, T) bootstrapping mask of load_input_data (unwrap_utils.py:52,68-70) -> frame-major [T][H][W] on the
-    device, so that entry n of the flat buffer is pixel n of the index table."""
-    return mask_frames.permute(2, 0, 1).contiguous().to(device=device, dtype=torch.float32)
+def pack_mask_frames(mask_frames: torch.Tensor, device, t_begin: int = 0, t_end: Optional[int] = None) -> torch.Tensor:
+    """(H, W, T) bootstrapping mask of load_input_data (unwrap_utils.py:52,68-70) -> frame-major [T'][H][W] on the
+    device for the resident frames [t_begin, t_end) (default: all), so that entry n of the flat buffer is pixel
+    n + t_begin*H*W of the index table.  A frame shard's trainer takes the matte of its own frames only."""
+    return mask_frames[:, :, t_begin:t_end].permute(2, 0, 1).contiguous().to(device=device, dtype=torch.float32)
 
 
 class SegTrainer:
-    """Flat parameters / optimiser state of (mapping1, mapping2, alpha, atlas) + the seg step."""
+    """Flat parameters / optimiser state of (mapping1, mapping2, alpha, atlas) + the seg step.
+
+    Frame-sharded data parallelism: with a `process_group`, `video` holds this rank's frame block (DeviceVideo with
+    t_begin / t_end and the whole-video bitmaps) and `mask` the matte of those frames (pack_mask_frames(..., t_begin,
+    t_end)); every rank draws the same index batch.  A rank's trip normalises by the global batch and flow counts,
+    so one SUM over the ranks of [gradients || loss vector] gives the unsharded trip (loss entries 12, 13, the flow
+    counts, then read world * count).  The exchange is b200_dp_adam_step over symmetric memory (FusedDp) when
+    available -- `fused_dp` True requires it, also on one rank; False or a failed set-up use NCCL all-reduce + the
+    local Adam."""
 
     def __init__(self, video: Optional[DeviceVideo], mask: Optional[torch.Tensor], config: Optional[dict] = None,
-                 precision: int = N.PREC_FP32, device="cuda", lr: float = 1e-4, resx: Optional[int] = None):
+                 precision: int = N.PREC_FP32, device="cuda", lr: float = 1e-4, resx: Optional[int] = None,
+                 process_group=None, fused_dp: Optional[bool] = None):
         self.lib = N.lib()
         self.video, self.mask = video, mask
         self.cfg = dict(SEG_DEFAULTS)
@@ -80,11 +90,23 @@ class SegTrainer:
         self.offsets = dict(zip(NETS, [int(o) for o in offs]))
         self.layouts = {k: mlp_layout(self.descs[k]) for k in NETS}
         dev = self.device
-        self.params = torch.zeros(self.n_params, dtype=torch.float32, device=dev)
-        self.grads = torch.zeros_like(self.params)
+        self.pg, self.world = process_group, 1
+        if process_group is not None:
+            import torch.distributed as dist
+            self.world = dist.get_world_size(process_group)
+        # gradients + the loss vector share one buffer so that data parallelism needs ONE exchange
+        self._dp = None
+        if process_group is not None and dev.type == "cuda" and fused_dp is not False and (self.world > 1 or fused_dp):
+            self._dp = FusedDp.create(process_group, dev, self.n_params, N.SEG_LOSS_FLOATS, required=bool(fused_dp))
+        if self._dp is None:
+            self.params = torch.zeros(self.n_params, dtype=torch.float32, device=dev)
+            self.grad_loss = torch.zeros(self.n_params + N.SEG_LOSS_FLOATS, dtype=torch.float32, device=dev)
+        else:
+            self.params, self.grad_loss = self._dp.params, self._dp.grad_loss
+        self.grads = self.grad_loss[:self.n_params]
+        self.losses = self.grad_loss[self.n_params:]
         self.exp_avg = torch.zeros_like(self.params)
         self.exp_avg_sq = torch.zeros_like(self.params)
-        self.losses = torch.zeros(N.SEG_LOSS_FLOATS, dtype=torch.float32, device=dev)
         self.step_count = torch.zeros(1, dtype=torch.int64, device=dev)
         B = int(self.cfg["samples_batch"])
         self.indices = torch.zeros(B, dtype=torch.int64, device=dev)
@@ -133,7 +155,9 @@ class SegTrainer:
         return {k: v.detach().clone() for k, v in self.param_views(which).items()}
 
     def optimizer_state_dict(self):
-        """Schema of torch.optim.Adam.state_dict() for the four groups of :165-169 (what evaluate.py:223 stores)."""
+        """Schema of torch.optim.Adam.state_dict() for the four groups of :165-169 (what evaluate.py:223 stores).
+        Collective under the fused optimiser: every rank calls it."""
+        self.gather_moments()
         state, groups, idx = {}, [], 0
         step = self.step_count.detach().float().cpu().reshape(())
         for which in NETS:
@@ -198,14 +222,33 @@ class SegTrainer:
                                         0.9, 0.999, 1e-8, 1.0, N.ptr(self.step_count if step is None else step),
                                         N.current_stream()), "b200_adam_step")
 
+    def dp_adam(self):
+        """reduce-scatter + Adam + all-gather in one kernel (b200_dp_adam_step)."""
+        self._dp.adam_step(self.exp_avg, self.exp_avg_sq, self.lr, self.step_count)
+
+    def gather_moments(self):
+        """Under the fused optimiser a rank keeps the Adam moments of its slice only: assemble them (collective)."""
+        if self._dp is not None:
+            self._dp.gather_moments(self.exp_avg, self.exp_avg_sq)
+
+    def all_reduce(self):
+        if self.pg is not None and self.world > 1:
+            import torch.distributed as dist
+            dist.all_reduce(self.grad_loss, group=self.pg)      # one collective: gradients || loss vector
+
     def _iteration(self, it: int):
         self.loss_grad(it)
-        self.adam()
+        if self._dp is not None:
+            self.dp_adam()
+        else:
+            self.all_reduce()
+            self.adam()
 
     def step(self, it: int, use_graph: bool = True):
-        """One loop trip on the indices in self.indices (device): losses + gradients, then one Adam update of all four
-        networks (same lr / betas in every group, so one sweep over the flat buffer).  The trip is captured once per
-        regime (global rigidity on / off, bootstrapping on / off) in a CUDA graph and replayed."""
+        """One loop trip on the indices in self.indices (device): losses + gradients, the exchange between ranks (if
+        any), then one Adam update of all four networks (same lr / betas in every group, so one sweep over the flat
+        buffer).  The trip is captured once per regime (global rigidity on / off, bootstrapping on / off) in a CUDA
+        graph and replayed."""
         if not use_graph or self.device.type != "cuda":
             self._iteration(it)
             return self.losses

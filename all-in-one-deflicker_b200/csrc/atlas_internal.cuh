@@ -19,9 +19,11 @@ struct SampleGeom {
 int launch_video_pack(const float* fr, const float* dx, const float* dy, const float* ff, const float* fb,
                       const float* mf, const float* mb, int H, int W, int T, int t_begin, int t_end,
                       float* rec, uint32_t* bits_f, uint32_t* bits_b, cudaStream_t st);
+// matte: bootstrapping matte of the resident frames, frame-major [t_end - t_begin][H][W] (segmentation variant), copied
+// into target column 11; null: column 11 stays zero (single-layer variant)
 int launch_select_sample(const int64_t* indices, int B, const B200Video& vid, const SampleGeom& geo, int cap,
                          int n_groups, int* counters, int* list, float* x_map, float* targets,
-                         cudaStream_t st);
+                         cudaStream_t st, const float* matte = nullptr);
 int launch_pretrain_sample(const int64_t* ys, const int64_t* xs, int B, int cap, float half_larger,
                            float t_norm, float* x_map, int* counters, cudaStream_t st);
 int launch_pretrain_loss(const float* x_map, const float* uv, int B, int cap, float uv_scale, float* d_uv,

@@ -96,8 +96,8 @@ __device__ __forceinline__ int warp_claim(bool take, int* counter, int lane) {
 
 template <bool ALL_LOCAL>
 __global__ void sample_kernel(const int64_t* __restrict__ indices, int* __restrict__ counters, B200Video vid,
-                              SampleGeom geo, int cap, int batch, int n_groups, float4* __restrict__ x_map,
-                              float* __restrict__ targets) {
+                              SampleGeom geo, int cap, int batch, int n_groups, const float* __restrict__ matte,
+                              float4* __restrict__ x_map, float* __restrict__ targets) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;      // index into the global batch (or a padding slot)
   const int lane = threadIdx.x & 31;
   bool local = false, wf = false, wb = false, gf = false, gb = false;
@@ -165,7 +165,9 @@ __global__ void sample_kernel(const int64_t* __restrict__ indices, int* __restri
     float4* tdst = reinterpret_cast<float4*>(targets + (int64_t)s * TARGET_FLOATS);
     tdst[0] = make_float4(v[0], v[1], v[2], v[3]);
     tdst[1] = make_float4(v[4], v[5], v[6], v[7]);
-    tdst[2] = make_float4(v[8], wf ? (float)(pf + 1) : 0.f, wb ? (float)(pb + 1) : 0.f, 0.f);
+    // column 11: the sample's matte value, which travels with its slot (slot order is not batch order on a shard)
+    const float a_gt = matte ? matte[((int64_t)(t - vid.t_begin) * vid.H + y) * vid.W + x] : 0.f;
+    tdst[2] = make_float4(v[8], wf ? (float)(pf + 1) : 0.f, wb ? (float)(pb + 1) : 0.f, a_gt);
   } else if (ALL_LOCAL && b < cap) {
     // padding slots of the last tile: finite rows, zero targets
 #pragma unroll
@@ -178,14 +180,14 @@ __global__ void sample_kernel(const int64_t* __restrict__ indices, int* __restri
 
 int launch_select_sample(const int64_t* indices, int B, const B200Video& vid, const SampleGeom& geo, int cap,
                          int n_groups, int* counters, int* list, float* x_map, float* targets,
-                         cudaStream_t st) {
+                         cudaStream_t st, const float* matte) {
   (void)list;
   B200_CHECK_CUDA(cudaMemsetAsync(counters, 0, 32, st));
   if (vid.t_begin == 0 && vid.t_end == vid.T)
-    sample_kernel<true><<<(cap + 127) / 128, 128, 0, st>>>(indices, counters, vid, geo, cap, B, n_groups,
+    sample_kernel<true><<<(cap + 127) / 128, 128, 0, st>>>(indices, counters, vid, geo, cap, B, n_groups, matte,
                                                             reinterpret_cast<float4*>(x_map), targets);
   else
-    sample_kernel<false><<<(B + 127) / 128, 128, 0, st>>>(indices, counters, vid, geo, cap, B, n_groups,
+    sample_kernel<false><<<(B + 127) / 128, 128, 0, st>>>(indices, counters, vid, geo, cap, B, n_groups, matte,
                                                            reinterpret_cast<float4*>(x_map), targets);
   B200_CHECK_LAUNCH();
   return B200_OK;

@@ -270,16 +270,18 @@ static int mlp_prepare(const B200MlpDesc* d, int64_t rows, void* ws, int64_t ws_
   return B200_OK;
 }
 
-int b200_mlp_forward(const B200MlpDesc* d, const float* params, const float* x, float* y, int64_t rows,
-                     int training, int precision, void* ws, int64_t ws_bytes, void* stream) {
+// live: the live rows of a group-major batch of `rows` rows (a multiple of 128), or null: all rows
+static int mlp_forward_impl(const B200MlpDesc* d, const float* params, const float* x, float* y, int64_t rows,
+                            const TcRows* live, int training, int precision, void* ws, int64_t ws_bytes,
+                            cudaStream_t st) {
   MlpShape s; MlpScratch sc; RowSpan span;
   B200_REQUIRE(params && x && y, "null pointer");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (precision == B200_PREC_TC) {
     TcNet net; int64_t rows_pad; TcCallPlan pl;
     B200_PROPAGATE(tc_call_prepare(d, rows, ws, ws_bytes, &s, &net, &rows_pad, &pl));
     B200_PROPAGATE(launch_pack_rows(x, s.in_dim, s.in_dim, pl.x, net == TcNet::Atlas ? 2 : 4, rows, rows_pad, st));
-    B200_PROPAGATE(tc_single_forward(s, net, params, pl.x, pl.y, rows_pad, training != 0, pl.tc, g_persistent_ws, st));
+    B200_PROPAGATE(tc_single_forward(s, net, params, pl.x, pl.y, live ? *live : tc_all_rows(rows_pad), training != 0,
+                                     pl.tc, g_persistent_ws, st));
     B200_CHECK_CUDA(cudaMemcpyAsync(y, pl.y, (size_t)rows * s.out_dim * 4, cudaMemcpyDeviceToDevice, st));
     return B200_OK;
   }
@@ -302,12 +304,17 @@ int b200_mlp_forward(const B200MlpDesc* d, const float* params, const float* x, 
   return B200_OK;
 }
 
-int b200_mlp_backward(const B200MlpDesc* d, const float* params, const float* x, const float* dy,
-                      float* dparams, float* dx, int64_t rows, int precision, void* ws, int64_t ws_bytes,
-                      void* stream) {
+int b200_mlp_forward(const B200MlpDesc* d, const float* params, const float* x, float* y, int64_t rows,
+                     int training, int precision, void* ws, int64_t ws_bytes, void* stream) {
+  return mlp_forward_impl(d, params, x, y, rows, nullptr, training, precision, ws, ws_bytes,
+                          reinterpret_cast<cudaStream_t>(stream));
+}
+
+static int mlp_backward_impl(const B200MlpDesc* d, const float* params, const float* x, const float* dy,
+                             float* dparams, float* dx, int64_t rows, const TcRows* live, int precision, void* ws,
+                             int64_t ws_bytes, cudaStream_t st) {
   MlpShape s; MlpScratch sc; RowSpan span;
   B200_REQUIRE(params && dy && dparams && x, "null pointer");
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (precision == B200_PREC_TC) {
     // the workspace still holds the padded input, the outputs and the activation images of the forward call
     TcNet net; int64_t rows_pad; TcCallPlan pl;
@@ -318,7 +325,7 @@ int b200_mlp_backward(const B200MlpDesc* d, const float* params, const float* x,
     B200_CHECK_CUDA(cudaMemsetAsync(pl.gmax2, 0, 8, st));
     B200_PROPAGATE(launch_absmax(pl.dy, rows_pad * s.out_dim, pl.gmax2 + (tc_net_is_mapping(net) ? 1 : 0), st));
     B200_PROPAGATE(tc_single_backward(s, net, params, dparams, pl.x, pl.y, pl.dy, (tc_net_has_dpe(net) && dx) ? pl.d_in : nullptr,
-                                      pl.gmax2, rows_pad, pl.tc, g_persistent_ws, st));
+                                      pl.gmax2, live ? *live : tc_all_rows(rows_pad), pl.tc, g_persistent_ws, st));
     if (tc_net_has_dpe(net) && dx) B200_CHECK_CUDA(cudaMemcpyAsync(dx, pl.d_in, (size_t)rows * 8, cudaMemcpyDeviceToDevice, st));
     return B200_OK;
   }
@@ -343,6 +350,13 @@ int b200_mlp_backward(const B200MlpDesc* d, const float* params, const float* x,
     B200_PROPAGATE(simt_mlp_backward(s, params, x, s.in_dim, span, sc, dy, dparams, dx, s.in_dim, st));
   }
   return B200_OK;
+}
+
+int b200_mlp_backward(const B200MlpDesc* d, const float* params, const float* x, const float* dy,
+                      float* dparams, float* dx, int64_t rows, int precision, void* ws, int64_t ws_bytes,
+                      void* stream) {
+  return mlp_backward_impl(d, params, x, dy, dparams, dx, rows, nullptr, precision, ws, ws_bytes,
+                           reinterpret_cast<cudaStream_t>(stream));
 }
 
 int b200_video_pack(const float* frames, const float* frames_dx, const float* frames_dy, const float* flow_fwd,
@@ -651,3 +665,17 @@ int b200_render_for(const B200MlpDesc* mapping, const float* params, int32_t H, 
 }
 
 }  // extern "C"
+
+namespace b200 {
+
+int mlp_forward_rows(const B200MlpDesc* d, const float* params, const float* x, float* y, const TcRows& live,
+                     int training, int precision, void* ws, int64_t ws_bytes, cudaStream_t st) {
+  return mlp_forward_impl(d, params, x, y, live.rows(), &live, training, precision, ws, ws_bytes, st);
+}
+
+int mlp_backward_rows(const B200MlpDesc* d, const float* params, const float* x, const float* dy, float* dparams,
+                      float* dx, const TcRows& live, int precision, void* ws, int64_t ws_bytes, cudaStream_t st) {
+  return mlp_backward_impl(d, params, x, dy, dparams, dx, live.rows(), &live, precision, ws, ws_bytes, st);
+}
+
+}  // namespace b200

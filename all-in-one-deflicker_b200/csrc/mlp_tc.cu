@@ -185,19 +185,20 @@ struct Pipe {                        // weight-image ring shared by the producer
 };
 
 struct TileIter {                    // static round-robin over the live tiles of a group-major batch
-  int t0, tf, tb, total, cap_tiles, n_groups, flow;
-  // counters: [0] rows of an ordinary group, [5] / [6] rows of the compacted flow-match groups (G_FWD = 5, G_BWD = 6
-  // of the mapping batch when `flow_groups` is set); nullptr: every row of every group is live
-  __device__ __forceinline__ void init(int cap, int groups, const int* counters, int flow_groups) {
+  int t0, tf, tb, total, cap_tiles, n_groups, gf, gb;
+  // counters: [0] rows of an ordinary group, [5] / [6] rows of the compacted flow-match groups g_fwd / g_bwd (-1: the
+  // batch has no such group); nullptr: every row of every group is live
+  __device__ __forceinline__ void init(int cap, int groups, const int* counters, int g_fwd, int g_bwd) {
     cap_tiles = cap / TM;
     n_groups = groups;
-    flow = (flow_groups && groups > 6) ? 1 : 0;
+    gf = (counters && g_fwd < groups) ? g_fwd : -1;
+    gb = (counters && g_bwd < groups) ? g_bwd : -1;
     t0 = counters ? min(cap_tiles, (counters[0] + TM - 1) / TM) : cap_tiles;
-    tf = flow ? min(cap_tiles, (counters[5] + TM - 1) / TM) : t0;
-    tb = flow ? min(cap_tiles, (counters[6] + TM - 1) / TM) : t0;
-    total = t0 * (groups - (flow ? 2 : 0)) + (flow ? tf + tb : 0);
+    tf = gf >= 0 ? min(cap_tiles, (counters[5] + TM - 1) / TM) : t0;
+    tb = gb >= 0 ? min(cap_tiles, (counters[6] + TM - 1) / TM) : t0;
+    total = t0 * (groups - (gf >= 0) - (gb >= 0)) + (gf >= 0 ? tf : 0) + (gb >= 0 ? tb : 0);
   }
-  __device__ __forceinline__ int group_tiles(int g) const { return (flow && g == 5) ? tf : ((flow && g == 6) ? tb : t0); }
+  __device__ __forceinline__ int group_tiles(int g) const { return g == gf ? tf : (g == gb ? tb : t0); }
   __device__ __forceinline__ int global_tile(int t) const {
     for (int g = 0; g < n_groups; ++g) {
       const int n = group_tiles(g);
@@ -393,7 +394,7 @@ struct FwdParams {
   int64_t w_off[B200_MAX_LAYERS], b_off[B200_MAX_LAYERS];
   NetImages img;
   int cap, n_groups; const int* n_valid;
-  int flow_groups;           // mapping batch of the loop: groups 5 / 6 are compacted to counters[5] / counters[6] rows
+  int g_fwd, g_bwd;          // groups compacted to counters[5] / counters[6] rows (-1: none; see TileIter)
   float in_scale, in_shift;  // atlas: network input = x * in_scale + in_shift (0.5, 0.5 inside the loop: uv -> [0,1])
   int store_images;          // 0: inference (render / IMLP.forward without grad): no activation images, no flags
   int tanh_out;
@@ -426,7 +427,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_fwd_kernel(const __grid_cons
   // real encoding columns of the 3-input family; the alpha network's 5 frequencies are part of its identity (tc_net_of)
   const int pe_cols = VAR == 1 ? 30 : 6 * P.pe_freqs;
   setup_cta(sm);
-  TileIter ti; ti.init(P.cap, P.n_groups, P.n_valid, P.flow_groups);
+  TileIter ti; ti.init(P.cap, P.n_groups, P.n_valid, P.g_fwd, P.g_bwd);
 
   if (warp >= CONSUMER_WGS * 4) {
     // ------------------------------------------------------------------ producer (consumption order)
@@ -647,7 +648,7 @@ struct BwdParams {
   NetImages img;
   int cap, n_groups; const int* n_valid;
   int* gmax_bits;            // [0] max |dL/dy| from the loss head, [1] max |dL/duv| after the atlas backward
-  int flow_groups;
+  int g_fwd, g_bwd;
   float in_scale;            // atlas: d(network input)/d(x) (0.5 inside the loop)
   int d_in_accumulate;       // atlas: 1 = d_in already holds the direct loss-head gradient (the loop), 0 = overwrite
   int tanh_out;
@@ -683,7 +684,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_bwd_kernel(const __grid_cons
   float* s_w0acc = s_bacc + (L - 1) * 256;               // mapping: 768
   for (int i = threadIdx.x; i < (L - 1) * 256 + (ATLAS ? 0 : 768); i += blockDim.x) s_bacc[i] = 0.f;
   setup_cta(sm);
-  TileIter ti; ti.init(P.cap, P.n_groups, P.n_valid, P.flow_groups);
+  TileIter ti; ti.init(P.cap, P.n_groups, P.n_valid, P.g_fwd, P.g_bwd);
   float s_g, inv_sg;
   grad_scales(P.gmax_bits, MAPPING, s_g, inv_sg);
 
@@ -912,7 +913,7 @@ struct WgradItem {
   int cap, n_groups;      // row geometry of the network this item belongs to
   int split, n_split;     // this cluster's share of the live tiles
   int mapping;            // 1: gradients of the mapping network (second gradient scale)
-  int flow_groups;        // row geometry: compacted flow-match groups (mapping batch of the loop)
+  int g_fwd, g_bwd;       // row geometry: compacted flow-match groups (-1: none)
 };
 constexpr int MAX_WGRAD_ITEMS = 768;
 struct WgradItems { WgradItem it[MAX_WGRAD_ITEMS]; int n; long long cycles[256]; };   // cycles: per-CTA duration (diagnostics)
@@ -1031,7 +1032,7 @@ tc_wgrad_kernel(const WgradItems* __restrict__ items, const int* __restrict__ n_
       uint32_t gs = 0;                                  // running stage counter across units, equal in both CTAs
       for (int it = cluster; it < n_items; it += n_clusters) {
         const WgradItem W = items->it[it];
-        TileIter ti; ti.init(W.cap, W.n_groups, n_valid, W.flow_groups);
+        TileIter ti; ti.init(W.cap, W.n_groups, n_valid, W.g_fwd, W.g_bwd);
         int t_begin, t_end; unit_tiles(W, ti, t_begin, t_end);
         const int a_atoms = W.a_cols / 64, b_atoms = W.b_cols / 64;
         const bool split_rows = W.a_cols == 64;         // 64x64: CTA r takes the r-th half of the 32-row steps
@@ -1080,7 +1081,7 @@ tc_wgrad_kernel(const WgradItems* __restrict__ items, const int* __restrict__ n_
     uint32_t gs = 0;
     for (int it = cluster; it < n_items; it += n_clusters) {
       const WgradItem W = items->it[it];
-      TileIter ti; ti.init(W.cap, W.n_groups, n_valid, W.flow_groups);
+      TileIter ti; ti.init(W.cap, W.n_groups, n_valid, W.g_fwd, W.g_bwd);
       int t_begin, t_end; unit_tiles(W, ti, t_begin, t_end);
       const int n_steps = (t_end - t_begin) * 4;
       if (n_steps == 0) continue;
@@ -1184,7 +1185,7 @@ static FwdParams fill_fwd(const MlpShape& sh, const NetImages& im, const float* 
                           int groups, const int* n_valid) {
   FwdParams P{};
   P.x = x; P.y = y; P.params = params; P.img = im; P.cap = cap; P.n_groups = groups; P.n_valid = n_valid;
-  P.in_scale = 0.5f; P.in_shift = 0.5f; P.store_images = 1; P.tanh_out = 1; P.flow_groups = 0; P.pe_freqs = sh.pe;
+  P.in_scale = 0.5f; P.in_shift = 0.5f; P.store_images = 1; P.tanh_out = 1; P.g_fwd = P.g_bwd = -1; P.pe_freqs = sh.pe;
   for (int l = 0; l < sh.L; ++l) { P.w_off[l] = sh.w_off[l]; P.b_off[l] = sh.b_off[l]; }
   return P;
 }
@@ -1203,7 +1204,7 @@ static BwdParams fill_bwd(const MlpShape& sh, const NetImages& im, const float* 
   BwdParams P{};
   P.dy = dy; P.y = y; P.x = x; P.d_in = d_in; P.params = params; P.grads = grads; P.img = im;
   P.cap = cap; P.n_groups = groups; P.n_valid = n_valid; P.gmax_bits = gmax_bits;
-  P.in_scale = 0.5f; P.d_in_accumulate = 1; P.tanh_out = 1; P.flow_groups = 0;
+  P.in_scale = 0.5f; P.d_in_accumulate = 1; P.tanh_out = 1; P.g_fwd = P.g_bwd = -1;
   for (int l = 0; l < sh.L; ++l) { P.w_off[l] = sh.w_off[l]; P.b_off[l] = sh.b_off[l]; }
   return P;
 }
@@ -1250,16 +1251,16 @@ static double step_cost(int a_cols, int b_cols) {
 }
 
 struct WgProto { const char* a; int64_t a_term; int a_cols; const char* b; int64_t b_term; int b_cols; int transposed;
-                 float* out; int ld; int n_rows, n_cols, groups; double bytes; int mapping; };
+                 float* out; int ld; int n_rows, n_cols, groups; double bytes; int mapping; int g_fwd, g_bwd; };
 
 static void protos_for_net(WgProto* protos, int& np, const MlpShape& sh, const NetImages& im, float* g, TcNet net,
-                           int groups) {
+                           int groups, int g_fwd = -1, int g_bwd = -1) {
   const bool pe = tc_pe_first(net);
   const int mapping = tc_net_is_mapping(net) ? 1 : 0;
   auto add = [&](const char* a, int64_t a_term, int a_cols, const char* b, int64_t b_term, int b_cols, float* out, int ld,
                  int n_rows, int n_cols, int transposed = 0) {
     protos[np++] = WgProto{a, a_term, a_cols, b, b_term, b_cols, transposed, out, ld, n_rows, n_cols, groups,
-                           (double)groups * step_cost(a_cols, b_cols), mapping};
+                           (double)groups * step_cost(a_cols, b_cols), mapping, g_fwd, g_bwd};
   };
   for (int l = 1; l <= sh.L - 2; ++l)
     add(im.dz + (int64_t)l * im.slot_stride, im.term_stride, 256, im.act + (int64_t)(l - 1) * im.slot_stride,
@@ -1287,7 +1288,7 @@ static void protos_for_net(WgProto* protos, int& np, const MlpShape& sh, const N
 // it); on a 132-SM H100 the work list is the same as with one unit per SM.
 constexpr int WG_UNITS_PER_CLUSTER = 2;
 static int wg_clusters() { return g_wg_clusters[current_device()]; }
-static void apportion_items(WgradItems& wi, const WgProto* protos, int np, int cap, int flow_groups) {
+static void apportion_items(WgradItems& wi, const WgProto* protos, int np, int cap) {
   double total_bytes = 0;
   for (int i = 0; i < np; ++i) total_bytes += protos[i].bytes;
   const int sms = wg_clusters() * WG_UNITS_PER_CLUSTER;
@@ -1318,7 +1319,7 @@ static void apportion_items(WgradItems& wi, const WgProto* protos, int np, int c
       it.b_img = pr.b; it.b_term = pr.b_term; it.b_cols = pr.b_cols; it.transposed = pr.transposed;
       it.out = pr.out; it.ld_out = pr.ld; it.n_rows = pr.n_rows; it.n_cols = pr.n_cols;
       it.cap = cap; it.n_groups = pr.groups; it.split = sp; it.n_split = n_split[i]; it.mapping = pr.mapping;
-      it.flow_groups = (pr.mapping && flow_groups) ? 1 : 0;
+      it.g_fwd = pr.g_fwd; it.g_bwd = pr.g_bwd;
     }
   }
 }
@@ -1331,7 +1332,7 @@ static void apportion_items(WgradItems& wi, const WgProto* protos, int np, int c
 struct TabKey {
   int dev; const void* ws; TcNet net;   // fused step: net = Atlas (mapping + atlas) or the mapping's (pre-training)
   int pe;                               // encoding frequencies of the (mapping) network: its tables depend on them
-  bool step, with_bwd; int cap, groups, flow;
+  bool step, with_bwd; int cap, groups, g_fwd, g_bwd;
   const void* params; const void* grads;   // grads null: a stand-alone forward, served by the entry of its backward
 };
 struct TcTables { TabKey key; PrepJobs* d_prep = nullptr; int n_prep = -1; WgradItems* d_wg = nullptr; int n_wg = -1; };
@@ -1350,7 +1351,7 @@ static TcTables* find_tables(const TabKey& k, bool add) {
   for (TcTables* t : g_tabs) {
     TabKey& e = t->key;
     if (e.dev == k.dev && e.ws == k.ws && e.net == k.net && e.pe == k.pe && e.step == k.step && e.with_bwd == k.with_bwd &&
-        e.cap == k.cap && e.groups == k.groups && e.flow == k.flow && e.params == k.params &&
+        e.cap == k.cap && e.groups == k.groups && e.g_fwd == k.g_fwd && e.g_bwd == k.g_bwd && e.params == k.params &&
         (!k.grads || !e.grads || e.grads == k.grads)) {
       if (!e.grads) e.grads = k.grads;
       return t;
@@ -1375,9 +1376,13 @@ template <class T> static int upload(const T& host, T** dst, bool own, cudaStrea
   return B200_OK;
 }
 
+// the compacted flow-match groups of the fused step's mapping batch: G_FWD = 5, G_BWD = 6 when it has them
+static int step_g_fwd(const TcStep& s) { return (s.flow_groups && s.n_groups > 6) ? 5 : -1; }
+static int step_g_bwd(const TcStep& s) { return (s.flow_groups && s.n_groups > 6) ? 6 : -1; }
+
 static TabKey step_key(const TcStep& s) {
   return TabKey{current_device(), s.plan->base, s.y_atlas ? TcNet::Atlas : tc_net_of(*s.ms), s.ms->pe, true, true, s.cap,
-                s.n_groups, s.flow_groups, s.params, s.grads};
+                s.n_groups, step_g_fwd(s), step_g_bwd(s), s.params, s.grads};
 }
 
 static bool step_shapes_ok(const TcStep& s) {
@@ -1408,10 +1413,10 @@ int tc_begin_step(const TcStep& s, cudaStream_t st) {
     if (g_pj.n > MAX_PREP_JOBS) { set_error("table overflow"); return B200_ERR_INVALID; }
     // ---- wgrad items
     WgProto protos[32]; int np = 0;
-    protos_for_net(protos, np, *s.ms, lay.map, s.grads, mnet, s.n_groups);
+    protos_for_net(protos, np, *s.ms, lay.map, s.grads, mnet, s.n_groups, step_g_fwd(s), step_g_bwd(s));
     if (atlas) protos_for_net(protos, np, *s.as, lay.atl, s.grads + s.ms->total, TcNet::Atlas, 3);
     g_wi.n = 0;
-    apportion_items(g_wi, protos, np, s.cap, s.flow_groups);
+    apportion_items(g_wi, protos, np, s.cap);
     B200_PROPAGATE(upload(g_pj, &tab->d_prep, true, st));
     B200_PROPAGATE(upload(g_wi, &tab->d_wg, true, st));
     tab->n_prep = g_pj.n; tab->n_wg = g_wi.n;
@@ -1439,7 +1444,7 @@ int tc_step_forward(const TcStep& s, cudaStream_t st) {
   B200_CHECK_CUDA(cudaStreamWaitEvent(st, sd.join, 0));
   sd.pending = false;
   FwdParams pm = fill_fwd_mapping(*s.ms, lay.map, s.x_map, s.uv, s.params, s.cap, s.n_groups, s.counters);
-  pm.flow_groups = s.flow_groups;
+  pm.g_fwd = step_g_fwd(s); pm.g_bwd = step_g_bwd(s);
   timer_begin(TAG_MAP_FWD, st);
   B200_PROPAGATE(launch_fwd(tc_net_of(*s.ms), pm, s.n_groups * (s.cap / TM), st));
   timer_end(TAG_MAP_FWD, st);
@@ -1488,7 +1493,7 @@ int tc_step_backward(const TcStep& s, cudaStream_t st) {
   }
   BwdParams pm = fill_bwd(*s.ms, lay.map, s.d_uv, s.uv, s.x_map, nullptr, s.params, s.grads, s.cap, s.n_groups,
                           s.counters, gmax);
-  pm.flow_groups = s.flow_groups;
+  pm.g_fwd = step_g_fwd(s); pm.g_bwd = step_g_bwd(s);
   timer_begin(TAG_MAP_BWD, st);
   B200_PROPAGATE(launch_bwd(tc_net_of(*s.ms), pm, s.n_groups * (s.cap / TM), st));
   timer_end(TAG_MAP_BWD, st);
@@ -1567,30 +1572,43 @@ int64_t tc_single_workspace_bytes(const MlpShape& sh, TcNet net, int64_t rows) {
   return pl.bytes + 2048;
 }
 
-static int check_single(const MlpShape& sh, TcNet net, int64_t rows) {
+static int check_single(const MlpShape& sh, TcNet net, const TcRows& r) {
   B200_PROPAGATE(ensure_attrs());
   B200_REQUIRE(net != TcNet::None && tc_net_of(sh) == net, "tensor-core IMLP: the shape is not the network it is "
                "called for (mapping 3-256x{4,2}-2, atlas 2-PE10-256x6-3 with skips 4, 7, alpha 3-PE5-256x6-1, "
                "PE mapping 3-PE{1..10}-256x{4,2}-2)");
-  B200_REQUIRE(rows > 0 && rows % TM == 0 && rows / TM < (1 << 20), "rows must be a positive multiple of %d", TM);
+  B200_REQUIRE(r.cap > 0 && r.cap % TM == 0 && r.groups > 0 && r.rows() / TM < (1 << 20),
+               "rows must be a positive multiple of %d", TM);
+  B200_REQUIRE(r.g_fwd < 0 || r.g_bwd < 0 || r.g_fwd != r.g_bwd, "the two compacted groups must differ");
   return B200_OK;
 }
 
-// The tables of a stand-alone call: the cache entry of a persistent workspace, else the workspace's own slots.
-static TcTables* single_tables(TcTables& eph, const MlpShape& sh, TcNet net, const char* ws, int64_t rows, const float* params,
-                               const float* grads, bool training, bool persistent) {
+// The tables of a stand-alone call: the cache entry of a persistent workspace, else the workspace's own slots.  The
+// weight-gradient items depend on the row geometry (cap, groups, compacted groups), not on the counts themselves.
+static TcTables* single_tables(TcTables& eph, const MlpShape& sh, TcNet net, const char* ws, const TcRows& r,
+                               const float* params, const float* grads, bool training, bool persistent) {
   if (!persistent) return &eph;
-  return find_tables(TabKey{current_device(), ws, net, sh.pe, false, training, (int)rows, 1, 0, params, grads}, true);
+  return find_tables(TabKey{current_device(), ws, net, sh.pe, false, training, r.cap, r.groups, r.g_fwd, r.g_bwd,
+                            params, grads}, true);
 }
 
-// x: mapping [rows][4], atlas [rows][2] (network input itself).  y: [rows][out_dim].
-int tc_single_forward(const MlpShape& sh, TcNet net, const float* params, const float* x, float* y, int64_t rows,
+static FwdParams fill_single_fwd(const MlpShape& sh, const NetImages& im, const float* x, float* y, const float* params,
+                                 const TcRows& r) {
+  FwdParams P = fill_fwd(sh, im, x, y, params, r.cap, r.groups, r.counters);
+  P.g_fwd = r.g_fwd; P.g_bwd = r.g_bwd;
+  return P;
+}
+
+// x: mapping [rows][4], atlas [rows][2] (network input itself).  y: [rows][out_dim].  Only the tiles holding live rows
+// of `r` are evaluated; the other rows of y are left as they were.
+int tc_single_forward(const MlpShape& sh, TcNet net, const float* params, const float* x, float* y, const TcRows& r,
                       bool training, char* ws, bool persistent, cudaStream_t st) {
-  B200_PROPAGATE(check_single(sh, net, rows));
+  B200_PROPAGATE(check_single(sh, net, r));
+  const int64_t rows = r.rows();
   SinglePlan pl{};
   plan_single(sh, net, rows, ws, &pl);
   TcTables eph{}; eph.d_prep = pl.d_prep;
-  TcTables* tab = single_tables(eph, sh, net, ws, rows, params, nullptr, training, persistent);
+  TcTables* tab = single_tables(eph, sh, net, ws, r, params, nullptr, training, persistent);
   B200_REQUIRE(tab, "too many distinct tensor-core workspaces in one process (%d)", MAX_TABLES);
   if (tab->n_prep < 0) {
     g_pj.n = 0;
@@ -1600,35 +1618,37 @@ int tc_single_forward(const MlpShape& sh, TcNet net, const float* params, const 
   }
   tc_prep_kernel<<<tab->n_prep * 4, 128, 0, st>>>(tab->d_prep);
   B200_CHECK_LAUNCH();
-  FwdParams P = fill_fwd(sh, pl.im, x, y, params, (int)rows, 1, nullptr);
+  FwdParams P = fill_single_fwd(sh, pl.im, x, y, params, r);
   P.in_scale = 1.0f; P.in_shift = 0.0f; P.store_images = training ? 1 : 0; P.tanh_out = sh.tanh_out ? 1 : 0;
   return launch_fwd(net, P, (int)(rows / TM), st);
 }
 
-// after tc_single_forward(training) on the same workspace.  y: the saved outputs, dy [rows][out_dim] (zero in padding
-// rows), gmax: device int holding the bits of max|dy| (>= 0), d_in: atlas only, [rows][2] or null.
+// after tc_single_forward(training) on the same workspace and row geometry.  y: the saved outputs, dy [rows][out_dim]
+// (zero in the padding rows of the live tiles), gmax: device int holding the bits of max|dy| (>= 0), d_in: atlas only,
+// [rows][2] or null (written for the live tiles only).
 int tc_single_backward(const MlpShape& sh, TcNet net, const float* params, float* grads, const float* x,
-                       const float* y, const float* dy, float* d_in, int* gmax2, int64_t rows, char* ws,
+                       const float* y, const float* dy, float* d_in, int* gmax2, const TcRows& r, char* ws,
                        bool persistent, cudaStream_t st) {
-  B200_PROPAGATE(check_single(sh, net, rows));
+  B200_PROPAGATE(check_single(sh, net, r));
+  const int64_t rows = r.rows();
   SinglePlan pl{};
   plan_single(sh, net, rows, ws, &pl);
   TcTables eph{}; eph.d_wg = pl.d_wg;
-  TcTables* tab = single_tables(eph, sh, net, ws, rows, params, grads, true, persistent);
+  TcTables* tab = single_tables(eph, sh, net, ws, r, params, grads, true, persistent);
   B200_REQUIRE(tab, "too many distinct tensor-core workspaces in one process (%d)", MAX_TABLES);
   if (tab->n_wg < 0) {
     WgProto protos[32]; int np = 0;
-    protos_for_net(protos, np, sh, pl.im, grads, net, 1);
+    protos_for_net(protos, np, sh, pl.im, grads, net, r.groups, r.g_fwd, r.g_bwd);
     g_wi.n = 0;
-    apportion_items(g_wi, protos, np, (int)rows, 0);
+    apportion_items(g_wi, protos, np, r.cap);
     B200_PROPAGATE(upload(g_wi, &tab->d_wg, persistent, st));
     tab->n_wg = g_wi.n;
   }
   // gmax2: [0] atlas scale, [1] mapping scale
-  BwdParams P = fill_bwd(sh, pl.im, dy, y, x, d_in, params, grads, (int)rows, 1, nullptr, gmax2);
-  P.in_scale = 1.0f; P.d_in_accumulate = 0; P.tanh_out = sh.tanh_out ? 1 : 0;
+  BwdParams P = fill_bwd(sh, pl.im, dy, y, x, d_in, params, grads, r.cap, r.groups, r.counters, gmax2);
+  P.in_scale = 1.0f; P.d_in_accumulate = 0; P.tanh_out = sh.tanh_out ? 1 : 0; P.g_fwd = r.g_fwd; P.g_bwd = r.g_bwd;
   B200_PROPAGATE(launch_bwd(net, P, (int)(rows / TM), st));
-  tc_wgrad_kernel<<<wgrad_grid(tab->n_wg), WG_THREADS, WG_SMEM, st>>>(tab->d_wg, nullptr, gmax2);
+  tc_wgrad_kernel<<<wgrad_grid(tab->n_wg), WG_THREADS, WG_SMEM, st>>>(tab->d_wg, r.counters, gmax2);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }

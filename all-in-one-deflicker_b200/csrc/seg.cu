@@ -138,11 +138,12 @@ __global__ void seg_atlas_in_kernel(const float* __restrict__ uv1, const float* 
   reinterpret_cast<float2*>(xat)[i] = make_float2(__fadd_rn(v.x * 0.5f, sh), __fadd_rn(v.y * 0.5f, sh));
 }
 
-// d uv += 0.5 * d(atlas input) for the three colour groups of both layers
-__global__ void seg_chain_kernel(const float* __restrict__ d_xat, int64_t rows_per_layer, float* __restrict__ d_uv1,
-                                 float* __restrict__ d_uv2) {
+// d uv += 0.5 * d(atlas input) for the three colour groups of both layers, on the resident samples' rows (the other
+// rows of d uv stay zero, so that max |d uv| does not see what the counted atlas backward left there)
+__global__ void seg_chain_kernel(const float* __restrict__ d_xat, int64_t rows_per_layer, int cap,
+                                 const int* __restrict__ counters, float* __restrict__ d_uv1, float* __restrict__ d_uv2) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= 2 * rows_per_layer) return;
+  if (i >= 2 * rows_per_layer || i % cap >= counters[0]) return;
   const bool second = i >= rows_per_layer;
   const float2 g = reinterpret_cast<const float2*>(d_xat)[i];
   float2* d = reinterpret_cast<float2*>(second ? d_uv2 : d_uv1) + (second ? i - rows_per_layer : i);
@@ -151,14 +152,17 @@ __global__ void seg_chain_kernel(const float* __restrict__ d_xat, int64_t rows_p
   *d = v;
 }
 
+// One thread per slot.  Slots [0, counters[0]) hold the resident samples (all of the batch on one GPU); the others
+// are padding, whose target rows may never have been written.  Every term is normalised by the GLOBAL batch and flow
+// counts, so that a SUM over the ranks of a frame-sharded trip gives the unsharded loss vector and gradients; the
+// count entries 12, 13 then hold world * count.
 __global__ void seg_loss_kernel(const float* __restrict__ uv1, const float* __restrict__ uv2, const float* __restrict__ ar,
                                 const float* __restrict__ yat, const float* __restrict__ targets,
-                                const float* __restrict__ mask, const int64_t* __restrict__ indices,
-                                const int* __restrict__ counters, int cap, int batch, SegLossConfig cfg,
+                                const int* __restrict__ counters, int cap, SegLossConfig cfg,
                                 float* __restrict__ d_uv1, float* __restrict__ d_uv2, float* __restrict__ d_ar,
                                 float* __restrict__ d_yat, float* __restrict__ losses) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
-  const int n_f = counters[1], n_b = counters[2], n_lf = counters[5], n_lb = counters[6];
+  const int n_local = counters[0], n_f = counters[1], n_b = counters[2], n_lf = counters[5], n_lb = counters[6];
   cfg.inv_nf = n_f > 0 ? 1.0f / (float)n_f : 0.f;
   cfg.inv_nb = n_b > 0 ? 1.0f / (float)n_b : 0.f;
   float part[SV_COUNT];
@@ -167,7 +171,7 @@ __global__ void seg_loss_kernel(const float* __restrict__ uv1, const float* __re
   if (s < cap) {
     SegSampleOut out;
     int pf = -1, pb = -1;
-    if (s < batch) {
+    if (s < n_local) {
       SegSampleIn in;
       const float* tg = targets + (int64_t)s * TARGET_FLOATS;
       pf = (int)tg[9] - 1; pb = (int)tg[10] - 1;
@@ -191,7 +195,7 @@ __global__ void seg_loss_kernel(const float* __restrict__ uv1, const float* __re
         for (int c = 0; c < 3; ++c) in.y[k][c] = yat[((int64_t)k * cap + s) * 3 + c];
 #pragma unroll
       for (int c = 0; c < 3; ++c) { in.rgb[c] = tg[c]; in.dx[c] = tg[3 + c]; in.dy[c] = tg[6 + c]; }
-      in.a_gt = mask[indices[s]];
+      in.a_gt = tg[11];
       in.wf = pf >= 0 ? 1.f : 0.f; in.wb = pb >= 0 ? 1.f : 0.f;
       seg_sample_loss(in, cfg, out);
 #pragma unroll
@@ -322,14 +326,16 @@ int b200_seg_loss_grad(const B200SegConfig* cfg, const B200Video* video, const f
                        const float* params, float* grads, float* losses, void* ws, int64_t ws_bytes, void* stream) {
   B200_REQUIRE(cfg && video && mask && indices && params && grads && losses, "null pointer");
   B200_REQUIRE(video->records && video->H > 0 && video->W > 0 && video->T > 0, "empty video");
-  B200_REQUIRE(video->t_begin == 0 && video->t_end == video->T, "the segmentation variant needs the whole video resident");
+  B200_REQUIRE(video->t_begin >= 0 && video->t_begin < video->t_end && video->t_end <= video->T, "bad resident frame range");
+  B200_REQUIRE(video->t_end - video->t_begin == video->T || (video->mask_fwd_bits && video->mask_bwd_bits),
+               "a frame shard needs the whole-video validity bitmaps");
   SegPlan pl;
   B200_PROPAGATE(seg_prepare(cfg, ws, ws_bytes, &pl));
   // the caller keeps `ws`, `params` and `grads` across trips: the networks' job tables are cached after the first
   // (eager) trip, which also makes the whole trip graph-capturable
   PersistentWorkspaceScope persistent;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const int cap = pl.cap, B = cfg->batch;
+  const int cap = pl.cap, B = cfg->batch;   // B: the GLOBAL batch; this rank keeps the samples of its frames
   const B200MlpDesc* descs[4] = {&cfg->mapping1, &cfg->mapping2, &cfg->alpha, &cfg->atlas};
   B200_CHECK_CUDA(cudaMemsetAsync(grads, 0, (size_t)pl.total_params * 4, st));
   B200_CHECK_CUDA(cudaMemsetAsync(losses, 0, B200_SEG_LOSS_FLOATS * 4, st));
@@ -343,7 +349,8 @@ int b200_seg_loss_grad(const B200SegConfig* cfg, const B200Video* video, const f
   geo.d_global = cfg->global_derivative_amount;
   // without the global rigidity term the two D-offset groups are neither produced nor evaluated
   const int n_groups = cfg->with_global ? G_COUNT : G_YMG;
-  B200_PROPAGATE(launch_select_sample(indices, B, *video, geo, cap, n_groups, pl.counters, nullptr, pl.x_map, pl.targets, st));
+  B200_PROPAGATE(launch_select_sample(indices, B, *video, geo, cap, n_groups, pl.counters, nullptr, pl.x_map, pl.targets, st,
+                                      mask));
   const int64_t map_rows = (int64_t)n_groups * cap;
   seg_pack_kernel<<<(unsigned)((map_rows + 255) / 256), 256, 0, st>>>(reinterpret_cast<const float4*>(pl.x_map), cap,
                                                                      map_rows, pl.x3, pl.xa);
@@ -351,15 +358,23 @@ int b200_seg_loss_grad(const B200SegConfig* cfg, const B200Video* video, const f
   float* const ins[4] = {pl.x3, pl.x3, pl.xa, pl.xat};
   float* const outs[4] = {pl.uv1, pl.uv2, pl.ar, pl.yat};
   float* const douts[4] = {pl.d_uv1, pl.d_uv2, pl.d_ar, pl.d_yat};
-  const int64_t net_rows[4] = {map_rows, map_rows, (int64_t)A_COUNT * cap, (int64_t)SEG_ATLAS_ROWS * cap};
+  // live rows of each network's batch: the resident samples in every group, the compacted flow-match rows in the two
+  // flow groups; the tensor-core launches visit only the tiles holding them
+  TcRows live[4];
+  const int n_net_groups[4] = {n_groups, n_groups, A_COUNT, SEG_ATLAS_ROWS};
+  const int g_fwd[4] = {G_FWD, G_FWD, A_FWD, -1}, g_bwd[4] = {G_BWD, G_BWD, A_BWD, -1};
+  for (int k = 0; k < 4; ++k) {
+    live[k].cap = cap; live[k].groups = n_net_groups[k]; live[k].counters = pl.counters;
+    live[k].g_fwd = g_fwd[k]; live[k].g_bwd = g_bwd[k];
+  }
   for (int k = 0; k < 3; ++k)
-    B200_PROPAGATE(b200_mlp_forward(descs[k], params + pl.net[k].p_off, ins[k], outs[k], net_rows[k], 1,
-                                    pl.net[k].prec, pl.net[k].ws, pl.net[k].ws_bytes, stream));
+    B200_PROPAGATE(mlp_forward_rows(descs[k], params + pl.net[k].p_off, ins[k], outs[k], live[k], 1, pl.net[k].prec,
+                                    pl.net[k].ws, pl.net[k].ws_bytes, st));
   const int64_t layer_rows = 3ll * cap;
   seg_atlas_in_kernel<<<(unsigned)((2 * layer_rows + 255) / 256), 256, 0, st>>>(pl.uv1, pl.uv2, layer_rows, pl.xat);
   B200_CHECK_LAUNCH();
-  B200_PROPAGATE(b200_mlp_forward(descs[3], params + pl.net[3].p_off, pl.xat, pl.yat, (int64_t)SEG_ATLAS_ROWS * cap, 1,
-                                  pl.net[3].prec, pl.net[3].ws, pl.net[3].ws_bytes, stream));
+  B200_PROPAGATE(mlp_forward_rows(descs[3], params + pl.net[3].p_off, pl.xat, pl.yat, live[3], 1, pl.net[3].prec,
+                                  pl.net[3].ws, pl.net[3].ws_bytes, st));
   SegLossConfig lc;
   lc.larger_dim = (float)larger; lc.uv_scale = cfg->uv_mapping_scale;
   lc.d_local = cfg->derivative_amount; lc.d_global = cfg->global_derivative_amount;
@@ -368,17 +383,18 @@ int b200_seg_loss_grad(const B200SegConfig* cfg, const B200Video* video, const f
   lc.c_flow = cfg->flow_coeff; lc.c_alpha_flow = cfg->alpha_flow_factor; lc.c_sparsity = cfg->sparsity_coeff;
   lc.c_boot = cfg->bootstrapping_factor; lc.with_global = cfg->with_global != 0;
   lc.inv_batch = 1.0f / (float)B; lc.inv_nf = lc.inv_nb = 0.f;
-  seg_loss_kernel<<<(cap + 127) / 128, 128, 0, st>>>(pl.uv1, pl.uv2, pl.ar, pl.yat, pl.targets, mask, indices, pl.counters,
-                                                      cap, B, lc, pl.d_uv1, pl.d_uv2, pl.d_ar, pl.d_yat, losses);
+  seg_loss_kernel<<<(cap + 127) / 128, 128, 0, st>>>(pl.uv1, pl.uv2, pl.ar, pl.yat, pl.targets, pl.counters, cap, lc,
+                                                      pl.d_uv1, pl.d_uv2, pl.d_ar, pl.d_yat, losses);
   B200_CHECK_LAUNCH();
   // backward: atlas first (its input gradient feeds both mappings), then the other three networks
-  B200_PROPAGATE(b200_mlp_backward(descs[3], params + pl.net[3].p_off, pl.xat, pl.d_yat, grads + pl.net[3].p_off, pl.d_xat,
-                                   (int64_t)SEG_ATLAS_ROWS * cap, pl.net[3].prec, pl.net[3].ws, pl.net[3].ws_bytes, stream));
-  seg_chain_kernel<<<(unsigned)((2 * layer_rows + 255) / 256), 256, 0, st>>>(pl.d_xat, layer_rows, pl.d_uv1, pl.d_uv2);
+  B200_PROPAGATE(mlp_backward_rows(descs[3], params + pl.net[3].p_off, pl.xat, pl.d_yat, grads + pl.net[3].p_off, pl.d_xat,
+                                   live[3], pl.net[3].prec, pl.net[3].ws, pl.net[3].ws_bytes, st));
+  seg_chain_kernel<<<(unsigned)((2 * layer_rows + 255) / 256), 256, 0, st>>>(pl.d_xat, layer_rows, cap, pl.counters,
+                                                                             pl.d_uv1, pl.d_uv2);
   B200_CHECK_LAUNCH();
   for (int k = 2; k >= 0; --k)
-    B200_PROPAGATE(b200_mlp_backward(descs[k], params + pl.net[k].p_off, ins[k], douts[k], grads + pl.net[k].p_off, nullptr,
-                                     net_rows[k], pl.net[k].prec, pl.net[k].ws, pl.net[k].ws_bytes, stream));
+    B200_PROPAGATE(mlp_backward_rows(descs[k], params + pl.net[k].p_off, ins[k], douts[k], grads + pl.net[k].p_off, nullptr,
+                                     live[k], pl.net[k].prec, pl.net[k].ws, pl.net[k].ws_bytes, st));
   return B200_OK;
 }
 

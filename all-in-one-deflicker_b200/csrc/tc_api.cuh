@@ -55,15 +55,35 @@ int64_t tc_infer_workspace_bytes(const MlpShape& ms, const MlpShape& as);
 int tc_infer_forward(const MlpShape& ms, const MlpShape& as, const float* params, const float* x_map, float* uv,
                      float* y, int64_t rows, char* ws, cudaStream_t st);
 
+// Rows of a stand-alone call: `groups` groups of `cap` rows each, group-major.  counters null: every row is live.
+// Otherwise (device counters of the sampling kernels) the first counters[0] rows of each group are live, except in
+// the compacted groups g_fwd / g_bwd (-1: none), whose first counters[5] / counters[6] rows are; the kernels visit only
+// the 128-row tiles that hold live rows.
+struct TcRows {
+  int cap = 0, groups = 1;
+  const int* counters = nullptr;
+  int g_fwd = -1, g_bwd = -1;
+  int64_t rows() const { return (int64_t)cap * groups; }
+};
+inline TcRows tc_all_rows(int64_t rows) { TcRows r; r.cap = (int)rows; return r; }
+
 // stand-alone IMLP (one network, autograd): see mlp_tc.cu
 int64_t tc_single_workspace_bytes(const MlpShape& sh, TcNet net, int64_t rows);
 // persistent: the caller keeps this workspace and these parameter / gradient buffers across calls -> job tables are
 // cached in their own device allocations and the calls become graph-capturable after one eager call
-int tc_single_forward(const MlpShape& sh, TcNet net, const float* params, const float* x, float* y, int64_t rows,
+int tc_single_forward(const MlpShape& sh, TcNet net, const float* params, const float* x, float* y, const TcRows& r,
                       bool training, char* ws, bool persistent, cudaStream_t st);
 int tc_single_backward(const MlpShape& sh, TcNet net, const float* params, float* grads, const float* x,
-                       const float* y, const float* dy, float* d_in, int* gmax2, int64_t rows, char* ws, bool persistent,
-                       cudaStream_t st);
+                       const float* y, const float* dy, float* d_in, int* gmax2, const TcRows& r, char* ws,
+                       bool persistent, cudaStream_t st);
+
+// b200_mlp_forward / b200_mlp_backward on a group-major batch whose live rows `live` describes (live.rows() rows):
+// on the tensor cores only the tiles holding live rows are evaluated (the fp32 path evaluates every row).  The rows
+// of dy outside the live ones must be zero or lie in tiles without live rows.  Used by the segmentation step.
+int mlp_forward_rows(const B200MlpDesc* d, const float* params, const float* x, float* y, const TcRows& live,
+                     int training, int precision, void* ws, int64_t ws_bytes, cudaStream_t st);
+int mlp_backward_rows(const B200MlpDesc* d, const float* params, const float* x, const float* dy, float* dparams,
+                      float* dx, const TcRows& live, int precision, void* ws, int64_t ws_bytes, cudaStream_t st);
 
 // Scope guard used by entry points that own a persistent workspace (the segmentation step): while alive,
 // b200_mlp_forward / backward calls made by this thread use the cached-table path above.

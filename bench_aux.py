@@ -195,8 +195,9 @@ def _reference_line(args):
 
 def seg_line(args, rank, world, local):
     """`bench.py --workload seg`: the segmentation variant of the stage-1 loop (SURVEY §8 f3) at the headline geometry
-    (80 x 432 x 768, 10 000 samples per iteration, config_flow_100.json), one GPU.  A step = one loop trip
-    (b200_seg_loss_grad + b200_adam_step).  `--impl reference` / cpu_baseline: oracle/seg_oracle.py on the host cores,
+    (80 x 432 x 768, 10 000 samples per iteration, config_flow_100.json), one GPU, or N GPUs under torchrun with the
+    frames sharded (each rank holds its frame block; one exchange of gradients || losses per trip; strong scaling).
+    A step = one loop trip (b200_seg_loss_grad + the exchange + Adam).  `--impl reference` / cpu_baseline: oracle/seg_oracle.py on the host cores,
     a bounded sample of whole iterations."""
     import time
     from b200 import synth
@@ -241,13 +242,17 @@ def seg_line(args, rank, world, local):
                                                "sample": f"{n} whole iterations of oracle/seg_oracle.py, {threads} threads"},
                               "e2e": {"value": v, "unit": unit, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}))
         return
-    assert world == 1, "the segmentation variant is single-GPU (whole video resident)"
+    import torch.distributed as dist
     from b200 import _native as N, atlas as A, seg as SG
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
-    vid = A.DeviceVideo.from_reference_layout(data, dev)
+    if world > 1:
+        dist.init_process_group("nccl", device_id=dev)
+    t0, t1 = A.frame_range(rank, world, T)
+    vid = A.DeviceVideo.from_reference_layout(data, dev, t0, t1)
     prec = N.PREC_TC if (args.precision != "fp32" and N.lib().b200_device_supports_tc()) else N.PREC_FP32
-    tr = SG.SegTrainer(vid, SG.pack_mask_frames(masks, dev), None, precision=prec, device=dev)
+    tr = SG.SegTrainer(vid, SG.pack_mask_frames(masks, dev, t0, t1), None, precision=prec, device=dev,
+                       process_group=dist.group.WORLD if world > 1 else None)
     torch.manual_seed(0)
     tr.init_like_reference()
     steps, warm = max(2, args.steps), max(3, args.warmup)
@@ -264,13 +269,15 @@ def seg_line(args, rank, world, local):
     l0 = N.lib().b200_launch_count()
     tr.step(0, use_graph=False)                       # kernels of one trip, counted on an eager (un-captured) trip
     n_launch = float(N.lib().b200_launch_count() - l0)
-    ms = _event_ms(step, steps, warm)
+    ms = _event_ms(step, steps, warm, world, dev)
     k[0] = 0
     ems = _event_ms(lambda: (tr.step_host(inds_h[k[0] % 8], 0 if k[0] % steps < steps // 2 else 6000), k.__setitem__(0, k[0] + 1)),
-                    steps, 2)
-    out = {"metric": metric, "value": 1000.0 / ms, "unit": unit, "n_gpus": 1, "steps": steps, "warmup": warm,
+                    steps, 2, world, dev)
+    if rank != 0:
+        return
+    out = {"metric": metric, "value": 1000.0 / ms, "unit": unit, "n_gpus": world, "steps": steps, "warmup": warm,
            "ms_per_step": ms, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
-           "dtype": ("mapping1 + atlas: 2-term fp16 split operands / fp32 accumulate (wgmma); mapping2 + alpha: fp32 CUDA cores"
+           "dtype": ("all four networks: 2-term fp16 split operands / fp32 accumulate (wgmma)"
                      if prec == N.PREC_TC else "fp32"), "data": "synthetic", "config": config,
            "e2e": {"value": 1000.0 / ems, "unit": unit, "h2d_bytes_per_step": B * 8, "d2h_bytes_per_step": N.SEG_LOSS_FLOATS * 4},
            "gpu_launches": int(round(n_launch * steps)), "launches_per_step": n_launch,

@@ -313,7 +313,10 @@ int b200_render_for(const B200MlpDesc* mapping, const float* params, int32_t H, 
  * alpha flow loss (:385-408), bootstrapping BCE and sparsity (seg script :249-307).
  * The four networks may have any IMLP shape; with precision == B200_PREC_TC each network whose
  * shape has tensor-core kernels (b200_mlp_tc_architecture != 0) uses them, the others the fp32
- * kernels.  Single device: the whole video must be resident (t_begin = 0, t_end = T).
+ * kernels.  The video may be the whole clip or a frame shard (t_begin, t_end with the
+ * whole-video bitmaps, as for b200_atlas_loss_grad): a rank evaluates its resident samples only
+ * (the tensor-core launches visit only the tiles that hold them), normalised by the GLOBAL batch
+ * and flow counts, so that one SUM over the ranks of [grads || losses] is the unsharded trip.
  * ------------------------------------------------------------------------------------------ */
 typedef struct B200SegConfig {
   int32_t batch;             /* samples_batch                                                  */
@@ -334,7 +337,9 @@ typedef struct B200SegConfig {
 
 /* loss vector of b200_seg_loss_grad:
  *   0 total  1 rgb  2 gradient  3 sparsity  4 rigidity1  5 rigidity2  6 global rigidity1
- *   7 global rigidity2  8 flow1  9 flow2  10 flow alpha  11 bootstrapping  12 n_fwd  13 n_bwd    */
+ *   7 global rigidity2  8 flow1  9 flow2  10 flow alpha  11 bootstrapping  12 n_fwd  13 n_bwd
+ * On a frame shard 0-11 are this rank's share; 12, 13 are the whole batch's counts on every rank
+ * (world * count after a SUM over ranks).  The flow terms are NaN on every rank when a count is 0. */
 #define B200_SEG_LOSS_FLOATS 16
 
 /* Which tensor-core kernels serve a network shape: 1 = mapping-shaped (3 -> 256 x {2,4} -> 2, no
@@ -351,8 +356,9 @@ int b200_mlp_tc_architecture(const B200MlpDesc* d);
 int64_t b200_seg_param_floats(const B200SegConfig* cfg, int64_t* offsets);
 int64_t b200_seg_workspace_bytes(const B200SegConfig* cfg);
 
-/* mask: the bootstrapping mask as [T][H][W] fp32 (mask_frames[y, x, t] of load_input_data,
- * unwrap_utils.py:40-72, frame-major).  grads and losses are overwritten. */
+/* mask: the bootstrapping mask of the RESIDENT frames as [t_end - t_begin][H][W] fp32
+ * (mask_frames[y, x, t] of load_input_data, unwrap_utils.py:40-72, frame-major; the whole [T][H][W]
+ * mask when the whole video is resident).  grads and losses are overwritten. */
 int b200_seg_loss_grad(const B200SegConfig* cfg, const B200Video* video, const float* mask,
                        const int64_t* indices, const float* params, float* grads, float* losses,
                        void* ws, int64_t ws_bytes, void* stream);
