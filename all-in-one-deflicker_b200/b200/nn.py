@@ -13,7 +13,7 @@ ACT = {"none": 0, "relu": 1, "leaky": 2, "sigmoid": 3, "tanh": 4}
 # summation order), "tc" = wgmma with fp16 operands and fp32 accumulation — the operand precision the
 # reference itself uses for these layers (fp16 autocast in RAFT, TF32 cuDNN in stage 2).
 _conv_precision = "fp32"
-_weight_images = {}        # id(weight tensor) -> (weakref to it, {(version, stride): packed fp16 images})
+_weight_images = {}        # id(weight tensor) -> (weakref to it, {image key (_image_key): packed fp16 images})
 
 
 def set_conv_precision(mode):
@@ -30,25 +30,36 @@ def conv_precision():
 
 
 def _images_for(d, w):
-    """Packed weight images, cached per weight TENSOR OBJECT (not per address: a freed tensor's address is reused)
-    and per in-place version.  Pass module parameters themselves (conv.weight) to benefit from the cache."""
+    """Packed weight images, cached per weight TENSOR OBJECT (not per address alone: a freed tensor's address is
+    reused) and keyed on everything the image depends on: the storage (`w.data = t`, `module.to(...)`), the in-place
+    version, the stride and whether the x taps are folded into the channel vector (decided by the upsampling mode
+    for a given weight shape).  Pass module parameters themselves (conv.weight) to benefit from the cache.
+    Writes through `w.data` (`w.data.copy_(t)`) bump no version and keep the storage, so they are not seen: call
+    `clear_weight_images()` after them."""
     key = id(w)
     ent = _weight_images.get(key)
     if ent is None or ent[0]() is not w:
         ent = (weakref.ref(w, lambda _r, k=key: _weight_images.pop(k, None)), {})
         _weight_images[key] = ent
-    sub = (w._version, d.stride)
+    nbytes = N.lib().b200_conv_tma_weight_image_bytes(C.byref(d))
+    if nbytes <= 0:
+        raise N.B200Error("conv weight image size: invalid descriptor: " + N.last_error())
+    sub = (w.data_ptr(), str(w.device), w._version, d.stride, d.upsample_mode)
     img = ent[1].get(sub)
     if img is None:
         ent[1].clear()
-        nbytes = N.lib().b200_conv_tma_weight_image_bytes(C.byref(d))
-        if nbytes <= 0:
-            raise N.B200Error("conv weight image size: invalid descriptor: " + N.last_error())
         img = torch.empty(nbytes, dtype=torch.uint8, device=w.device)
         N.check(N.lib().b200_conv_tma_weight_images(C.byref(d), N.ptr(w), N.ptr(img), N.current_stream()),
                 "conv weight images")
         ent[1][sub] = img
+    assert img.numel() == nbytes, "cached weight image does not match the convolution's layout"
     return img
+
+
+def clear_weight_images():
+    """Drop the cached packed weight images (needed after writes through `w.data`, which the cache cannot see).
+    Only when no captured CUDA graph still refers to them."""
+    _weight_images.clear()
 
 
 def _check(t):

@@ -52,11 +52,6 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, i
       : "memory");
 }
 
-__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
-  const __half2 h = __floats2half2_rn(a, b);
-  return *reinterpret_cast<const uint32_t*>(&h);
-}
-
 template <int ACT>
 __device__ __forceinline__ float tm_act(float v) {
   if (ACT == 1) return fmaxf(v, 0.f);
@@ -162,7 +157,8 @@ __device__ __forceinline__ void tma_consume(const ConvTmaArgs& a, char* sA, char
           }
           v[e] = val;
         }
-        if (ypix && j < d.Cout) *reinterpret_cast<uint32_t*>(ypix + j) = pack_half2(v[0], v[1]);   // Cout % 8 == 0 here
+        // saturating like the repack (split2_f16), so a chained consumer sees the operands an unchained one would
+        if (ypix && j < d.Cout) *reinterpret_cast<uint32_t*>(ypix + j) = cvt_pack_f16x2(v[0], v[1]);   // Cout % 8 == 0 here
       }
     }
   }
@@ -419,6 +415,7 @@ __global__ void conv_tma_weight_images_kernel(const float* __restrict__ w, char*
 
 struct TmaGeom {
   int HU, WU, OH, OW, phases, shift, HP2, WP2, Cp, cchunks, n_chunks, n_tile, n_tiles_n;
+  int a_rows;       // pixel rows of one activation box: 128 outputs plus the x taps that share it
   int fold_cf;      // > 0: the KW x taps are folded into the channel dimension, fold_cf channels per tap (narrow inputs)
   int64_t pack_bytes;
 };
@@ -450,6 +447,8 @@ static int tma_geometry(const B200ConvDesc* d, TmaGeom* g) {
     g->WP2 = g->OW;
     g->n_chunks = d->KH;
   }
+  g->a_rows = 128 + (((g->fold_cf ? 1 : d->KW) - 1) >> g->shift);   // folded: the x taps live in the channel dimension
+  B200_REQUIRE(g->a_rows <= 256, "filter too wide");                // the TMA box holds at most 256 rows
   g->n_tiles_n = (d->Cout + 255) / 256;
   const int per_tile = (d->Cout + g->n_tiles_n - 1) / g->n_tiles_n;
   g->n_tile = per_tile <= 64 ? 64 : (per_tile <= 128 ? 128 : 256);   // the wgmma N shapes the kernel is built for
@@ -503,8 +502,7 @@ static int launch_conv_tma(const B200ConvDesc* d, const TmaGeom& g, const float*
   const cuuint64_t dims[4] = {(cuuint64_t)g.Cp, (cuuint64_t)g.WP2, (cuuint64_t)g.HP2, (cuuint64_t)d->N * g.phases};
   const cuuint64_t strides[3] = {(cuuint64_t)g.Cp * 2, (cuuint64_t)g.WP2 * g.Cp * 2, (cuuint64_t)g.HP2 * g.WP2 * g.Cp * 2};
   const int kw_eff = g.fold_cf ? 1 : d->KW;               // folded: the x taps live in the channel dimension
-  const int a_rows = 128 + ((kw_eff - 1) >> g.shift);
-  B200_REQUIRE(a_rows <= 256, "filter too wide");
+  const int a_rows = g.a_rows;
   const cuuint32_t box[4] = {64, (cuuint32_t)a_rows, 1, 1};
   const cuuint32_t estr[4] = {1, 1, 1, 1};
   for (int term = 0; term <= split; ++term) {
@@ -612,6 +610,7 @@ int b200_conv2d_tma_chain(const B200ConvDesc* d, const float* x, void* in_packed
   if (int rc = tma_geometry(d, &g)) return rc;
   B200_REQUIRE(d->in_c_off >= 0 && d->in_c_off + d->Cin <= d->in_c_total && d->out_c_off >= 0 &&
                d->out_c_off + d->Cout <= d->out_c_total, "channel slice out of range");
+  if (residual) B200_REQUIRE(d->res_c_off >= 0 && d->res_c_off + d->Cout <= d->res_c_total, "residual slice out of range");
   if (!b200_device_supports_tc()) { set_error("b200_conv2d_tma_chain needs a compute-capability 9.x device"); return B200_ERR_UNSUPPORTED; }
   char* base = nullptr;
   if (in_packed) {

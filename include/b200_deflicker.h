@@ -463,7 +463,8 @@ int b200_conv2d(const B200ConvDesc* d, const float* x, const float* w, const flo
  *              workspace are then ignored
  *   out_packed (or NULL) + next + next_c_off: ALSO write act(conv) as fp16 into the packed input of the consumer
  *              convolution `next` at its input channel next_c_off (several producers may fill one consumer: concat);
- *              y may then be NULL (no fp32 NCHW output at all)
+ *              y may then be NULL (no fp32 NCHW output at all); the fp16 store saturates at +-65504 like the repack
+ * Filters wider than 129 taps at stride 1 (258 at stride 2) are refused: the size functions return -1 for them.
  * `next` / `d` with a packed input must satisfy b200_conv_tma_chainable: stride 1, no upsampling, zero or reflection
  * padding (a reflection halo is mirrored from the interior by the consumer call), whole input tensor (no channel slice),
  * Cin * KW > 64. */
