@@ -18,7 +18,8 @@
 //                    activation image the weight-gradient kernel consumes; first/last (K=3 / N=2,3) layers and the
 //                    positional encoding run on CUDA cores inside the same kernel
 //   tc_bwd_kernel    same structure for dL/dz: tanh', last layer on CUDA cores, hidden layers as
-//                    dZ * W (B = W^T images), ReLU mask from 1-bit flags, bias gradients by shuffle column sums
+//                    dZ * W (B = W^T images), ReLU mask from 1-bit flags; bias gradients (and the mapping's dW0)
+//                    as row sums of each dZ tile by m64n8k16 MMAs against a [1, x, y, t] operand
 //   tc_wgrad_kernel  dW = dZ^T * H as wgmma with both operands MN-major straight from the images
 //                    the two kernels above left in HBM; split over rows, fp32 vector reductions; clusters of two CTAs
 //                    split the 256-wide operand and multicast the other, so each image byte is read once
@@ -336,22 +337,21 @@ __device__ __forceinline__ float quad_sum(float v) {
   v += __shfl_xor_sync(0xffffffffu, v, 1);
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
-// sum over the 16 rows of a warp of v (this thread's two rows already added): every lane of a column ends with it
-__device__ __forceinline__ float rows_sum(float v) {
-  v += __shfl_xor_sync(0xffffffffu, v, 4);
-  v += __shfl_xor_sync(0xffffffffu, v, 8);
-  return v + __shfl_xor_sync(0xffffffffu, v, 16);
-}
 
 // dynamic shared memory map: [A tile hi 64 KB | lo 64 KB][weight ring][aux tile 32 KB (atlas forward)][consts][barriers]
 constexpr int SMEM_A = 2 * TILE_IMG_BYTES;
 constexpr int SMEM_AUX = 2 * ATOM_BYTES;
-constexpr int SMEM_BWD_CONST_FLOATS = 7 * 256 + 768;         // bias-gradient accumulators (+ dW0 of the mapping)
+// backward: per consumer warpgroup the B operand of the row-sum MMAs (64 rows x 8 fp16) and a slice of gradient
+// accumulators (bias gradients of layers 0..L-2, + dW0 of the mapping: 7 * 256 for the atlas, 5 * 256 + 768 for the
+// 6-layer mapping)
+constexpr int RSUM_B_BYTES = 64 * 16;
+constexpr int BWD_ACC_FLOATS = 5 * 256 + 768;
+constexpr int SMEM_BWD_CONST_FLOATS = CONSUMER_WGS * (RSUM_B_BYTES / 4 + BWD_ACC_FLOATS);
 constexpr int SMEM_BARS = 256;
 constexpr int SMEM_MAX = 227 * 1024;                         // opt-in shared memory of one sm_90 CTA
 // Every kernel keeps as many 16 KB weight slots as the shared memory allows next to the A tile and, in the atlas
 // forward, the positional-encoding tile (6 mapping forward, 4 atlas forward); the backward kernels also hold their
-// gradient accumulators (5 slots).
+// gradient accumulators and row-sum operands (5 slots).
 template <bool ATLAS, bool BWD> struct KCfg {
   static constexpr int NST = BWD ? 5 : (ATLAS ? 4 : 6);
   static constexpr int SMEM = SMEM_A + NST * ITEM_BYTES + (ATLAS && !BWD ? SMEM_AUX : 0) +
@@ -679,10 +679,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_bwd_kernel(const __grid_cons
   constexpr int LOW = 1;                                  // dgrad layers L-2 .. 1 (atlas: + the dPE product)
   constexpr bool HAS_DPE = ATLAS && !PE3;                 // input gradient through the positional encoding
   constexpr bool MAPPING = OUT == 2;                      // the 3 -> 2 mappings, with or without encoding
-  // shared accumulators: bias gradients of layers 0..L-2; (mapping) dW0
-  float* s_bacc = sm.cst;                                // (L-1)*256
-  float* s_w0acc = s_bacc + (L - 1) * 256;               // mapping: 768
-  for (int i = threadIdx.x; i < (L - 1) * 256 + (ATLAS ? 0 : 768); i += blockDim.x) s_bacc[i] = 0.f;
+  // per consumer warpgroup: the B operand of its row-sum MMAs and its slice of the gradient accumulators, [bias
+  // gradients of layers 0..L-2 (256 each) | (plain mapping) dW0 [256][3]]
+  static_assert((L - 1) * 256 + (ATLAS ? 0 : 768) <= BWD_ACC_FLOATS, "gradient accumulators exceed their slice");
+  char* rsum_b = reinterpret_cast<char*>(sm.cst);
+  float* s_acc = sm.cst + CONSUMER_WGS * RSUM_B_BYTES / 4;
+  for (int i = threadIdx.x; i < CONSUMER_WGS * BWD_ACC_FLOATS; i += blockDim.x) s_acc[i] = 0.f;
   setup_cta(sm);
   TileIter ti; ti.init(P.cap, P.n_groups, P.n_valid, P.g_fwd, P.g_bwd);
   float s_g, inv_sg;
@@ -706,11 +708,47 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_bwd_kernel(const __grid_cons
   const uint16_t* bits16 = reinterpret_cast<const uint16_t*>(P.img.bits);
   const float* wlast = P.params + P.w_off[L - 1];
   const uint32_t a_rows = smem_u32(sm.a_tile) + c.g * WG_ROW_BYTES;
+  const uint32_t b_rows = smem_u32(rsum_b) + c.g * RSUM_B_BYTES;
+  float* g_acc = s_acc + c.g * BWD_ACC_FLOATS;
   float acc[128];
-  // bias-gradient column sums of one column pair (this thread's two rows), then over the warp's 16 rows
-  auto col_sums = [&](float* dst, int col, float a0, float a1) {
-    a0 = rows_sum(a0); a1 = rows_sum(a1);
-    if ((lane >> 2) == 0) { atomicAdd(dst + col, a0); atomicAdd(dst + col + 1, a1); }
+  // Sums over this warpgroup's 64 rows of the dZ tile it has just written (both terms), on the tensor cores:
+  // D[n][j] = sum_m dZ[m][n] B[m][j], A = the tile as an MN-major operand (M = its 256 columns, one atom block per
+  // m64n8k16, K = the rows), B = [1, 0, x_hi, x_lo, y_hi, y_lo, t_hi, t_lo] per row (S_ACT * x; plain mapping, else
+  // [1, 0, ...]).  Lane q of a quad holds B columns 2q, 2q + 1, one hi / lo pair: q = 0 the bias gradient of layer
+  // `slot`, q = 1..3 (the plain mapping's slot 0) dW0[n][q - 1].  Every element of the slice has one owning thread: plain
+  // loads and stores.  The accumulator is the first 16 registers of acc, free once the epilogue has written the tile.
+  auto row_sums = [&](int slot) {
+    float (&red)[16] = *reinterpret_cast<float(*)[16]>(&acc);
+    // two base descriptors, built here and not hoisted out of the tile loop (36 live descriptors would spill);
+    // the others add the byte offset / 16 to the start-address field
+    uint32_t a_base = a_rows, b_base = b_rows;
+    asm volatile("" : "+r"(a_base), "+r"(b_base));
+    const uint64_t ad = make_desc(a_base, ATOM_BYTES, 1024), bd = make_desc_rows16(b_base);
+    wgmma_fence();
+#pragma unroll
+    for (int blk = 0; blk < 4; ++blk)
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {                   // 16 rows = two groups of 8 rows
+        const uint64_t a = ad + ((blk * ATOM_BYTES + ks * 2048) >> 4), b = bd + ((ks * 256) >> 4);
+        float (&d)[4] = *reinterpret_cast<float(*)[4]>(&red[4 * blk]);
+        wgmma_n8<1, 1>(d, a, b, ks > 0 ? 1u : 0u);
+        wgmma_n8<1, 1>(d, a + (TILE_IMG_BYTES >> 4), b, 1u);
+      }
+    wgmma_commit();
+    wgmma_wait<0>();
+    acc_fence(red);
+    const bool w0 = !ATLAS && slot == 0;
+    if (c.q == 0 || w0) {
+#pragma unroll
+      for (int blk = 0; blk < 4; ++blk)
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          const int n = 64 * blk + 16 * c.w4 + (c.lane >> 2) + 8 * rr;
+          const float v = (red[4 * blk + 2 * rr] + red[4 * blk + 2 * rr + 1]) * inv_sg;
+          if (c.q == 0) g_acc[slot * 256 + n] += v;
+          else g_acc[(L - 1) * 256 + n * 3 + c.q - 1] += v * (1.0f / S_ACT);
+        }
+    }
   };
   auto put = [&](int m, int col, float v0, float v1) {
     uint32_t h, lo;
@@ -761,6 +799,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_bwd_kernel(const __grid_cons
     }
     // dA_{L-1}[k] = sum_j dz[j] W_last[j][k], masked by relu'(h_{L-2}) -> dZ_{L-2}
     a_tile_reusable(c);
+    if (c.tid < 64) {                                   // this tile's row-sum B operand (published by a_tile_written)
+      uint4 b = make_uint4(0x3C00u, 0u, 0u, 0u);        // fp16 1.0, then zeros
+      if (!ATLAS) {
+        const float4 xv = *reinterpret_cast<const float4*>(P.x + ((int64_t)gt * TM + 64 * c.g + c.tid) * 4);
+        __half h, lo;
+        split_f16(xv.x * S_ACT, h, lo); b.y = pack2(h, lo);
+        split_f16(xv.y * S_ACT, h, lo); b.z = pack2(h, lo);
+        split_f16(xv.z * S_ACT, h, lo); b.w = pack2(h, lo);
+      }
+      *reinterpret_cast<uint4*>(rsum_b + c.g * RSUM_B_BYTES + c.tid * 16) = b;
+    }
 #pragma unroll
     for (int i = 0; i < 32; ++i) {
       const int col = 8 * i + 2 * c.q;
@@ -780,13 +829,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_bwd_kernel(const __grid_cons
         v[e] = ((bits0 >> sh) & 1u) ? a0 : 0.f;
         v[2 + e] = ((bits1 >> sh) & 1u) ? a1 : 0.f;
       }
-      col_sums(s_bacc + (L - 2) * 256, col, v[0] + v[2], v[1] + v[3]);
       put(c.m0, col, v[0], v[1]);
       put(c.m0 + 8, col, v[2], v[3]);
     }
     a_tile_written(c);
     store_tile_rows(c, sm.a_tile, P.img.dz + (int64_t)(L - 2) * P.img.slot_stride + (int64_t)gt * TILE_IMG_BYTES,
                     P.img.term_stride);
+    row_sums(L - 2);
     // ---------------- hidden layers: dA_l = dZ_l W_l  ->  dZ_{l-1}
 #pragma unroll 1
     for (int l = L - 2; l >= LOW; --l) {
@@ -796,13 +845,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_bwd_kernel(const __grid_cons
                                 pending, c);
       finish_pass(pp, acc, pending, c);
       const int slot = l - 1;                           // produces dZ_{l-1}
-      const bool need_img = ATLAS || slot >= 1;         // mapping dZ_0 feeds only the CUDA-core layer-0 gradient
-      const bool need_a = HAS_DPE ? true : (slot >= 1); // dZ_0 is an MMA operand only for the dPE product
-      float4 x0 = make_float4(0.f, 0.f, 0.f, 0.f), x1 = x0;
-      if (!ATLAS && slot == 0) {
-        x0 = *reinterpret_cast<const float4*>(P.x + row0 * 4);
-        x1 = *reinterpret_cast<const float4*>(P.x + (row0 + 8) * 4);
-      }
+      const bool need_img = ATLAS || slot >= 1;         // mapping dZ_0 feeds only its row sums (b0, dW0)
       a_tile_reusable(c);
 #pragma unroll
       for (int i = 0; i < 32; ++i) {
@@ -815,26 +858,14 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_bwd_kernel(const __grid_cons
         v[1] = ((bits0 >> (sh - 1)) & 1u) ? __fmul_rn(acc[4 * i + 1], inv_dgrad) : 0.f;
         v[2] = ((bits1 >> sh) & 1u) ? __fmul_rn(acc[4 * i + 2], inv_dgrad) : 0.f;
         v[3] = ((bits1 >> (sh - 1)) & 1u) ? __fmul_rn(acc[4 * i + 3], inv_dgrad) : 0.f;
-        col_sums(s_bacc + slot * 256, col, v[0] + v[2], v[1] + v[3]);
-        if (!ATLAS && slot == 0) {
-          // layer-0 weight gradient dW0[n][d] = sum_m dZ0[m][n] * x[m][d]
-          const float xa[3] = {x0.x, x0.y, x0.z}, xb[3] = {x1.x, x1.y, x1.z};
-#pragma unroll
-          for (int dd = 0; dd < 3; ++dd) {
-            float s0 = rows_sum(v[0] * xa[dd] + v[2] * xb[dd]);
-            float s1 = rows_sum(v[1] * xa[dd] + v[3] * xb[dd]);
-            if ((lane >> 2) == 0) { atomicAdd(&s_w0acc[col * 3 + dd], s0); atomicAdd(&s_w0acc[(col + 1) * 3 + dd], s1); }
-          }
-        }
-        if (need_img || need_a) {
-          put(c.m0, col, v[0], v[1]);
-          put(c.m0 + 8, col, v[2], v[3]);
-        }
+        put(c.m0, col, v[0], v[1]);
+        put(c.m0 + 8, col, v[2], v[3]);
       }
       a_tile_written(c);
       if (need_img)
         store_tile_rows(c, sm.a_tile, P.img.dz + (int64_t)slot * P.img.slot_stride + (int64_t)gt * TILE_IMG_BYTES,
                         P.img.term_stride);
+      row_sums(slot);
     }
     if (HAS_DPE) {
       // ---------------- dPE = dZ_0 W_0 (64 columns, 40 real) -> d(in) -> d_in += in_scale * d(in); the accumulator is
@@ -885,15 +916,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_bwd_kernel(const __grid_cons
     }
   }
   if (c.leader) bulk_wait_all0();
-  // flush the per-CTA accumulators
+  // flush the per-CTA accumulators: the two warpgroups' slices summed
   named_bar(BAR_CONSUMERS, CONSUMERS);
+  static_assert(CONSUMER_WGS == 2, "the flush sums two slices");
   for (int i = threadIdx.x; i < (L - 1) * 256; i += CONSUMERS) {
-    const float v = s_bacc[i];
+    const float v = s_acc[i] + s_acc[BWD_ACC_FLOATS + i];
     if (v != 0.f) atomicAdd(P.grads + P.b_off[i >> 8] + (i & 255), v);
   }
   if (!ATLAS)
     for (int i = threadIdx.x; i < 768; i += CONSUMERS) {
-      const float v = s_w0acc[i];
+      const float v = s_acc[(L - 1) * 256 + i] + s_acc[BWD_ACC_FLOATS + (L - 1) * 256 + i];
       if (v != 0.f) atomicAdd(P.grads + P.w_off[0] + i, v);
     }
 }

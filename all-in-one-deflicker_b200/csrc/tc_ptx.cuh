@@ -150,6 +150,18 @@ __device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t a_desc, uint6
       : "memory");
 }
 
+// D[64 x 8] (+)= A[64 x 16] * B[16 x 8], both operands from shared memory (fp16 in, fp32 accumulate).
+// TA / TB: 0 = K-major, 1 = MN-major operand.  scale_d == 0 overwrites D.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n8(float (&d)[4], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n8k16.f32.f16.f16 {%0, %1, %2, %3}, %4, %5, p, 1, 1, %7, %8;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d), "n"(TA), "n"(TB)
+      : "memory");
+}
+
 // ------------------------------------------------------------------------------------ descriptors
 // wgmma shared-memory matrix descriptor: start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), layout type [62,64)
 // (1 = 128-byte swizzle).  K-major SW128: SBO = stride of 8-row groups (LBO unused); MN-major SW128: LBO = stride of
@@ -170,6 +182,16 @@ __device__ __forceinline__ uint64_t make_desc_sw64(uint32_t smem_addr, uint32_t 
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
   d |= (uint64_t)2 << 62;
+  return d;
+}
+// no swizzle (layout type 0), for an operand of 8-element (16-byte) rows: MN-major, 8 MN elements x 8 k = one 128-byte
+// core matrix, k groups of 8 at consecutive 128 bytes.  With N = 8 there is one MN group, so LBO and SBO (whose roles
+// the interleaved MN-major layout swaps against the swizzled ones) are both the 128-byte k-group stride.
+__device__ __forceinline__ uint64_t make_desc_rows16(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
+  d |= (uint64_t)(128 >> 4) << 16;
+  d |= (uint64_t)(128 >> 4) << 32;
   return d;
 }
 
