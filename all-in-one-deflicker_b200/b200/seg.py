@@ -38,17 +38,28 @@ LOSS_NAMES = ("total", "rgb", "gradient", "sparsity", "rigidity1", "rigidity2", 
               "flow1", "flow2", "flow_alpha", "bootstrapping", "n_fwd", "n_bwd")
 
 
+def _pe_freqs(c: dict, key: str, enabled: bool = True) -> int:
+    """Frequencies of an encoded network.  The reference builds a network on a 0-wide encoding when asked for 0
+    frequencies; the library has no such network (pe_freqs 0 means the raw input), so that is refused."""
+    if not enabled:
+        return 0
+    n = int(c[key])
+    if n < 1:
+        raise N.B200Error(f"{key} = {n}: a positionally encoded network needs at least one frequency")
+    return n
+
+
 def seg_descs(c: dict) -> Dict[str, N.MlpDesc]:
     """The four IMLP constructor calls of stage1_neural_atlas_seg.py:127-161."""
     return dict(
         mapping1=make_desc(3, 2, int(c["number_of_channels_mapping1"]), int(c["number_of_layers_mapping1"]),
-                           int(c["number_of_positional_encoding_mapping1"]) if c["use_positional_encoding_mapping1"] else 0, ()),
+                           _pe_freqs(c, "number_of_positional_encoding_mapping1", c["use_positional_encoding_mapping1"]), ()),
         mapping2=make_desc(3, 2, int(c["number_of_channels_mapping2"]), int(c["number_of_layers_mapping2"]),
-                           int(c["number_of_positional_encoding_mapping2"]) if c["use_positional_encoding_mapping2"] else 0, ()),
+                           _pe_freqs(c, "number_of_positional_encoding_mapping2", c["use_positional_encoding_mapping2"]), ()),
         alpha=make_desc(3, 1, int(c["number_of_channels_alpha"]), int(c["number_of_layers_alpha"]),
-                        int(c["positional_encoding_num_alpha"]), ()),
+                        _pe_freqs(c, "positional_encoding_num_alpha"), ()),
         atlas=make_desc(2, 3, int(c["number_of_channels_atlas"]), int(c["number_of_layers_atlas"]),
-                        int(c["positional_encoding_num_atlas"]), (4, 7)))
+                        _pe_freqs(c, "positional_encoding_num_atlas"), (4, 7)))
 
 
 def pack_mask_frames(mask_frames: torch.Tensor, device, t_begin: int = 0, t_end: Optional[int] = None) -> torch.Tensor:

@@ -83,7 +83,9 @@ int64_t plan_mlp_scratch(const MlpShape& s, int64_t rows, bool training, char* b
     sc.act[l] = reinterpret_cast<float*>(carve(p, rows * s.K[l] * 4));
   }
   sc.y = reinterpret_cast<float*>(carve(p, rows * s.out_dim * 4));
-  const int64_t wz = s.hidden > s.enc ? s.hidden : s.enc;
+  // dz first holds the output gradient (rows x out_dim), then the hidden layers' gradients (rows x hidden)
+  int64_t wz = s.hidden > s.enc ? s.hidden : s.enc;
+  if (s.out_dim > wz) wz = s.out_dim;
   sc.dz[0] = reinterpret_cast<float*>(carve(p, rows * wz * 4));
   sc.dz[1] = reinterpret_cast<float*>(carve(p, rows * wz * 4));
   sc.bytes = p - base;

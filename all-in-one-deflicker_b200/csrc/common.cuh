@@ -83,7 +83,7 @@ struct RowSpan {
 struct MlpScratch {
   float* act[B200_MAX_LAYERS];      // input of layer i: [rows, K[i]]  (post-ReLU, skip part appended)
   float* y = nullptr;               // network output after tanh [rows, out_dim]
-  float* dz[2] = {nullptr, nullptr};// ping-pong gradient buffers [rows, max(hidden, enc)]
+  float* dz[2] = {nullptr, nullptr};// ping-pong gradient buffers [rows, max(hidden, enc, out_dim)]
   int64_t bytes = 0;
 };
 int64_t plan_mlp_scratch(const MlpShape& s, int64_t rows, bool training, char* base, MlpScratch* out);

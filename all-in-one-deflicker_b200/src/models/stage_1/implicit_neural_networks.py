@@ -60,6 +60,10 @@ class IMLP(nn.Module):
         super().__init__()
         if apply_softmax:
             raise NotImplementedError("apply_softmax is unused by the stage-1 scripts and not provided")
+        if use_positional and positional_dim < 1:
+            # the reference builds a network on a 0-wide encoding (layer 0 sees no input); the library has no such
+            # network and would otherwise build the one on the raw input instead
+            raise N.B200Error(f"use_positional=True needs positional_dim >= 1 (got {positional_dim})")
         self.verbose, self.use_tanh = verbose, use_tanh
         self.skip_layers, self.num_layers = list(skip_layers), num_layers
         self.positional_dim, self.use_positional = positional_dim, use_positional
