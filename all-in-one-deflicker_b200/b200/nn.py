@@ -264,6 +264,38 @@ def corr_lookup(pyr, coords, radius=4):
     return out
 
 
+def corr_alt_build(fmap1, fmap2, out=None):
+    """fmaps (1, C, H8, W8) -> the state of the on-the-fly correlation (b200_corr_alt_floats floats: fmap1 and the
+    four average-pooled levels of fmap2, pixel-major).  No all-pairs volume: O(C * H8 * W8) memory."""
+    _check(fmap1); _check(fmap2)
+    b, c, h, w = fmap1.shape
+    if b != 1 or fmap2.shape != fmap1.shape:
+        raise N.B200Error("correlation kernels take batch 1 (the reference runs one frame pair at a time)")
+    n = int(N.lib().b200_corr_alt_floats(c, h, w))
+    if n <= 0:
+        raise N.B200Error(f"corr_alt_build: feature maps of {c} channels at {h}x{w} are not supported")
+    state = out if out is not None else torch.empty(n, dtype=torch.float32, device=fmap1.device)
+    _check(state)
+    if state.numel() != n:
+        raise N.B200Error("corr_alt_build: `out` has the wrong size")
+    N.check(N.lib().b200_corr_alt_build(N.ptr(fmap1), N.ptr(fmap2), c, h, w, N.ptr(state), N.current_stream()),
+            "b200_corr_alt_build")
+    return state
+
+
+def corr_alt_lookup(state, coords, dim, radius=4):
+    """What corr_lookup returns on the pyramid of the same feature maps (dim channels), computed from the state of
+    corr_alt_build: coords (1, 2, H8, W8) -> (1, 4 (2r+1)^2, H8, W8)."""
+    _check(state); _check(coords)
+    b, _, h, w = coords.shape
+    if state.numel() != int(N.lib().b200_corr_alt_floats(dim, h, w)):
+        raise N.B200Error("corr_alt_lookup: the state was built for another geometry")
+    out = torch.empty(b, 4 * (2 * radius + 1) ** 2, h, w, dtype=torch.float32, device=coords.device)
+    N.check(N.lib().b200_corr_alt_lookup(N.ptr(state), N.ptr(coords), N.ptr(out), dim, b, h, w, radius,
+                                         N.current_stream()), "b200_corr_alt_lookup")
+    return out
+
+
 def instance_norm(x, eps=1e-5, relu=False):
     _check(x)
     n, c, h, w = x.shape

@@ -9,11 +9,23 @@ import contextlib
 import torch
 import torch.nn as nn
 
+from b200 import _native as N
 from b200 import nn as K
-from src.models.stage_1.core.corr import CorrBlock
+from src.models.stage_1.core.corr import AlternateCorrBlock, CorrBlock
 from src.models.stage_1.core.extractor import BasicEncoder
 from src.models.stage_1.core.update import BasicUpdateBlock
 from src.models.stage_1.core.utils.utils import coords_grid
+
+
+def corr_block_class(args, H8, W8, device_bytes):
+    """The correlation block RAFT uses for feature maps of H8 x W8: `AlternateCorrBlock` when `args.alternate_corr` is
+    set (the reference's switch) or when the all-pairs pyramid would take more than half of the device's memory
+    (`device_bytes`; 4K frames need 89 GB), `CorrBlock` otherwise.  `device_bytes=None`: memory not known."""
+    if getattr(args, "alternate_corr", False):
+        return AlternateCorrBlock
+    if device_bytes is not None and int(N.lib().b200_corr_pyramid_floats(H8, W8)) * 4 > device_bytes // 2:
+        return AlternateCorrBlock
+    return CorrBlock
 
 
 class RAFT(nn.Module):
@@ -32,7 +44,7 @@ class RAFT(nn.Module):
         self.fnet = BasicEncoder(output_dim=256, norm_fn='instance', dropout=args.dropout)
         self.cnet = BasicEncoder(output_dim=hdim + cdim, norm_fn='batch', dropout=args.dropout)
         self.update_block = BasicUpdateBlock(self.args, hidden_dim=hdim)
-        self._graph_state = {}          # (fmap shape, iters, device) -> captured refinement loop + its buffers
+        self._graph_state = {}          # (fmap shape, iters, device, block) -> captured refinement loop + its buffers
 
     @contextlib.contextmanager
     def _autocast(self):
@@ -74,12 +86,15 @@ class RAFT(nn.Module):
     def _refine(self, fmap1, fmap2, image1, iters, flow_init, test_mode):
         """core/raft.py:109-148.  In test mode the `iters` refinement iterations (lookup -> update block -> coordinate
         update, ~100 launches each plus tensor glue) are captured once per geometry in ONE CUDA graph and replayed:
-        the correlation pyramid, hidden state, context and coordinates live in buffers owned by this module."""
+        the correlation block's state (pyramid or feature-map levels), hidden state, context and coordinates live in
+        buffers owned by this module."""
         use_graph = test_mode and getattr(self.args, "cuda_graph", True) and fmap1.is_cuda
-        key = (tuple(fmap1.shape), int(iters), fmap1.device)
+        block = corr_block_class(self.args, fmap1.shape[-2], fmap1.shape[-1],
+                                 torch.cuda.get_device_properties(fmap1.device).total_memory if fmap1.is_cuda else None)
+        key = (tuple(fmap1.shape), int(iters), fmap1.device, block)
         st = self._graph_state.get(key) if use_graph else None
-        corr_fn = CorrBlock(fmap1.float(), fmap2.float(), radius=self.args.corr_radius,
-                            out=st["pyr"] if st is not None else None)
+        corr_fn = block(fmap1.float(), fmap2.float(), radius=self.args.corr_radius,
+                        out=st["corr"] if st is not None else None)
         with self._autocast():
             cnet = self.cnet(image1)
         net, inp = torch.split(cnet, [self.hidden_dim, self.context_dim], dim=1)
@@ -91,8 +106,8 @@ class RAFT(nn.Module):
             if st is None:
                 # first call for this geometry: adopt the buffers, run the loop once eagerly (fills the weight-image
                 # caches, so nothing is packed or allocated outside the graph pool during capture), then capture
-                st = dict(pyr=corr_fn.pyramid, net=net.clone(), inp=inp.clone(), c0=coords0.clone(), c1=coords1.clone())
-                corr_fn.pyramid = st["pyr"]
+                st = dict(corr=corr_fn.state if block is AlternateCorrBlock else corr_fn.pyramid, net=net.clone(),
+                          inp=inp.clone(), c0=coords0.clone(), c1=coords1.clone())
                 self._loop(corr_fn, st["net"].clone(), st["inp"], st["c0"], st["c1"].clone(), iters, True)
                 torch.cuda.synchronize()
                 g = torch.cuda.CUDAGraph()

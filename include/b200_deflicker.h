@@ -396,8 +396,9 @@ int b200_eval_maps(const B200MlpDesc* mapping, const float* mapping_params, cons
                    float* flow_error, void* ws, int64_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * RAFT correlation — replaces CorrBlock (src/models/stage_1/core/corr.py:16-64); the reference's own
- * native hook for this operator is alt_cuda_corr.forward (corr.py:86-91, extension not shipped).
+ * RAFT correlation — replaces CorrBlock (src/models/stage_1/core/corr.py:16-64) with an all-pairs pyramid, and
+ * AlternateCorrBlock (corr.py:67-91) with the on-the-fly b200_corr_alt_* calls below, which take the place of the
+ * reference's unshipped alt_cuda_corr extension.
  * fmaps: [dim][H8*W8] fp32 (batch 1).  pyramid: level 0 [H8*W8][H8][W8], then 3 avg-pooled levels,
  * b200_corr_pyramid_floats() floats in total.
  * ------------------------------------------------------------------------------------------ */
@@ -415,6 +416,17 @@ int b200_corr_build_tc(const float* fmap1, const float* fmap2, int32_t dim, int3
                        void* workspace, int64_t workspace_bytes, void* stream);
 int b200_corr_lookup(const float* pyramid, const float* coords, float* out, int32_t batch,
                      int32_t H8, int32_t W8, int32_t radius, void* stream);
+/* On-the-fly correlation (AlternateCorrBlock): no all-pairs volume.  The state holds fmap1 and fmap2's four 2x2
+ * average-pooled levels, pixel-major ([pixels][dim]): b200_corr_alt_floats(dim, H8, W8) floats (-1 for a geometry
+ * the kernels do not take: dim a positive multiple of 16, H8, W8 >= 8), 16-byte aligned, owned by the caller.
+ * The lookup forms each window's dot products / sqrt(dim) when it is looked up and returns what b200_corr_lookup
+ * returns on the pyramid of the same fmaps, up to fp32 rounding (layout, taps, padding, NaN rules are the same);
+ * batch 1, radius 1..8.  Both calls are stream-ordered, allocate nothing and can be captured in a CUDA graph. */
+int64_t b200_corr_alt_floats(int32_t dim, int32_t H8, int32_t W8);
+int b200_corr_alt_build(const float* fmap1, const float* fmap2, int32_t dim, int32_t H8, int32_t W8, float* state,
+                        void* stream);
+int b200_corr_alt_lookup(const float* state, const float* coords, float* out, int32_t dim, int32_t batch, int32_t H8,
+                         int32_t W8, int32_t radius, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Convolution and image operators of the RAFT update block (core/update.py:6-136) and of the
