@@ -23,6 +23,8 @@ DEFAULTS = dict(samples_batch=10000, rgb_coeff=5000, optical_flow_coeff=500.0, g
                 rigidity_coeff=1.0, derivative_amount=1, uv_mapping_scale=0.8,
                 include_global_rigidity_loss=True, global_rigidity_derivative_amount_fg=100,
                 global_rigidity_coeff_fg=5.0, stop_global_rigidity=5000, use_gradient_loss=True)
+# pre_train_mapping draws 10000 pixels per step, whatever samples_batch is (unwrap_utils.py:183)
+PRETRAIN_BATCH = 10000
 
 MAPPING_DESC = dict(input_dim=3, output_dim=2, hidden_dim=256, num_layers=6, pe_freqs=0, skip_layers=())
 ATLAS_DESC = dict(input_dim=2, output_dim=3, hidden_dim=256, num_layers=8, pe_freqs=10, skip_layers=(4, 7))
@@ -273,42 +275,44 @@ class FusedDp:
             dist.all_reduce(t, group=self.pg)
 
 
-class AtlasTrainer:
-    """Flat parameters/optimiser state of (mapping, atlas) + the fused step."""
+class FlatTrainer:
+    """Flat parameters, Adam state, the exchange between ranks and CUDA-graph replay of a stage-1 trainer.
 
-    def __init__(self, video: Optional[DeviceVideo], config: Optional[dict] = None, precision: int = N.PREC_FP32,
-                 device="cuda", lr: float = 1e-4, process_group=None, resx: Optional[int] = None,
-                 fused_dp: Optional[bool] = None):
+    The networks of NETS share one flat fp32 parameter buffer in that order, which is also the order of the Adam
+    parameter groups; `hidden.{i}.weight|bias` are views into it.  Gradients and the loss vector share one buffer
+    (`grads`, `losses` are views) so that data parallelism needs ONE exchange: b200_dp_adam_step over symmetric memory
+    (FusedDp) with a process group on CUDA when it has more than one rank or `fused_dp` is True (True requires it);
+    with `fused_dp` False or a failed set-up, an NCCL all-reduce + the local Adam.
+
+    A subclass calls __init__, sets `cfg`, `descs`, `offsets`, `layouts` (mlp_layout of each network) and `n_params`,
+    then calls `_allocate`; it implements `_trip(it)` (one loss_grad of loop trip `it`) and `_regime(it)` (the key of the
+    graph that replays that trip)."""
+
+    NETS = ()                   # flat-buffer order = optimiser-group order
+    CONSTRUCTION_ORDER = ()     # order the reference script constructs (and so initialises) the networks
+
+    def __init__(self, video: Optional[DeviceVideo], precision: int, device, lr: float, process_group,
+                 resx: Optional[int]):
         self.lib = N.lib()
         self.video = video
-        self.cfg = dict(DEFAULTS)
-        if config:
-            self.cfg.update({k: v for k, v in config.items() if k in DEFAULTS})
-            check_architecture(config)
-        self.precision = precision
-        self.device = torch.device(device)
-        self.lr = lr
-        self.pg = process_group
-        self.world = 1
+        self.precision, self.device, self.lr = precision, torch.device(device), lr
+        self.resx = resx if resx is not None else (video.W if video is not None else 0)
+        self.pg, self.world = process_group, 1
         if process_group is not None:
             import torch.distributed as dist
             self.world = dist.get_world_size(process_group)
-        self.resx = resx if resx is not None else (video.W if video is not None else 0)
-        # the mapping of src/stage1_neural_atlas.py:112-119, with the positional encoding the config may ask for
-        self.map_desc = make_desc(**dict(MAPPING_DESC, pe_freqs=mapping_pe_freqs(config)))
-        self.atlas_desc = make_desc(**ATLAS_DESC)
-        self.map_w, self.map_b, self.map_total = mlp_layout(self.map_desc)
-        self.atl_w, self.atl_b, self.atl_total = mlp_layout(self.atlas_desc)
-        self.n_params = int(self.lib.b200_atlas_param_floats_for(C.byref(self.map_desc)))
-        assert self.n_params == self.map_total + self.atl_total
+        self._ws = None
+        self._scratch = {}
+        self._graphs = {}
+
+    def _allocate(self, n_losses: int, fused_dp: Optional[bool]):
         dev = self.device
-        # gradients + the loss vector share one buffer so that data parallelism needs ONE exchange
         self._dp = None
-        if self.world > 1 and dev.type == "cuda" and fused_dp is not False:
-            self._dp = FusedDp.create(process_group, dev, self.n_params, N.LOSS_FLOATS, required=bool(fused_dp))
+        if self.pg is not None and dev.type == "cuda" and fused_dp is not False and (self.world > 1 or fused_dp):
+            self._dp = FusedDp.create(self.pg, dev, self.n_params, n_losses, required=bool(fused_dp))
         if self._dp is None:
             self.params = torch.zeros(self.n_params, dtype=torch.float32, device=dev)
-            self.grad_loss = torch.zeros(self.n_params + N.LOSS_FLOATS, dtype=torch.float32, device=dev)
+            self.grad_loss = torch.zeros(self.n_params + n_losses, dtype=torch.float32, device=dev)
         else:
             self.params, self.grad_loss = self._dp.params, self._dp.grad_loss
         self.grads = self.grad_loss[:self.n_params]
@@ -316,20 +320,24 @@ class AtlasTrainer:
         self.exp_avg = torch.zeros_like(self.params)
         self.exp_avg_sq = torch.zeros_like(self.params)
         self.step_count = torch.zeros(1, dtype=torch.int64, device=dev)
-        self.indices = torch.zeros(self.cfg["samples_batch"], dtype=torch.int64, device=dev)
-        self._pin_inds = torch.zeros(self.cfg["samples_batch"], dtype=torch.int64).pin_memory() \
-            if dev.type == "cuda" else None
-        self._pin_loss = torch.zeros(N.LOSS_FLOATS, dtype=torch.float32).pin_memory() if dev.type == "cuda" else None
-        self._ws = None
-        self._graphs = {}
-        self.launches_per_step = None
+        B = int(self.cfg["samples_batch"])
+        self.indices = torch.zeros(B, dtype=torch.int64, device=dev)
+        self._pin_inds = torch.zeros(B, dtype=torch.int64).pin_memory() if dev.type == "cuda" else None
+        self._pin_loss = torch.zeros(n_losses, dtype=torch.float32).pin_memory() if dev.type == "cuda" else None
+
+    def _scratch_buffer(self, name: str, nbytes: int) -> torch.Tensor:
+        """Device scratch kept between calls, replaced by a larger one when a call needs more than `nbytes`."""
+        ws = self._scratch.get(name)
+        if ws is None or ws.numel() < nbytes:
+            ws = self._scratch[name] = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        return ws
 
     # ------------------------------------------------------------------ parameters / state dicts
     def _views(self, flat, which):
-        desc, w, b, base = ((self.map_desc, self.map_w, self.map_b, 0) if which == "mapping"
-                            else (self.atlas_desc, self.atl_w, self.atl_b, self.map_total))
+        w, b, _ = self.layouts[which]
+        base = self.offsets[which]
         out = {}
-        for i, (k, n) in enumerate(layer_dims(desc)):
+        for i, (k, n) in enumerate(layer_dims(self.descs[which])):
             out[f"hidden.{i}.weight"] = flat[base + w[i]: base + w[i] + k * n].view(n, k)
             out[f"hidden.{i}.bias"] = flat[base + b[i]: base + b[i] + n]
         return out
@@ -340,37 +348,38 @@ class AtlasTrainer:
     def grad_views(self, which):
         return self._views(self.grads, which)
 
-    def load_state(self, mapping_sd: Dict[str, torch.Tensor], atlas_sd: Dict[str, torch.Tensor]):
-        for which, sd in (("mapping", mapping_sd), ("atlas", atlas_sd)):
-            for k, v in self.param_views(which).items():
-                v.copy_(sd[k].to(self.device, torch.float32))
+    def net_slice(self, which):
+        return slice(self.offsets[which], self.offsets[which] + self.layouts[which][2])
 
     def init_like_reference(self):
-        """nn.Linear's default init on the global CPU generator, mapping first then atlas, weight
-        before bias — the stream order of src/stage1_neural_atlas.py:112-128."""
-        for which, desc in (("mapping", self.map_desc), ("atlas", self.atlas_desc)):
+        """nn.Linear's default init on the global CPU generator in the script's construction order, weight before
+        bias."""
+        for which in self.CONSTRUCTION_ORDER:
             views = self.param_views(which)
-            for i, (k, n) in enumerate(layer_dims(desc)):
+            for i, (k, n) in enumerate(layer_dims(self.descs[which])):
                 bound = 1.0 / math.sqrt(k)
                 views[f"hidden.{i}.weight"].copy_(torch.empty(n, k).uniform_(-bound, bound))
                 views[f"hidden.{i}.bias"].copy_(torch.empty(n).uniform_(-bound, bound))
+
+    def load_state(self, sds: Dict[str, Dict[str, torch.Tensor]]):
+        for which, sd in sds.items():
+            for k, v in self.param_views(which).items():
+                v.copy_(sd[k].to(self.device, torch.float32))
 
     def state_dict(self, which):
         return {k: v.detach().clone() for k, v in self.param_views(which).items()}
 
     def optimizer_state_dict(self):
-        """Schema of torch.optim.Adam.state_dict() for [{'params': mapping}, {'params': atlas}]
-        (what evaluate.py:621 stores)."""
+        """Schema of torch.optim.Adam.state_dict() with one group per network of NETS (what evaluate.py stores in the
+        checkpoint).  Collective under the fused optimiser: every rank calls it."""
         self.gather_moments()
         state, groups, idx = {}, [], 0
         step = self.step_count.detach().float().cpu().reshape(())
-        for which in ("mapping", "atlas"):
-            m = self._views(self.exp_avg, which)
-            v = self._views(self.exp_avg_sq, which)
+        for which in self.NETS:
+            m, v = self._views(self.exp_avg, which), self._views(self.exp_avg_sq, which)
             ids = []
             for k in m:
-                state[idx] = {"step": step.clone(), "exp_avg": m[k].detach().clone(),
-                              "exp_avg_sq": v[k].detach().clone()}
+                state[idx] = {"step": step.clone(), "exp_avg": m[k].detach().clone(), "exp_avg_sq": v[k].detach().clone()}
                 ids.append(idx)
                 idx += 1
             groups.append({"lr": self.lr, "betas": (0.9, 0.999), "eps": 1e-8, "weight_decay": 0, "amsgrad": False,
@@ -379,11 +388,9 @@ class AtlasTrainer:
         return {"state": state, "param_groups": groups}
 
     def load_optimizer_state_dict(self, sd):
-        idx = 0
-        step = 0
-        for which in ("mapping", "atlas"):
-            m = self._views(self.exp_avg, which)
-            v = self._views(self.exp_avg_sq, which)
+        idx, step = 0, 0
+        for which in self.NETS:
+            m, v = self._views(self.exp_avg, which), self._views(self.exp_avg_sq, which)
             for k in m:
                 st = sd["state"].get(idx)
                 if st is not None:
@@ -392,6 +399,134 @@ class AtlasTrainer:
                     step = int(st["step"])
                 idx += 1
         self.step_count.fill_(step)
+
+    # ------------------------------------------------------------------ optimiser and exchange between ranks
+    def adam(self, sl: Optional[slice] = None, m=None, v=None, step=None):
+        """b200_adam_step on the slice `sl` of the flat buffers (default: all), with the moments `m`, `v` and the step
+        counter `step` instead of the trainer's when given.  The slice's pointers are offsets, not tensor views:
+        pre-training calls this every step, and two views would add ~6 us of host time to a host-bound step."""
+        sl = slice(0, self.n_params) if sl is None else sl
+        at = lambda t: C.c_void_p(t.data_ptr() + 4 * sl.start)        # fp32 element sl.start of a flat buffer
+        N.check(self.lib.b200_adam_step(at(self.params), at(self.grads), at(self.exp_avg) if m is None else N.ptr(m),
+                                        at(self.exp_avg_sq) if v is None else N.ptr(v), sl.stop - sl.start, self.lr,
+                                        0.9, 0.999, 1e-8, 1.0, N.ptr(self.step_count if step is None else step),
+                                        N.current_stream()), "b200_adam_step")
+
+    def dp_adam(self):
+        """reduce-scatter + Adam + all-gather in one kernel (b200_dp_adam_step)."""
+        self._dp.adam_step(self.exp_avg, self.exp_avg_sq, self.lr, self.step_count)
+
+    def gather_moments(self):
+        """Under the fused optimiser a rank keeps the Adam moments of its slice only: assemble them (collective)."""
+        if self._dp is not None:
+            self._dp.gather_moments(self.exp_avg, self.exp_avg_sq)
+
+    def all_reduce(self):
+        if self.pg is not None and self.world > 1:
+            import torch.distributed as dist
+            dist.all_reduce(self.grad_loss, group=self.pg)      # one collective: gradients || loss vector
+
+    def _iteration(self, it: int):
+        self._trip(it)
+        if self._dp is not None:
+            self.dp_adam()
+        else:
+            self.all_reduce()
+            self.adam()
+
+    def step(self, it: int, use_graph: bool = True):
+        """One loop trip on the indices in self.indices (device): losses + gradients, the exchange between ranks (if
+        any), then one Adam update of every network (same lr / betas in every group, so one sweep over the flat
+        buffer).  On CUDA the trip is captured once per regime in a CUDA graph and replayed.  Returns the device loss
+        vector (valid after the stream reaches this point)."""
+        if not use_graph or self.device.type != "cuda":
+            self._iteration(it)
+            return self.losses
+        key = self._regime(it)
+        g = self._graphs.get(key)
+        if g is None:
+            # eager warm-up on a side stream (lazy module load, job tables, NCCL channels), state restored afterwards;
+            # capture does not execute, so the state is unchanged after it
+            state = (self.params, self.exp_avg, self.exp_avg_sq, self.step_count)
+            snap = [t.clone() for t in state]
+            side = torch.cuda.Stream()
+            side.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(side):
+                self._iteration(it)
+            torch.cuda.current_stream().wait_stream(side)
+            torch.cuda.synchronize()
+            for t, c in zip(state, snap):
+                t.copy_(c)
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                self._iteration(it)
+            self._graphs[key] = g
+        g.replay()
+        return self.losses
+
+    def step_host(self, inds_cpu: torch.Tensor, it: int, use_graph: bool = True) -> np.ndarray:
+        """End-to-end call with HOST buffers: pinned H2D of the index batch, one loop trip,
+        D2H of the loss vector (the step's result).  Synchronous."""
+        self._pin_inds.copy_(inds_cpu.reshape(-1))
+        self.indices.copy_(self._pin_inds, non_blocking=True)
+        losses = self.step(it, use_graph)
+        self._pin_loss.copy_(losses, non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        return self._pin_loss.numpy().copy()
+
+    # ------------------------------------------------------------------ pre-training
+    def _pretrain(self, sl: slice, T: int, H: int, W: int, iters: int, generator: Optional[torch.Generator], progress,
+                  loss_grad):
+        """pre_train_mapping (unwrap_utils.py:176-198) of the network in slice `sl` of the flat buffer: `iters` sweeps
+        over the T frames, PRETRAIN_BATCH random pixels of one frame per step, its own Adam(lr=1e-4) with fresh
+        moments.  Index draws come from the CPU generator in the reference's order (rows, then columns);
+        `loss_grad(f, ys, xs)` makes the native call of frame f on their device copies."""
+        n = sl.stop - sl.start
+        m = torch.zeros(n, dtype=torch.float32, device=self.device)
+        v = torch.zeros_like(m)
+        step = torch.zeros(1, dtype=torch.int64, device=self.device)
+        ys_d = torch.zeros(PRETRAIN_BATCH, dtype=torch.int64, device=self.device)
+        xs_d = torch.zeros_like(ys_d)
+        for i in range(iters):
+            for f in range(T):
+                ys = torch.randint(H, (PRETRAIN_BATCH, 1), generator=generator)
+                xs = torch.randint(W, (PRETRAIN_BATCH, 1), generator=generator)
+                ys_d.copy_(ys.reshape(-1), non_blocking=True)
+                xs_d.copy_(xs.reshape(-1), non_blocking=True)
+                loss_grad(f, ys_d, xs_d)
+                self.adam(sl, m, v, step)
+            if progress:
+                progress(i)
+
+
+class AtlasTrainer(FlatTrainer):
+    """Flat parameters/optimiser state of (mapping, atlas) + the fused step."""
+
+    NETS = CONSTRUCTION_ORDER = ("mapping", "atlas")
+
+    def __init__(self, video: Optional[DeviceVideo], config: Optional[dict] = None, precision: int = N.PREC_FP32,
+                 device="cuda", lr: float = 1e-4, process_group=None, resx: Optional[int] = None,
+                 fused_dp: Optional[bool] = None):
+        super().__init__(video, precision, device, lr, process_group, resx)
+        self.cfg = dict(DEFAULTS)
+        if config:
+            self.cfg.update({k: v for k, v in config.items() if k in DEFAULTS})
+            check_architecture(config)
+        # the mapping of src/stage1_neural_atlas.py:112-119, with the positional encoding the config may ask for
+        self.map_desc = make_desc(**dict(MAPPING_DESC, pe_freqs=mapping_pe_freqs(config)))
+        self.atlas_desc = make_desc(**ATLAS_DESC)
+        self.map_w, self.map_b, self.map_total = mlp_layout(self.map_desc)
+        self.atl_w, self.atl_b, self.atl_total = mlp_layout(self.atlas_desc)
+        self.n_params = int(self.lib.b200_atlas_param_floats_for(C.byref(self.map_desc)))
+        assert self.n_params == self.map_total + self.atl_total
+        self.descs = dict(mapping=self.map_desc, atlas=self.atlas_desc)
+        self.offsets = dict(mapping=0, atlas=self.map_total)
+        self.layouts = dict(mapping=(self.map_w, self.map_b, self.map_total),
+                            atlas=(self.atl_w, self.atl_b, self.atl_total))
+        self._allocate(N.LOSS_FLOATS, fused_dp)
+
+    def load_state(self, mapping_sd: Dict[str, torch.Tensor], atlas_sd: Dict[str, torch.Tensor]):
+        super().load_state(dict(mapping=mapping_sd, atlas=atlas_sd))
 
     # ------------------------------------------------------------------ native calls
     def _config(self, with_global: bool) -> N.AtlasConfig:
@@ -408,8 +543,8 @@ class AtlasTrainer:
             cfg = self._config(True)
             md = C.byref(self.map_desc)
             nbytes = int(self.lib.b200_atlas_workspace_bytes_for(C.byref(cfg), md))
-            if cfg.batch < 10000:        # pre_train_mapping always draws 10000 pixels (unwrap_utils.py:183)
-                cfg.batch = 10000
+            if cfg.batch < PRETRAIN_BATCH:        # pretrain shares this workspace
+                cfg.batch = PRETRAIN_BATCH
                 nbytes = max(nbytes, int(self.lib.b200_atlas_workspace_bytes_for(C.byref(cfg), md)))
             if nbytes < 0:
                 raise N.B200Error(self.lib.b200_last_error().decode())
@@ -443,109 +578,29 @@ class AtlasTrainer:
                                                   N.ptr(self.losses), N.ptr(ws), ws.numel(), N.current_stream()),
                 "b200_atlas_loss_grad_for")
 
-    # ------------------------------------------------------------------ data parallelism over NVLink peer memory
-    def dp_adam(self):
-        """reduce-scatter + Adam + all-gather in one kernel (b200_dp_adam_step)."""
-        self._dp.adam_step(self.exp_avg, self.exp_avg_sq, self.lr, self.step_count)
+    def _trip(self, it: int):
+        self.loss_grad(self.uses_global(it))
 
-    def gather_moments(self):
-        """With the fused optimiser a rank maintains only the Adam moments of its slice: assemble the full state
-        (checkpoint time) with one all-reduce of the owned slices."""
-        if self._dp is not None:
-            self._dp.gather_moments(self.exp_avg, self.exp_avg_sq)
-
-    def all_reduce(self):
-        if self.pg is not None and self.world > 1:
-            import torch.distributed as dist
-            dist.all_reduce(self.grad_loss, group=self.pg)      # one collective: 2.7 MB grads + 8 losses
-
-    def adam(self, params=None, grads=None, m=None, v=None, step=None, n=None):
-        params = self.params if params is None else params
-        N.check(self.lib.b200_adam_step(N.ptr(params), N.ptr(self.grads if grads is None else grads),
-                                        N.ptr(self.exp_avg if m is None else m),
-                                        N.ptr(self.exp_avg_sq if v is None else v),
-                                        self.n_params if n is None else n, self.lr, 0.9, 0.999, 1e-8, 1.0,
-                                        N.ptr(self.step_count if step is None else step), N.current_stream()),
-                "b200_adam_step")
-
-    def _iteration(self, with_global: bool):
-        self.loss_grad(with_global)
-        if self._dp is not None:
-            self.dp_adam()
-        else:
-            self.all_reduce()
-            self.adam()
-
-    def step(self, it: int, use_graph: bool = True):
-        """One loop trip on the indices in self.indices (device).  Returns the device loss vector
-        (valid after the stream reaches this point)."""
-        wg = self.uses_global(it)
-        if not use_graph or self.device.type != "cuda":
-            self._iteration(wg)
-            return self.losses
-        g = self._graphs.get(("step", wg))
-        if g is None:
-            # warm-up outside capture (lazy module load, NCCL channels), restoring the state after
-            snap = [t.clone() for t in (self.params, self.exp_avg, self.exp_avg_sq, self.step_count)]
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                self._iteration(wg)
-            torch.cuda.current_stream().wait_stream(side)
-            torch.cuda.synchronize()
-            for t, s in zip((self.params, self.exp_avg, self.exp_avg_sq, self.step_count), snap):
-                t.copy_(s)
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._iteration(wg)
-            # capture does not execute; state is unchanged here
-            self._graphs[("step", wg)] = g
-        g.replay()
-        return self.losses
-
-    def step_host(self, inds_cpu: torch.Tensor, it: int, use_graph: bool = True) -> np.ndarray:
-        """End-to-end call with HOST buffers: pinned H2D of the index batch, one loop trip,
-        D2H of the loss vector (the step's result).  Synchronous."""
-        self._pin_inds.copy_(inds_cpu.reshape(-1))
-        self.indices.copy_(self._pin_inds, non_blocking=True)
-        losses = self.step(it, use_graph)
-        self._pin_loss.copy_(losses, non_blocking=True)
-        torch.cuda.current_stream().synchronize()
-        return self._pin_loss.numpy().copy()
+    def _regime(self, it: int):
+        return self.uses_global(it)
 
     # ------------------------------------------------------------------ pre-training
     def pretrain(self, T: int, H: int, W: int, iters: int, generator: Optional[torch.Generator] = None,
                  progress=None):
-        """pre_train_mapping (unwrap_utils.py:176-198): `iters` sweeps over the T frames, 10 000 random
-        pixels of one frame per step, its own Adam(lr=1e-4) on the mapping block only.  Index draws
-        come from the CPU generator in the reference's order (rows, then columns)."""
+        """pre_train_mapping of the mapping block (FlatTrainer._pretrain).  Returns the device loss vector of the last
+        step, None when no step ran."""
         larger = max(W, H)
         cfg = self._config(False)
-        cfg.batch = 10000                      # unwrap_utils.py:183 hard-codes 10000, whatever samples_batch is
+        cfg.batch = PRETRAIN_BATCH
         ws = self._workspace()
-        n = self.map_total
-        m = torch.zeros(n, dtype=torch.float32, device=self.device)
-        v = torch.zeros(n, dtype=torch.float32, device=self.device)
-        step = torch.zeros(1, dtype=torch.int64, device=self.device)
-        ys_d = torch.zeros(10000, dtype=torch.int64, device=self.device)
-        xs_d = torch.zeros(10000, dtype=torch.int64, device=self.device)
-        last = None
-        for i in range(iters):
-            for f in range(T):
-                ys = torch.randint(H, (10000, 1), generator=generator)
-                xs = torch.randint(W, (10000, 1), generator=generator)
-                ys_d.copy_(ys.reshape(-1), non_blocking=True)
-                xs_d.copy_(xs.reshape(-1), non_blocking=True)
-                N.check(self.lib.b200_pretrain_loss_grad_for(C.byref(cfg), C.byref(self.map_desc), larger, T, f,
-                                                             N.ptr(ys_d), N.ptr(xs_d), N.ptr(self.params),
-                                                             N.ptr(self.grads), N.ptr(self.losses), N.ptr(ws),
-                                                             ws.numel(), N.current_stream()),
-                        "b200_pretrain_loss_grad_for")
-                self.adam(self.params, self.grads, m, v, step, n)
-                last = self.losses
-            if progress:
-                progress(i)
-        return last
+
+        def loss_grad(f, ys, xs):
+            N.check(self.lib.b200_pretrain_loss_grad_for(C.byref(cfg), C.byref(self.map_desc), larger, T, f,
+                                                         N.ptr(ys), N.ptr(xs), N.ptr(self.params), N.ptr(self.grads),
+                                                         N.ptr(self.losses), N.ptr(ws), ws.numel(),
+                                                         N.current_stream()), "b200_pretrain_loss_grad_for")
+        self._pretrain(self.net_slice("mapping"), T, H, W, iters, generator, progress, loss_grad)
+        return self.losses if iters > 0 and T > 0 else None
 
     # ------------------------------------------------------------------ render / evaluate
     def render_frame(self, f: int, H: int, W: int, T: int, chunk: Optional[int] = None, want_u8: bool = False,
@@ -557,10 +612,7 @@ class AtlasTrainer:
         rgb = torch.empty(H * W * 3, dtype=torch.float32, device=self.device)
         u8 = torch.empty(H * W * 3, dtype=torch.uint8, device=self.device) if want_u8 else None
         md = C.byref(self.map_desc)
-        nbytes = int(self.lib.b200_render_workspace_bytes_for(md, chunk))
-        ws = getattr(self, "_render_ws", None)
-        if ws is None or ws.numel() < nbytes:
-            ws = self._render_ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        ws = self._scratch_buffer("render", int(self.lib.b200_render_workspace_bytes_for(md, chunk)))
         for p0 in range(0, H * W, chunk):
             p1 = min(H * W, p0 + chunk)
             N.check(self.lib.b200_render_for(md, N.ptr(self.params), H, W, T, f, p0, p1, N.ptr(rgb[p0 * 3:]),
@@ -568,7 +620,6 @@ class AtlasTrainer:
                                              ws.numel(), N.current_stream()), "b200_render_for")
         out = rgb.view(H, W, 3)
         return (out, u8.view(H, W, 3)) if want_u8 else out
-
 
     def eval_maps(self, f: int, chunk: Optional[int] = None):
         """Per-pixel maps of frame f that the reference's evaluation dashboards show (evaluate.py:640-700): uv (H, W, 2),
@@ -579,10 +630,7 @@ class AtlasTrainer:
         uv = torch.empty(H * W * 2, dtype=torch.float32, device=self.device)
         rig = torch.empty(H * W, dtype=torch.float32, device=self.device)
         flow = torch.empty(H * W, dtype=torch.float32, device=self.device)
-        nbytes = int(self.lib.b200_eval_maps_workspace_bytes(C.byref(self.map_desc), chunk))
-        ws = getattr(self, "_eval_ws", None)
-        if ws is None or ws.numel() < nbytes:
-            ws = self._eval_ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        ws = self._scratch_buffer("eval", int(self.lib.b200_eval_maps_workspace_bytes(C.byref(self.map_desc), chunk)))
         for p0 in range(0, H * W, chunk):
             p1 = min(H * W, p0 + chunk)
             N.check(self.lib.b200_eval_maps(C.byref(self.map_desc), N.ptr(self.params), C.byref(v.struct), f, p0, p1,

@@ -10,14 +10,12 @@ Mirrors, on the reference side (paths relative to the reference root):
 from __future__ import annotations
 
 import ctypes as C
-import math
 from typing import Dict, Optional
 
-import numpy as np
 import torch
 
 from . import _native as N
-from .atlas import DeviceVideo, FusedDp, layer_dims, make_desc, mlp_layout
+from .atlas import PRETRAIN_BATCH, DeviceVideo, FlatTrainer, make_desc, mlp_layout
 
 # hyper-parameters of src/config/config_flow_100.json that the seg loop reads
 SEG_DEFAULTS = dict(
@@ -33,7 +31,6 @@ SEG_DEFAULTS = dict(
     positional_encoding_num_atlas=10)
 
 NETS = ("mapping1", "mapping2", "alpha", "atlas")          # optimiser-group order (:165-169) = flat-buffer order
-CONSTRUCTION_ORDER = ("mapping1", "mapping2", "atlas", "alpha")   # order the script builds them (:127-161)
 LOSS_NAMES = ("total", "rgb", "gradient", "sparsity", "rigidity1", "rigidity2", "rigidity_global1", "rigidity_global2",
               "flow1", "flow2", "flow_alpha", "bootstrapping", "n_fwd", "n_bwd")
 
@@ -69,29 +66,28 @@ def pack_mask_frames(mask_frames: torch.Tensor, device, t_begin: int = 0, t_end:
     return mask_frames[:, :, t_begin:t_end].permute(2, 0, 1).contiguous().to(device=device, dtype=torch.float32)
 
 
-class SegTrainer:
+class SegTrainer(FlatTrainer):
     """Flat parameters / optimiser state of (mapping1, mapping2, alpha, atlas) + the seg step.
 
     Frame-sharded data parallelism: with a `process_group`, `video` holds this rank's frame block (DeviceVideo with
     t_begin / t_end and the whole-video bitmaps) and `mask` the matte of those frames (pack_mask_frames(..., t_begin,
     t_end)); every rank draws the same index batch.  A rank's trip normalises by the global batch and flow counts,
     so one SUM over the ranks of [gradients || loss vector] gives the unsharded trip (loss entries 12, 13, the flow
-    counts, then read world * count).  The exchange is b200_dp_adam_step over symmetric memory (FusedDp) when
-    available -- `fused_dp` True requires it, also on one rank; False or a failed set-up use NCCL all-reduce + the
-    local Adam."""
+    counts, then read world * count).  FlatTrainer describes the exchange and `fused_dp`."""
+
+    NETS = NETS
+    CONSTRUCTION_ORDER = ("mapping1", "mapping2", "atlas", "alpha")   # order the script builds them (:127-161)
 
     def __init__(self, video: Optional[DeviceVideo], mask: Optional[torch.Tensor], config: Optional[dict] = None,
                  precision: int = N.PREC_FP32, device="cuda", lr: float = 1e-4, resx: Optional[int] = None,
                  process_group=None, fused_dp: Optional[bool] = None):
-        self.lib = N.lib()
-        self.video, self.mask = video, mask
+        super().__init__(video, precision, device, lr, process_group, resx)
+        self.mask = mask
         self.cfg = dict(SEG_DEFAULTS)
         if config:
             self.cfg.update({k: v for k, v in config.items() if k in SEG_DEFAULTS})
         if float(self.cfg["global_rigidity_derivative_amount_fg"]) != float(self.cfg["global_rigidity_derivative_amount_bg"]):
             raise N.B200Error("global_rigidity_derivative_amount_fg and _bg must be equal (both 100 in the reference's config)")
-        self.precision, self.device, self.lr = precision, torch.device(device), lr
-        self.resx = resx if resx is not None else (video.W if video is not None else 0)
         self.descs = seg_descs(self.cfg)
         offs = (C.c_int64 * 4)()
         c0 = self._config(0)
@@ -100,101 +96,7 @@ class SegTrainer:
             raise N.B200Error("invalid network configuration")
         self.offsets = dict(zip(NETS, [int(o) for o in offs]))
         self.layouts = {k: mlp_layout(self.descs[k]) for k in NETS}
-        dev = self.device
-        self.pg, self.world = process_group, 1
-        if process_group is not None:
-            import torch.distributed as dist
-            self.world = dist.get_world_size(process_group)
-        # gradients + the loss vector share one buffer so that data parallelism needs ONE exchange
-        self._dp = None
-        if process_group is not None and dev.type == "cuda" and fused_dp is not False and (self.world > 1 or fused_dp):
-            self._dp = FusedDp.create(process_group, dev, self.n_params, N.SEG_LOSS_FLOATS, required=bool(fused_dp))
-        if self._dp is None:
-            self.params = torch.zeros(self.n_params, dtype=torch.float32, device=dev)
-            self.grad_loss = torch.zeros(self.n_params + N.SEG_LOSS_FLOATS, dtype=torch.float32, device=dev)
-        else:
-            self.params, self.grad_loss = self._dp.params, self._dp.grad_loss
-        self.grads = self.grad_loss[:self.n_params]
-        self.losses = self.grad_loss[self.n_params:]
-        self.exp_avg = torch.zeros_like(self.params)
-        self.exp_avg_sq = torch.zeros_like(self.params)
-        self.step_count = torch.zeros(1, dtype=torch.int64, device=dev)
-        B = int(self.cfg["samples_batch"])
-        self.indices = torch.zeros(B, dtype=torch.int64, device=dev)
-        self._pin_inds = torch.zeros(B, dtype=torch.int64).pin_memory() if dev.type == "cuda" else None
-        self._pin_loss = torch.zeros(N.SEG_LOSS_FLOATS, dtype=torch.float32).pin_memory() if dev.type == "cuda" else None
-        self._ws = None
-        self._render_ws = None
-        self._graphs = {}
-
-    # ------------------------------------------------------------------ parameters / state dicts
-    def _views(self, flat, which):
-        desc = self.descs[which]
-        w, b, _ = self.layouts[which]
-        base = self.offsets[which]
-        out = {}
-        for i, (k, n) in enumerate(layer_dims(desc)):
-            out[f"hidden.{i}.weight"] = flat[base + w[i]: base + w[i] + k * n].view(n, k)
-            out[f"hidden.{i}.bias"] = flat[base + b[i]: base + b[i] + n]
-        return out
-
-    def param_views(self, which):
-        return self._views(self.params, which)
-
-    def grad_views(self, which):
-        return self._views(self.grads, which)
-
-    def net_slice(self, which):
-        return slice(self.offsets[which], self.offsets[which] + self.layouts[which][2])
-
-    def init_like_reference(self):
-        """nn.Linear's default init on the global CPU generator in the script's construction order
-        (mapping1, mapping2, atlas, alpha), weight before bias."""
-        for which in CONSTRUCTION_ORDER:
-            views = self.param_views(which)
-            for i, (k, n) in enumerate(layer_dims(self.descs[which])):
-                bound = 1.0 / math.sqrt(k)
-                views[f"hidden.{i}.weight"].copy_(torch.empty(n, k).uniform_(-bound, bound))
-                views[f"hidden.{i}.bias"].copy_(torch.empty(n).uniform_(-bound, bound))
-
-    def load_state(self, sds: Dict[str, Dict[str, torch.Tensor]]):
-        for which, sd in sds.items():
-            for k, v in self.param_views(which).items():
-                v.copy_(sd[k].to(self.device, torch.float32))
-
-    def state_dict(self, which):
-        return {k: v.detach().clone() for k, v in self.param_views(which).items()}
-
-    def optimizer_state_dict(self):
-        """Schema of torch.optim.Adam.state_dict() for the four groups of :165-169 (what evaluate.py:223 stores).
-        Collective under the fused optimiser: every rank calls it."""
-        self.gather_moments()
-        state, groups, idx = {}, [], 0
-        step = self.step_count.detach().float().cpu().reshape(())
-        for which in NETS:
-            m, v = self._views(self.exp_avg, which), self._views(self.exp_avg_sq, which)
-            ids = []
-            for k in m:
-                state[idx] = {"step": step.clone(), "exp_avg": m[k].detach().clone(), "exp_avg_sq": v[k].detach().clone()}
-                ids.append(idx)
-                idx += 1
-            groups.append({"lr": self.lr, "betas": (0.9, 0.999), "eps": 1e-8, "weight_decay": 0, "amsgrad": False,
-                           "maximize": False, "foreach": None, "capturable": False, "differentiable": False,
-                           "fused": None, "params": ids})
-        return {"state": state, "param_groups": groups}
-
-    def load_optimizer_state_dict(self, sd):
-        idx, step = 0, 0
-        for which in NETS:
-            m, v = self._views(self.exp_avg, which), self._views(self.exp_avg_sq, which)
-            for k in m:
-                st = sd["state"].get(idx)
-                if st is not None:
-                    m[k].copy_(st["exp_avg"].to(self.device))
-                    v[k].copy_(st["exp_avg_sq"].to(self.device))
-                    step = int(st["step"])
-                idx += 1
-        self.step_count.fill_(step)
+        self._allocate(N.SEG_LOSS_FLOATS, fused_dp)
 
     # ------------------------------------------------------------------ native calls
     def _config(self, it: int) -> N.SegConfig:
@@ -225,74 +127,13 @@ class SegTrainer:
                                             N.ptr(self.params), N.ptr(self.grads), N.ptr(self.losses), N.ptr(ws),
                                             ws.numel(), N.current_stream()), "b200_seg_loss_grad")
 
-    def adam(self, sl: Optional[slice] = None, m=None, v=None, step=None):
-        sl = slice(0, self.n_params) if sl is None else sl
-        N.check(self.lib.b200_adam_step(N.ptr(self.params[sl]), N.ptr(self.grads[sl]),
-                                        N.ptr(self.exp_avg[sl] if m is None else m),
-                                        N.ptr(self.exp_avg_sq[sl] if v is None else v), sl.stop - sl.start, self.lr,
-                                        0.9, 0.999, 1e-8, 1.0, N.ptr(self.step_count if step is None else step),
-                                        N.current_stream()), "b200_adam_step")
-
-    def dp_adam(self):
-        """reduce-scatter + Adam + all-gather in one kernel (b200_dp_adam_step)."""
-        self._dp.adam_step(self.exp_avg, self.exp_avg_sq, self.lr, self.step_count)
-
-    def gather_moments(self):
-        """Under the fused optimiser a rank keeps the Adam moments of its slice only: assemble them (collective)."""
-        if self._dp is not None:
-            self._dp.gather_moments(self.exp_avg, self.exp_avg_sq)
-
-    def all_reduce(self):
-        if self.pg is not None and self.world > 1:
-            import torch.distributed as dist
-            dist.all_reduce(self.grad_loss, group=self.pg)      # one collective: gradients || loss vector
-
-    def _iteration(self, it: int):
+    def _trip(self, it: int):
         self.loss_grad(it)
-        if self._dp is not None:
-            self.dp_adam()
-        else:
-            self.all_reduce()
-            self.adam()
 
-    def step(self, it: int, use_graph: bool = True):
-        """One loop trip on the indices in self.indices (device): losses + gradients, the exchange between ranks (if
-        any), then one Adam update of all four networks (same lr / betas in every group, so one sweep over the flat
-        buffer).  The trip is captured once per regime (global rigidity on / off, bootstrapping on / off) in a CUDA
-        graph and replayed."""
-        if not use_graph or self.device.type != "cuda":
-            self._iteration(it)
-            return self.losses
+    def _regime(self, it: int):
+        """Global rigidity on / off and bootstrapping on / off."""
         cfg = self._config(it)
-        key = (int(cfg.with_global), float(cfg.bootstrapping_factor))
-        g = self._graphs.get(key)
-        if g is None:
-            # eager warm-up on a side stream (builds the cached job tables), state restored afterwards; then capture
-            state = (self.params, self.exp_avg, self.exp_avg_sq, self.step_count)
-            snap = [t.clone() for t in state]
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                self._iteration(it)
-            torch.cuda.current_stream().wait_stream(side)
-            torch.cuda.synchronize()
-            for t, c in zip(state, snap):
-                t.copy_(c)
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._iteration(it)
-            self._graphs[key] = g
-        g.replay()
-        return self.losses
-
-    def step_host(self, inds_cpu: torch.Tensor, it: int) -> np.ndarray:
-        """End-to-end call with HOST buffers: pinned H2D of the index batch, one loop trip, D2H of the loss vector."""
-        self._pin_inds.copy_(inds_cpu.reshape(-1))
-        self.indices.copy_(self._pin_inds, non_blocking=True)
-        losses = self.step(it)
-        self._pin_loss.copy_(losses, non_blocking=True)
-        torch.cuda.current_stream().synchronize()
-        return self._pin_loss.numpy().copy()
+        return int(cfg.with_global), float(cfg.bootstrapping_factor)
 
     def loss_dict(self, losses=None) -> Dict[str, float]:
         v = (self.losses if losses is None else torch.as_tensor(losses)).detach().float().cpu().numpy()
@@ -301,32 +142,20 @@ class SegTrainer:
     # ------------------------------------------------------------------ pre-training
     def pretrain(self, which: str, T: int, H: int, W: int, iters: int, generator: Optional[torch.Generator] = None,
                  progress=None):
-        """pre_train_mapping (unwrap_utils.py:176-198) of one of the two mapping networks: its own Adam(lr=1e-4),
-        10 000 random pixels of one frame per step, index draws from the CPU generator in the reference's order."""
+        """pre_train_mapping of one of the two mapping networks (FlatTrainer._pretrain).  Returns the device loss of
+        the last step."""
         desc, sl = self.descs[which], self.net_slice(which)
-        n = sl.stop - sl.start
         larger = max(W, H)
-        nbytes = int(self.lib.b200_mlp_pretrain_workspace_bytes(C.byref(desc), 10000))
+        nbytes = int(self.lib.b200_mlp_pretrain_workspace_bytes(C.byref(desc), PRETRAIN_BATCH))
         ws = torch.zeros(nbytes, dtype=torch.uint8, device=self.device)
-        m = torch.zeros(n, dtype=torch.float32, device=self.device)
-        v = torch.zeros_like(m)
-        step = torch.zeros(1, dtype=torch.int64, device=self.device)
-        ys_d = torch.zeros(10000, dtype=torch.int64, device=self.device)
-        xs_d = torch.zeros_like(ys_d)
         loss = torch.zeros(1, dtype=torch.float32, device=self.device)
-        for i in range(iters):
-            for f in range(T):
-                ys = torch.randint(H, (10000, 1), generator=generator)
-                xs = torch.randint(W, (10000, 1), generator=generator)
-                ys_d.copy_(ys.reshape(-1), non_blocking=True)
-                xs_d.copy_(xs.reshape(-1), non_blocking=True)
-                N.check(self.lib.b200_mlp_pretrain_loss_grad(
-                    C.byref(desc), 10000, float(self.cfg["uv_mapping_scale"]), larger, T, f, N.ptr(ys_d), N.ptr(xs_d),
-                    N.ptr(self.params[sl]), N.ptr(self.grads[sl]), N.ptr(loss), self.precision, N.ptr(ws), ws.numel(),
-                    N.current_stream()), "b200_mlp_pretrain_loss_grad")
-                self.adam(sl, m, v, step)
-            if progress:
-                progress(i)
+
+        def loss_grad(f, ys, xs):
+            N.check(self.lib.b200_mlp_pretrain_loss_grad(
+                C.byref(desc), PRETRAIN_BATCH, float(self.cfg["uv_mapping_scale"]), larger, T, f, N.ptr(ys), N.ptr(xs),
+                N.ptr(self.params[sl]), N.ptr(self.grads[sl]), N.ptr(loss), self.precision, N.ptr(ws), ws.numel(),
+                N.current_stream()), "b200_mlp_pretrain_loss_grad")
+        self._pretrain(sl, T, H, W, iters, generator, progress, loss_grad)
         return loss
 
     # ------------------------------------------------------------------ reconstruction
@@ -338,10 +167,7 @@ class SegTrainer:
         rgb = torch.empty(H * W * 3, dtype=torch.float32, device=self.device)
         alpha = torch.empty(H * W, dtype=torch.float32, device=self.device)
         u8 = torch.empty(H * W * 3, dtype=torch.uint8, device=self.device) if want_u8 else None
-        nbytes = int(self.lib.b200_seg_render_workspace_bytes(C.byref(cfg), chunk))
-        if self._render_ws is None or self._render_ws.numel() < nbytes:
-            self._render_ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
-        ws = self._render_ws
+        ws = self._scratch_buffer("render", int(self.lib.b200_seg_render_workspace_bytes(C.byref(cfg), chunk)))
         for p0 in range(0, H * W, chunk):
             p1 = min(H * W, p0 + chunk)
             N.check(self.lib.b200_seg_render(C.byref(cfg), N.ptr(self.params), H, W, T, f, p0, p1, N.ptr(rgb[p0 * 3:]),

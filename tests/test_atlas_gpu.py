@@ -399,6 +399,47 @@ def test_dp_adam_single_rank_equals_adam():
     assert covered == n + extra
 
 
+@pytest.fixture
+def one_rank_group():
+    import torch.distributed as dist
+    os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
+    os.environ.setdefault("MASTER_PORT", str(29700 + os.getpid() % 1000))
+    torch.cuda.set_device(0)
+    dist.init_process_group("nccl", rank=0, world_size=1, device_id=torch.device("cuda", 0))
+    yield dist.group.WORLD
+    dist.destroy_process_group()
+
+
+@pytest.mark.parametrize("fused", [True, False])
+def test_trainer_with_one_rank_group_matches_ungrouped(golden_dir, one_rank_group, fused):
+    """With a one-rank NCCL group the trainer takes the fused optimiser exactly when fused_dp is True (the rule of the
+    segmentation trainer), and three graph-replayed steps match the ungrouped trainer on the same index batches.  The
+    exchange and Adam are bit-exact (test_dp_adam_single_rank_equals_adam); the trip's fp32 atomics may sum in another
+    order, so losses agree to rtol 1e-4 and parameters to 6e-4, the most three Adam steps of lr 1e-4 can diverge."""
+    data, _ = _golden_video(golden_dir)
+    B = 64
+    vid = A.DeviceVideo.from_reference_layout(data, DEV)
+    try:
+        grouped = A.AtlasTrainer(vid, {"samples_batch": B}, device=DEV, process_group=one_rank_group, fused_dp=fused)
+    except Exception as e:                      # noqa: BLE001 - symmetric memory unavailable on this machine
+        if fused:
+            pytest.skip(f"torch symmetric memory unavailable: {type(e).__name__}: {e}")
+        raise
+    assert (grouped._dp is not None) == fused
+    plain = A.AtlasTrainer(vid, {"samples_batch": B}, device=DEV)
+    mp, ap = _params(golden_dir)
+    for tr in (grouped, plain):
+        tr.load_state(O.state_dict_of(mp), O.state_dict_of(ap))
+    gi = torch.Generator().manual_seed(21)
+    for it in range(3):
+        inds = torch.randint(vid.num_pixels, (B, 1), generator=gi)
+        a, b = grouped.step_host(inds, it), plain.step_host(inds, it)
+        np.testing.assert_allclose(a[:6], b[:6], rtol=1e-4)
+        assert a[6] == b[6] and a[7] == b[7]
+    assert int(grouped.step_count) == int(plain.step_count) == 3
+    torch.testing.assert_close(grouped.params, plain.params, rtol=0, atol=6e-4)
+
+
 @pytest.mark.parametrize("precision", [N.PREC_FP32, N.PREC_TC])
 def test_eval_maps_match_reference_fixture(golden_dir, precision):
     """b200_eval_maps (uv, per-pixel rigidity, forward flow error of a whole frame) against the fixture frozen from the
