@@ -66,9 +66,20 @@ __host__ __device__ __forceinline__ int item_off(int n, int k) {          // k i
 // ---------------------------------------------------------------------------------------------
 // layout of the tensor-core workspace
 // ---------------------------------------------------------------------------------------------
+// Forward constants of one network, fp32, in the order the forward kernel's shared-memory copy holds them (float
+// offsets): [b_l * S_ACT, l = 0..L-2: 256 each][plain mapping: W0 * S_ACT, [256][3]][output layer: W_{L-1} / S_ACT,
+// [out][k_last]][b_{L-1}, out], padded to 16 bytes.
+struct FwdConsts { int w0, wl, bl, floats; };
+__host__ __device__ constexpr FwdConsts fwd_consts(int L, bool plain, int out, int k_last) {
+  const int w0 = (L - 1) * 256, wl = w0 + (plain ? 768 : 0), bl = wl + out * k_last;
+  return FwdConsts{w0, wl, bl, (bl + out + 3) / 4 * 4};
+}
+constexpr int FWD_CST_BYTES = 10752;                 // the largest block: the atlas, 2683 floats
+
 struct NetImages {
   // forward weight items, consumption order: per TC layer, per 64-wide k chunk: hi k 0-31, hi k 32-63, lo k 0-31, lo 32-63
   char* w_fwd; int64_t w_fwd_layer[B200_MAX_LAYERS]; int n_chunks_fwd[B200_MAX_LAYERS];
+  float* cst; int cst_floats;             // forward constants (FwdConsts)
   // dgrad weight items (W^T): per layer, per 64-wide chunk of the reduction (out) index: the same four items
   char* w_bwd; int64_t w_bwd_layer[B200_MAX_LAYERS];
   // activation images h_0..h_{L-2} and dZ images: [slot][term][tile][4 atoms][16 KB]
@@ -98,6 +109,8 @@ static void plan_fwd_weights(const MlpShape& s, TcNet net, char*& p, NetImages* 
     off += (int64_t)chunks * CHUNK_BYTES;
   }
   n->w_fwd = carve_tc(p, off);
+  n->cst_floats = fwd_consts(s.L, !pe, s.out_dim, s.K[s.L - 1]).floats;
+  n->cst = reinterpret_cast<float*>(carve_tc(p, (int64_t)n->cst_floats * 4));
 }
 
 static void plan_net(const MlpShape& s, int64_t rows, TcNet net, char*& p, NetImages* n) {
@@ -148,12 +161,19 @@ struct PrepJob {
   int n_rows, k0, k_cnt;            // valid image rows and the window [k0, k0+k_cnt) of the other index
   int transpose;                    // 0: image(row=n, col=k-k0) = W[n][k];  1: image(row=k, col=n-k0) = W[n][k]
   char* hi; char* lo;               // destination: two 16 KB items each (k 0-31, k 32-63), zero padded
+  float* f32; float f32_scale;      // non-null: a forward-constant job instead, f32[i] = W[i] * f32_scale, i < n_rows
 };
-constexpr int MAX_PREP_JOBS = 96;
+constexpr int MAX_PREP_JOBS = 128;
 struct PrepJobs { PrepJob j[MAX_PREP_JOBS]; int n; };
 
 __global__ void tc_prep_kernel(const PrepJobs* __restrict__ jobs_ptr) {
   const PrepJob jb = jobs_ptr->j[blockIdx.x >> 2];
+  if (jb.f32) {
+    // the same fp32 products the forward kernel formed from the parameters before (no fast math: bit for bit)
+    for (int i = (blockIdx.x & 3) * blockDim.x + threadIdx.x; i < jb.n_rows; i += 4 * blockDim.x)
+      jb.f32[i] = jb.W[i] * jb.f32_scale;
+    return;
+  }
   // one job = 256 rows x 64 cols; this block does 64 rows; thread handles one 16-byte chunk at a time
   for (int e = threadIdx.x; e < 64 * 8; e += blockDim.x) {
     const int row = (blockIdx.x & 3) * 64 + (e >> 3), c8 = (e & 7) * 8;
@@ -349,22 +369,23 @@ constexpr int BWD_ACC_FLOATS = 5 * 256 + 768;
 constexpr int SMEM_BWD_CONST_FLOATS = CONSUMER_WGS * (RSUM_B_BYTES / 4 + BWD_ACC_FLOATS);
 constexpr int SMEM_BARS = 256;
 constexpr int SMEM_MAX = 227 * 1024;                         // opt-in shared memory of one sm_90 CTA
-// Every kernel keeps as many 16 KB weight slots as the shared memory allows next to the A tile and, in the atlas
-// forward, the positional-encoding tile (6 mapping forward, 4 atlas forward); the backward kernels also hold their
-// gradient accumulators and row-sum operands (5 slots).
+// Every kernel keeps as many 16 KB weight slots as the shared memory allows next to the A tile and its constants.  The
+// forward kernels hold their network's forward constants (FwdConsts, <= 10.5 KB) resident, which costs one slot: 5 in
+// the mapping forward, 3 in the atlas forward, which also holds the positional-encoding tile.  The backward kernels
+// hold their gradient accumulators and row-sum operands (5 slots).
 template <bool ATLAS, bool BWD> struct KCfg {
-  static constexpr int NST = BWD ? 5 : (ATLAS ? 4 : 6);
+  static constexpr int NST = BWD ? 5 : (ATLAS ? 3 : 5);
   static constexpr int SMEM = SMEM_A + NST * ITEM_BYTES + (ATLAS && !BWD ? SMEM_AUX : 0) +
-                              (BWD ? SMEM_BWD_CONST_FLOATS * 4 : 0) + SMEM_BARS;
+                              (BWD ? SMEM_BWD_CONST_FLOATS * 4 : FWD_CST_BYTES) + SMEM_BARS;
   static_assert(SMEM <= SMEM_MAX, "fused kernel exceeds the shared memory of one CTA");
   static_assert(SMEM + ITEM_BYTES > SMEM_MAX, "one more weight slot would fit");
-  static_assert(2 * NST * 8 <= SMEM_BARS, "ring barriers exceed their shared-memory slot");
+  static_assert(2 * NST * 8 + 8 <= SMEM_BARS, "ring and constant barriers exceed their shared-memory slot");
 };
 
 template <int NST>
 struct SmemMap {
   char* a_tile; char* stage; char* aux; float* cst;
-  uint64_t* full; uint64_t* empty;
+  uint64_t* full; uint64_t* empty;   // [NST] each; the forward's constants barrier follows at empty[NST]
   __device__ __forceinline__ void init(char* raw, int aux_bytes, int cst_floats) {
     char* p = raw;                                   // 1024-aligned (checked in setup_cta)
     a_tile = p; p += SMEM_A;
@@ -377,10 +398,11 @@ struct SmemMap {
 };
 
 template <int NST>
-__device__ __forceinline__ void setup_cta(SmemMap<NST>& sm) {
+__device__ __forceinline__ void setup_cta(SmemMap<NST>& sm, bool cst_bar = false) {
   if (threadIdx.x == 0) {
     if (smem_u32(sm.a_tile) & 1023u) __trap();   // the swizzled operand layouts need 1024-byte alignment
     for (int i = 0; i < NST; ++i) { mbar_init(&sm.full[i], 1); mbar_init(&sm.empty[i], EMPTY_ARRIVALS); }
+    if (cst_bar) mbar_init(&sm.empty[NST], 1);
     fence_barrier_init();
   }
   __syncthreads();
@@ -415,7 +437,7 @@ template <bool ATLAS, int NL = (ATLAS ? 8 : 6), int VAR = 0>
 __global__ void __launch_bounds__(TC_THREADS, 1) tc_fwd_kernel(const __grid_constant__ FwdParams P) {
   extern __shared__ __align__(1024) char smem_raw[];
   constexpr int NST = KCfg<ATLAS, false>::NST;
-  SmemMap<NST> sm; sm.init(smem_raw, ATLAS ? SMEM_AUX : 0, 0);
+  SmemMap<NST> sm; sm.init(smem_raw, ATLAS ? SMEM_AUX : 0, FWD_CST_BYTES / 4);
   const int warp = warp_uniform(), lane = threadIdx.x & 31;
   constexpr int L = NL;                                   // mapping-shaped networks: 6 (stage-1 script) or 4 layers
   constexpr int FIRST_TC = ATLAS ? 0 : 1;
@@ -424,15 +446,21 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_fwd_kernel(const __grid_cons
   constexpr bool SKIPS = ATLAS && !PE3;                   // PE chunk concatenated at layers 4 and L-1
   constexpr int OUT = ATLAS ? (PE3 ? VAR : 3) : 2;
   constexpr int KLAST = SKIPS ? 296 : 256;
+  constexpr FwdConsts CST = fwd_consts(L, !ATLAS, OUT, KLAST);
+  static_assert(CST.floats * 4 <= FWD_CST_BYTES, "forward constants exceed their shared-memory slot");
+  uint64_t* cst_full = &sm.empty[NST];
   // real encoding columns of the 3-input family; the alpha network's 5 frequencies are part of its identity (tc_net_of)
   const int pe_cols = VAR == 1 ? 30 : 6 * P.pe_freqs;
-  setup_cta(sm);
+  setup_cta(sm, true);
   TileIter ti; ti.init(P.cap, P.n_groups, P.n_valid, P.g_fwd, P.g_bwd);
 
   if (warp >= CONSUMER_WGS * 4) {
     // ------------------------------------------------------------------ producer (consumption order)
     setmaxnreg_dec<PRODUCER_REGS>();
     if (warp == CONSUMER_WGS * 4 && lane == 0) {
+      // the constants, once per CTA, ahead of the first weight item
+      mbar_expect_tx(cst_full, CST.floats * 4);
+      bulk_g2s(sm.cst, P.img.cst, CST.floats * 4, cst_full);
       Pipe<NST> pp{sm.full, sm.empty, sm.stage, 0};
       for (int t = blockIdx.x; t < ti.total; t += gridDim.x)
         for (int l = FIRST_TC; l <= LAST_TC; ++l) {
@@ -450,15 +478,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_fwd_kernel(const __grid_cons
   Pipe<NST> pp{sm.full, sm.empty, sm.stage, 0};
   int pending = -1;
   const float inv_scale = 1.0f / S_W;                   // D / (S_a S_w) * S_a : activations stay scaled by S_ACT
-  uint16_t* bits16 = reinterpret_cast<uint16_t*>(P.img.bits);
-  const float* wlast = P.params + P.w_off[L - 1];
+  const float* wlast = sm.cst + CST.wl;                 // W_{L-1} / S_ACT
   const uint32_t a_rows = smem_u32(sm.a_tile) + c.g * WG_ROW_BYTES;
   const uint32_t aux_rows = smem_u32(sm.aux) + c.g * WG_ROW_BYTES;
   float acc[128];
+  mbar_wait(cst_full, 0);
   for (int t = blockIdx.x; t < ti.total; t += gridDim.x) {
     const int gt = ti.global_tile(t);
     const int64_t row0 = (int64_t)gt * TM + c.m0;
-    // epilogue store of one column pair of one row: split into the A tile, flags into `bw`
+    uint16_t* bits_row = reinterpret_cast<uint16_t*>(P.img.bits) + row0 * 16;   // flags of row0 in slot 0
+    // epilogue store of one column pair of one row: split into the A tile
     auto put = [&](int m, int col, float v0, float v1) {
       uint32_t h, lo;
       split2_packed(v0, v1, h, lo);
@@ -472,9 +501,18 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_fwd_kernel(const __grid_cons
       if ((i & 1) == 0) { held0 = b0; held1 = b1; return; }
       b0 = quad_or(b0 | held0); b1 = quad_or(b1 | held1);
       if (P.store_images && c.q == 0) {
-        bits16[((int64_t)slot * P.img.rows + row0) * 16 + (col >> 4)] = (uint16_t)b0;
-        bits16[((int64_t)slot * P.img.rows + row0 + 8) * 16 + (col >> 4)] = (uint16_t)b1;
+        uint16_t* dst = bits_row + (int64_t)slot * P.img.rows * 16 + (col >> 4);
+        dst[0] = (uint16_t)b0;
+        dst[8 * 16] = (uint16_t)b1;
       }
+    };
+    // one bias + ReLU column pair of a tensor-core layer's accumulators: v = relu(acc / S_W + b * S_ACT)
+    auto bias_relu = [&](const float* bias, int i, int col, float (&v)[4]) {
+      const float2 bs = *reinterpret_cast<const float2*>(bias + col);
+      v[0] = fmaxf(__fmaf_rn(acc[4 * i], inv_scale, bs.x), 0.f);
+      v[1] = fmaxf(__fmaf_rn(acc[4 * i + 1], inv_scale, bs.y), 0.f);
+      v[2] = fmaxf(__fmaf_rn(acc[4 * i + 2], inv_scale, bs.x), 0.f);
+      v[3] = fmaxf(__fmaf_rn(acc[4 * i + 3], inv_scale, bs.y), 0.f);
     };
     // ---------------- prologue: layer-0 input
     if (ATLAS) {
@@ -539,19 +577,21 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_fwd_kernel(const __grid_cons
       // layer 0 (3 -> 256) on CUDA cores: h0 = relu(W0 x + b0)
       const float4 x0 = *reinterpret_cast<const float4*>(P.x + row0 * 4);
       const float4 x1 = *reinterpret_cast<const float4*>(P.x + (row0 + 8) * 4);
-      const float* W0 = P.params + P.w_off[0];
-      const float* b0p = P.params + P.b_off[0];
+      const float* b0s = sm.cst;                         // b0 * S_ACT
+      const float* w0s = sm.cst + CST.w0;                // W0 * S_ACT, [256][3]
       a_tile_reusable(c);
 #pragma unroll
       for (int i = 0; i < 32; ++i) {
         const int col = 8 * i + 2 * c.q;
+        const float2 bs = *reinterpret_cast<const float2*>(b0s + col);
+        const float2 wa = *reinterpret_cast<const float2*>(w0s + col * 3);      // W0[col][0..1]
+        const float2 wb = *reinterpret_cast<const float2*>(w0s + col * 3 + 2);  // W0[col][2], W0[col+1][0]
+        const float2 wc = *reinterpret_cast<const float2*>(w0s + col * 3 + 4);  // W0[col+1][1..2]
+        const float w[2][3] = {{wa.x, wa.y, wb.x}, {wb.y, wc.x, wc.y}}, b[2] = {bs.x, bs.y};
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
-          const int n = col + e;
-          const float bs = __ldg(b0p + n) * S_ACT;
-          const float w0 = __ldg(W0 + n * 3) * S_ACT, w1 = __ldg(W0 + n * 3 + 1) * S_ACT, w2 = __ldg(W0 + n * 3 + 2) * S_ACT;
-          acc[4 * i + e] = fmaxf(__fmaf_rn(x0.z, w2, __fmaf_rn(x0.y, w1, __fmaf_rn(x0.x, w0, bs))), 0.f);
-          acc[4 * i + 2 + e] = fmaxf(__fmaf_rn(x1.z, w2, __fmaf_rn(x1.y, w1, __fmaf_rn(x1.x, w0, bs))), 0.f);
+          acc[4 * i + e] = fmaxf(__fmaf_rn(x0.z, w[e][2], __fmaf_rn(x0.y, w[e][1], __fmaf_rn(x0.x, w[e][0], b[e]))), 0.f);
+          acc[4 * i + 2 + e] = fmaxf(__fmaf_rn(x1.z, w[e][2], __fmaf_rn(x1.y, w[e][1], __fmaf_rn(x1.x, w[e][0], b[e]))), 0.f);
         }
         put(c.m0, col, acc[4 * i], acc[4 * i + 1]);
         put(c.m0 + 8, col, acc[4 * i + 2], acc[4 * i + 3]);
@@ -562,11 +602,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_fwd_kernel(const __grid_cons
       if (P.store_images) store_tile_rows(c, sm.a_tile, P.img.act + (int64_t)gt * TILE_IMG_BYTES, P.img.term_stride);
     }
     // ---------------- tensor-core layers
-    float outacc[2][OUT];
-#pragma unroll
-    for (int jj = 0; jj < OUT; ++jj) outacc[0][jj] = outacc[1][jj] = 0.f;
-#pragma unroll 1
-    for (int l = FIRST_TC; l <= LAST_TC; ++l) {
+    auto mma_layer = [&](int l) {
       uint32_t scale = 0u;
       if (ATLAS && (l == 0 || (SKIPS && l == 4)))
         consume_chunk<NST, 256>(pp, acc, aux_rows, aux_rows + ATOM_BYTES, scale, pending, c);
@@ -575,25 +611,29 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_fwd_kernel(const __grid_cons
           consume_chunk<NST, 256>(pp, acc, a_rows + kc * ATOM_BYTES, a_rows + TILE_IMG_BYTES + kc * ATOM_BYTES, scale,
                                   pending, c);
       finish_pass(pp, acc, pending, c);
-      const bool last = (l == LAST_TC);
-      const float* bias = P.params + P.b_off[l];
+    };
+    // every tensor-core layer: bias + ReLU + flags + split into the A tile (the next layer's operand, or the last
+    // layer's activation image); the last one also feeds the output layer on CUDA cores
+    float outacc[2][OUT];
+#pragma unroll
+    for (int jj = 0; jj < OUT; ++jj) outacc[0][jj] = outacc[1][jj] = 0.f;
+#pragma unroll 1
+    for (int l = FIRST_TC; l <= LAST_TC; ++l) {
+      mma_layer(l);
+      const bool last = l == LAST_TC;
+      const float* bias = sm.cst + l * 256;
       a_tile_reusable(c);
 #pragma unroll
       for (int i = 0; i < 32; ++i) {
         const int col = 8 * i + 2 * c.q;
-        const float bs0 = __ldg(bias + col) * S_ACT, bs1 = __ldg(bias + col + 1) * S_ACT;
         float v[4];
-        v[0] = fmaxf(__fmaf_rn(acc[4 * i], inv_scale, bs0), 0.f);
-        v[1] = fmaxf(__fmaf_rn(acc[4 * i + 1], inv_scale, bs1), 0.f);
-        v[2] = fmaxf(__fmaf_rn(acc[4 * i + 2], inv_scale, bs0), 0.f);
-        v[3] = fmaxf(__fmaf_rn(acc[4 * i + 3], inv_scale, bs1), 0.f);
+        bias_relu(bias, i, col, v);
         if (last) {
 #pragma unroll
           for (int jj = 0; jj < OUT; ++jj) {
-            const float wa = __ldg(wlast + jj * KLAST + col) * (1.0f / S_ACT);
-            const float wb = __ldg(wlast + jj * KLAST + col + 1) * (1.0f / S_ACT);
-            outacc[0][jj] = fmaf(v[1], wb, fmaf(v[0], wa, outacc[0][jj]));
-            outacc[1][jj] = fmaf(v[3], wb, fmaf(v[2], wa, outacc[1][jj]));
+            const float2 w = *reinterpret_cast<const float2*>(wlast + jj * KLAST + col);
+            outacc[0][jj] = fmaf(v[1], w.y, fmaf(v[0], w.x, outacc[0][jj]));
+            outacc[1][jj] = fmaf(v[3], w.y, fmaf(v[2], w.x, outacc[1][jj]));
           }
         }
         if (!last || P.store_images) {
@@ -619,7 +659,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_fwd_kernel(const __grid_cons
                            __half2float(*reinterpret_cast<const __half*>(sm.aux + ATOM_BYTES + off));     // S_ACT * pe
 #pragma unroll
           for (int jj = 0; jj < OUT; ++jj)
-            outacc[rr][jj] = fmaf(pv, __ldg(wlast + jj * KLAST + 256 + k) * (1.0f / S_ACT), outacc[rr][jj]);
+            outacc[rr][jj] = fmaf(pv, wlast[jj * KLAST + 256 + k], outacc[rr][jj]);
         }
       }
     }
@@ -627,7 +667,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) tc_fwd_kernel(const __grid_cons
     for (int rr = 0; rr < 2; ++rr)
 #pragma unroll
       for (int jj = 0; jj < OUT; ++jj) {
-        const float o = quad_sum(outacc[rr][jj]) + __ldg(P.params + P.b_off[L - 1] + jj);
+        const float o = quad_sum(outacc[rr][jj]) + sm.cst[CST.bl + jj];
         if (c.q == 0) P.y[(row0 + 8 * rr) * OUT + jj] = P.tanh_out ? tanhf(o) : o;
       }
   }
@@ -1246,11 +1286,22 @@ static void add_prep(PrepJobs& pj, const float* W, int ldw, int n_rows, int k0, 
   PrepJob& j = pj.j[pj.n++];
   j.W = W; j.ldw = ldw; j.n_rows = n_rows; j.k0 = k0; j.k_cnt = k_cnt; j.transpose = transpose;
   j.hi = dst; j.lo = dst + 2 * ITEM_BYTES;
+  j.f32 = nullptr; j.f32_scale = 0.f;
+}
+static void add_const(PrepJobs& pj, const float* src, int n, float scale, float* dst) {
+  PrepJob& j = pj.j[pj.n++];
+  j = PrepJob{};
+  j.W = src; j.n_rows = n; j.f32 = dst; j.f32_scale = scale;
 }
 
 static void prep_jobs_for_net(PrepJobs& pj, const MlpShape& sh, const NetImages& im, const float* pp, TcNet net,
                               bool with_bwd) {
   const bool pe = tc_pe_first(net);
+  const FwdConsts fc = fwd_consts(sh.L, !pe, sh.out_dim, sh.K[sh.L - 1]);
+  for (int l = 0; l < sh.L - 1; ++l) add_const(pj, pp + sh.b_off[l], 256, S_ACT, im.cst + l * 256);
+  if (!pe) add_const(pj, pp + sh.w_off[0], 768, S_ACT, im.cst + fc.w0);
+  add_const(pj, pp + sh.w_off[sh.L - 1], sh.out_dim * sh.K[sh.L - 1], 1.0f / S_ACT, im.cst + fc.wl);
+  add_const(pj, pp + sh.b_off[sh.L - 1], sh.out_dim, 1.0f, im.cst + fc.bl);
   for (int l = 0; l < sh.L; ++l) {
     char* dst = im.w_fwd + im.w_fwd_layer[l];
     if (im.n_chunks_fwd[l] == 0) continue;
