@@ -149,11 +149,15 @@ SIGNATURES = {
     "b200_conv_tma_chainable": (C.c_int, [C.POINTER(ConvDesc)]),
     "b200_conv2d_tma_chain": (C.c_int, [C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P, _P, C.POINTER(ConvDesc), _I32, _P,
                                         C.c_int64, _P]),
+    "b200_conv_tma_pack_chain": (C.c_int, [C.POINTER(ConvDesc), _P, _I32, _P, _I32, _P]),
+    "b200_convlstm_tma_weight_images": (C.c_int, [C.POINTER(ConvDesc), _P, _P, _P]),
+    "b200_convlstm_tma": (C.c_int, [C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P, _P, _P, C.c_int64, _P]),
     "b200_maxpool2": (C.c_int, [_P, _P, _I64, _I32, _I32, _P]),
     "b200_upsample_bilinear2": (C.c_int, [_P, _P, _I32, _I32, _I32, _I32, _I32, _I32, _P]),
     "b200_instance_norm": (C.c_int, [_P, _P, _I64, _I64, _F, _I32, _P]),
     "b200_add_relu": (C.c_int, [_P, _P, _P, _I64, _P]),
     "b200_gru_gate": (C.c_int, [_P, _P, _P, _P, _I64, _I64, _I64, _I32, _P]),
+    "b200_convlstm_cell": (C.c_int, [_P, _P, _P, _P, _I32, _I32, _I32, _I32, _P]),
     "b200_convlstm_zero_state": (C.c_int, [_P, _P, _P, _I32, _I32, _I32, _I32, _P]),
     "b200_convex_upsample": (C.c_int, [_P, _P, _P, _I32, _I32, _I32, _P]),
 }

@@ -29,11 +29,12 @@ def conv_precision():
     return _conv_precision
 
 
-def _images_for(d, w):
+def _images_for(d, w, lstm=False):
     """Packed weight images, cached per weight TENSOR OBJECT (not per address alone: a freed tensor's address is
     reused) and keyed on everything the image depends on: the storage (`w.data = t`, `module.to(...)`), the in-place
-    version, the stride and whether the x taps are folded into the channel vector (decided by the upsampling mode
-    for a given weight shape).  Pass module parameters themselves (conv.weight) to benefit from the cache.
+    version, the stride, whether the x taps are folded into the channel vector (decided by the upsampling mode
+    for a given weight shape) and the row layout (plain, or gate-interleaved for `convlstm` with lstm=True).
+    Pass module parameters themselves (conv.weight) to benefit from the cache.
     Writes through `w.data` (`w.data.copy_(t)`) bump no version and keep the storage, so they are not seen: call
     `clear_weight_images()` after them."""
     key = id(w)
@@ -44,13 +45,13 @@ def _images_for(d, w):
     nbytes = N.lib().b200_conv_tma_weight_image_bytes(C.byref(d))
     if nbytes <= 0:
         raise N.B200Error("conv weight image size: invalid descriptor: " + N.last_error())
-    sub = (w.data_ptr(), str(w.device), w._version, d.stride, d.upsample_mode)
+    sub = (w.data_ptr(), str(w.device), w._version, d.stride, d.upsample_mode, "lstm" if lstm else "plain")
     img = ent[1].get(sub)
     if img is None:
         ent[1].clear()
         img = torch.empty(nbytes, dtype=torch.uint8, device=w.device)
-        N.check(N.lib().b200_conv_tma_weight_images(C.byref(d), N.ptr(w), N.ptr(img), N.current_stream()),
-                "conv weight images")
+        build = N.lib().b200_convlstm_tma_weight_images if lstm else N.lib().b200_conv_tma_weight_images
+        N.check(build(C.byref(d), N.ptr(w), N.ptr(img), N.current_stream()), "conv weight images")
         ent[1][sub] = img
     assert img.numel() == nbytes, "cached weight image does not match the convolution's layout"
     return img
@@ -216,6 +217,85 @@ def convlstm_zero_state(gates, want_cell=True):
     cell = torch.empty_like(hidden) if want_cell else None
     N.check(N.lib().b200_convlstm_zero_state(N.ptr(gates), N.ptr(hidden), N.ptr(cell), n, c4 // 4, h, w,
                                              N.current_stream()), "b200_convlstm_zero_state")
+    return hidden, cell
+
+
+def _check_state(prev_state, shape, device):
+    """A ConvLSTM state: (hidden, cell), both contiguous fp32 CUDA tensors of `shape` on `device`."""
+    if not isinstance(prev_state, (tuple, list)) or len(prev_state) != 2:
+        raise N.B200Error("prev_state must be a (hidden, cell) pair")
+    for name, t in zip(("hidden", "cell"), prev_state):
+        if not isinstance(t, torch.Tensor):
+            raise N.B200Error(f"prev_state {name} is not a tensor")
+        _check(t)
+        if tuple(t.shape) != tuple(shape):
+            raise N.B200Error(f"prev_state {name} has shape {tuple(t.shape)}, expected {tuple(shape)}")
+        if t.device != torch.device(device):
+            raise N.B200Error(f"prev_state {name} is on {t.device}, the input on {device}")
+    return prev_state
+
+
+def convlstm_cell(gates, prev_cell=None, want_cell=True):
+    """ConvLSTM cell on fp32 gates (N, 4C, H, W), pre-activation in chunk(4, 1) order -> (hidden, cell); prev_cell
+    None is the zero state (what convlstm_zero_state computes)."""
+    _check(gates)
+    n, c4, h, w = gates.shape
+    if prev_cell is not None:
+        _check(prev_cell)
+        if tuple(prev_cell.shape) != (n, c4 // 4, h, w) or prev_cell.device != gates.device:
+            raise N.B200Error("prev_cell does not match the gates")
+    hidden = torch.empty(n, c4 // 4, h, w, dtype=torch.float32, device=gates.device)
+    cell = torch.empty_like(hidden) if want_cell else None
+    N.check(N.lib().b200_convlstm_cell(N.ptr(gates), N.ptr(prev_cell), N.ptr(hidden), N.ptr(cell), n, c4 // 4, h, w,
+                                       N.current_stream()), "b200_convlstm_cell")
+    return hidden, cell
+
+
+def convlstm(x, weight, bias, prev_state=None, want_cell=True):
+    """ConvLSTM step on the tensor cores (nn.Conv2d gates with 'same' zero padding, then the cell update fused into
+    the gate convolution's epilogue; the 4C gate channels are never stored) -> fresh (hidden, cell) tensors, cell None
+    with want_cell=False.  `weight` (4C, Cin, KH, KW) and `bias` (4C) are the reference's Gates parameters unchanged.
+    prev_state None: the zero state, `weight` holds only the input half (Cin = channels of x).  With a state
+    (hidden, cell), each (N, C, H, W): `weight` is the full (4C, 2C, KH, KW) tensor and `x` is either a tensor of C
+    channels or a `Chain` of 2C channels whose first C its producers wrote; the previous hidden state fills the rest."""
+    _check(weight); _check(bias)
+    c4, cin, kh, kw = weight.shape
+    if c4 % 32:
+        raise N.B200Error(f"ConvLSTM gates: {c4} output channels are not 4 * C with C a multiple of 8")
+    c = c4 // 4
+    packed_in = isinstance(x, Chain)
+    if packed_in:
+        n, cx, h, wd, dev = x.n, x.cin, x.h, x.w, x.buf.device
+        if x.pad_mode != "zeros" or (x.desc.KH, x.desc.KW, x.desc.pad_h, x.desc.pad_w) != (kh, kw, kh // 2, kw // 2):
+            raise N.B200Error("the chained input was packed for another filter geometry")
+    else:
+        _check(x)
+        n, cx, h, wd = x.shape
+        dev = x.device
+    if prev_state is not None:
+        _check_state(prev_state, (n, c, h, wd), dev)
+        if cin != 2 * c or cx != (2 * c if packed_in else c):
+            raise N.B200Error(f"ConvLSTM with a state: weight of {cin} input channels, input of {cx}, hidden of {c}")
+        if packed_in:
+            N.check(N.lib().b200_conv_tma_pack_chain(C.byref(x.desc), N.ptr(prev_state[0]), c, N.ptr(x.buf), c,
+                                                     N.current_stream()), "b200_conv_tma_pack_chain")
+        else:
+            x, cx = torch.cat((x, prev_state[0]), 1), 2 * c
+    elif cin != cx:
+        raise N.B200Error(f"weight expects {cin} input channels, got {cx}")
+    d = N.ConvDesc(n, cx, h, wd, cx, 0, c4, kh, kw, 1, kh // 2, kw // 2, 0, 1, c4, 0, 0, 1.0, 0, 0, 0)
+    ws, nbytes = None, 0
+    if not packed_in:
+        nbytes = N.lib().b200_conv_tma_workspace_bytes(C.byref(d))
+        if nbytes <= 0:
+            raise N.B200Error("b200_conv_tma_workspace_bytes: " + N.last_error())
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    hidden = torch.empty(n, c, h, wd, dtype=torch.float32, device=dev)
+    cell = torch.empty_like(hidden) if want_cell else None
+    N.check(N.lib().b200_convlstm_tma(
+        C.byref(d), None if packed_in else N.ptr(x), N.ptr(x.buf) if packed_in else None,
+        N.ptr(_images_for(d, weight, lstm=True)), N.ptr(bias), N.ptr(prev_state[1]) if prev_state is not None else None,
+        N.ptr(hidden), N.ptr(cell), N.ptr(ws), nbytes, N.current_stream()), "b200_convlstm_tma")
     return hidden, cell
 
 

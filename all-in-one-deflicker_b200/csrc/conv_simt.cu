@@ -195,10 +195,13 @@ __global__ void gru_gate_kernel(const float* __restrict__ a, const float* __rest
   out[n * out_stride + k] = v;
 }
 
-// ConvLSTM with zero previous state (network_local.py:25-53, prev_state=None):
-// gates [N][4C][H][W] (pre-activation) -> hidden = sigmoid(o) * tanh(sigmoid(i) * tanh(g)), cell
-__global__ void convlstm_zero_state_kernel(const float* __restrict__ gates, float* __restrict__ hidden,
-                                           float* __restrict__ cell, int C, int64_t plane, int64_t total) {
+// ConvLSTM cell (network_local.py:18-53): gates [N][4C][H][W] (pre-activation, chunk(4, 1) order in, remember, out,
+// cell) -> cell = sigmoid(r) * prev_cell + sigmoid(i) * tanh(g), hidden = sigmoid(o) * tanh(cell).
+// prev_cell == nullptr is prev_state=None: cell = sigmoid(i) * tanh(g).  The same expressions as the fused epilogue of
+// convlstm_tma_kernel (conv_tma.cu).
+__global__ void convlstm_cell_kernel(const float* __restrict__ gates, const float* __restrict__ prev_cell,
+                                     float* __restrict__ hidden, float* __restrict__ cell, int C, int64_t plane,
+                                     int64_t total) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total) return;
   const int64_t sp = i % plane, c = (i / plane) % C, n = i / (plane * C);
@@ -206,7 +209,13 @@ __global__ void convlstm_zero_state_kernel(const float* __restrict__ gates, floa
   const float in_g = 1.f / (1.f + expf(-g[(c)*plane + sp]));
   const float out_g = 1.f / (1.f + expf(-g[(2 * C + c) * plane + sp]));
   const float cell_g = tanhf(g[(3 * C + c) * plane + sp]);
-  const float cl = in_g * cell_g;                   // remember_gate * 0 + in_gate * cell_gate
+  float cl;
+  if (prev_cell) {                                  // torch: (remember * prev) + (in * cell_gate), each rounded
+    const float rem_g = 1.f / (1.f + expf(-g[(C + c) * plane + sp]));
+    cl = __fadd_rn(__fmul_rn(rem_g, prev_cell[i]), __fmul_rn(in_g, cell_g));
+  } else {
+    cl = in_g * cell_g;                             // remember_gate * 0 + in_gate * cell_gate
+  }
   hidden[i] = out_g * tanhf(cl);
   if (cell) cell[i] = cl;
 }
@@ -367,14 +376,19 @@ int b200_gru_gate(const float* a, const float* b, const float* c, float* out, in
   return B200_OK;
 }
 
-int b200_convlstm_zero_state(const float* gates, float* hidden, float* cell, int32_t N, int32_t C, int32_t H, int32_t W,
-                             void* stream) {
+int b200_convlstm_cell(const float* gates, const float* prev_cell, float* hidden, float* cell, int32_t N, int32_t C,
+                       int32_t H, int32_t W, void* stream) {
   B200_REQUIRE(gates && hidden && N > 0 && C > 0 && H > 0 && W > 0, "bad arguments");
   const int64_t plane = (int64_t)H * W, total = (int64_t)N * C * plane;
-  convlstm_zero_state_kernel<<<(unsigned)((total + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      gates, hidden, cell, C, plane, total);
+  convlstm_cell_kernel<<<(unsigned)((total + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      gates, prev_cell, hidden, cell, C, plane, total);
   B200_CHECK_LAUNCH();
   return B200_OK;
+}
+
+int b200_convlstm_zero_state(const float* gates, float* hidden, float* cell, int32_t N, int32_t C, int32_t H, int32_t W,
+                             void* stream) {
+  return b200_convlstm_cell(gates, nullptr, hidden, cell, N, C, H, W, stream);
 }
 
 int b200_convex_upsample(const float* flow, const float* mask, float* out, int32_t N, int32_t H, int32_t W, void* stream) {

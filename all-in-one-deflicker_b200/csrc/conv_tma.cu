@@ -14,6 +14,8 @@
 //   conv2d_tma_kernel       persistent, warps 0-7 = two consumer warpgroups (wgmma on 64 pixels each, then the
 //                           epilogue: bias, activation, scale, residual, NCHW fp32 / packed fp16 stores),
 //                           warp 8 = TMA producer (1 activation box + 1 weight image per stage)
+// and convlstm_tma_kernel, the same pipeline for a ConvLSTM gate convolution whose epilogue applies the cell update
+// (gate-interleaved weight image, see LstmArgs) instead of storing the gates.
 //
 // Same operator semantics as b200_conv2d (reference: nn.Conv2d / ReflectionPad2d / nn.Upsample call sites in
 // src/models/stage_1/core/update.py, src/models/network_filter.py, src/models/network_local.py).
@@ -44,6 +46,15 @@ struct ConvTmaArgs {
   __half* yp; int yp_hp2, yp_wp2, yp_cp, yp_pad_h, yp_pad_w, yp_c_off;
 };
 
+// ConvLSTM epilogue (convlstm_tma_kernel): the gate convolution's Cout = 4C columns come from a gate-interleaved weight
+// image (column 32b + 8k + r of an N tile = gate k of hidden channel 8b + r of that tile, gates in chunk(4, 1) order:
+// in, remember, out, cell), so every thread holds the four gates of its hidden channels.  NCHW fp32 [N][C][OH][OW].
+struct LstmArgs {
+  const float* prev_cell;                              // nullptr: zero state
+  float* hidden; float* cell;                          // cell may be nullptr
+  int C;
+};
+
 __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, int c0, int c1, int c2, int c3,
                                             uint64_t* bar) {
   asm volatile(
@@ -61,12 +72,14 @@ __device__ __forceinline__ float tm_act(float v) {
   return v;
 }
 
+__device__ __forceinline__ float tm_sigmoid(float v) { return 1.0f / (1.0f + expf(-v)); }
+
 // Consumer warpgroups for one N-tile width: the MMAs of a tile (this warpgroup's 64 pixels), then the epilogue on the
 // accumulator registers (bias, activation, scale, residual; NCHW fp32 stores and / or the fp16 channel pairs of the
-// next layer's packed input)
-template <int NT, int ACT>
-__device__ __forceinline__ void tma_consume(const ConvTmaArgs& a, char* sA, char* sB, uint64_t* a_full, uint64_t* a_empty,
-                                            uint64_t* b_full, uint64_t* b_empty) {
+// next layer's packed input), or with LSTM the ConvLSTM cell update (hidden / cell stores; the gates are never stored)
+template <int NT, int ACT, bool LSTM>
+__device__ __forceinline__ void tma_consume(const ConvTmaArgs& a, const LstmArgs& l, char* sA, char* sB, uint64_t* a_full,
+                                            uint64_t* a_empty, uint64_t* b_full, uint64_t* b_empty) {
   const B200ConvDesc& d = a.d;
   const int warp = warp_uniform(), lane = threadIdx.x & 31, g = warp >> 2, q = lane & 3;
   const int m0 = 64 * g + 16 * (warp & 3) + (lane >> 2);
@@ -133,6 +146,43 @@ __device__ __forceinline__ void tma_consume(const ConvTmaArgs& a, char* sA, char
     int r = t / a.n_tiles_n;
     const int xb = r % a.x_tiles; r /= a.x_tiles;
     const int oy = r % a.OH, n = r / a.OH;
+    if constexpr (LSTM) {
+      // accumulator column 8i + 2q + e with i = 4b + k: gate k of hidden channel h0 + 8b + 2q + e (C % 8 == 0, so a
+      // channel pair lies inside [0, C) or outside it together)
+      const int C = l.C, h0 = nt * (NT / 4);
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int x = xb * 128 + m0 + 8 * rr;
+        if (x >= a.OW) continue;
+        const int64_t pix = (int64_t)n * C * oplane + (int64_t)oy * a.OW + x;
+#pragma unroll
+        for (int b = 0; b < NT / 32; ++b) {
+          const int hc = h0 + 8 * b + 2 * q;
+          if (hc >= C) continue;
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int h = hc + e;
+            float gv[4];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              gv[k] = acc[4 * (4 * b + k) + 2 * rr + e];
+              if (a.bias) gv[k] += __ldg(a.bias + k * C + h);
+            }
+            // the expressions of convlstm_cell_kernel (conv_simt.cu), so both paths agree on the same gates
+            const float in_g = tm_sigmoid(gv[0]), out_g = tm_sigmoid(gv[2]), cell_g = tanhf(gv[3]);
+            const int64_t o = pix + (int64_t)h * oplane;
+            float cl;
+            if (l.prev_cell)                                // torch: (remember * prev) + (in * cell_gate), each rounded
+              cl = __fadd_rn(__fmul_rn(tm_sigmoid(gv[1]), __ldg(l.prev_cell + o)), __fmul_rn(in_g, cell_g));
+            else
+              cl = in_g * cell_g;
+            l.hidden[o] = out_g * tanhf(cl);
+            if (l.cell) l.cell[o] = cl;
+          }
+        }
+      }
+      continue;
+    }
 #pragma unroll
     for (int rr = 0; rr < 2; ++rr) {
       const int x = xb * 128 + m0 + 8 * rr;
@@ -164,24 +214,29 @@ __device__ __forceinline__ void tma_consume(const ConvTmaArgs& a, char* sA, char
   }
 }
 
-template <int NT>
-__device__ __forceinline__ void tma_consume_act(const ConvTmaArgs& a, char* sA, char* sB, uint64_t* a_full,
-                                                uint64_t* a_empty, uint64_t* b_full, uint64_t* b_empty) {
+template <int NT, bool LSTM>
+__device__ __forceinline__ void tma_consume_act(const ConvTmaArgs& a, const LstmArgs& l, char* sA, char* sB,
+                                                uint64_t* a_full, uint64_t* a_empty, uint64_t* b_full,
+                                                uint64_t* b_empty) {
+  if constexpr (LSTM) {                                  // no activation, scale or residual in front of the cell
+    tma_consume<NT, 0, true>(a, l, sA, sB, a_full, a_empty, b_full, b_empty);
+    return;
+  }
   switch (a.d.act) {
-    case 1: tma_consume<NT, 1>(a, sA, sB, a_full, a_empty, b_full, b_empty); break;
-    case 2: tma_consume<NT, 2>(a, sA, sB, a_full, a_empty, b_full, b_empty); break;
-    case 3: tma_consume<NT, 3>(a, sA, sB, a_full, a_empty, b_full, b_empty); break;
-    case 4: tma_consume<NT, 4>(a, sA, sB, a_full, a_empty, b_full, b_empty); break;
-    default: tma_consume<NT, 0>(a, sA, sB, a_full, a_empty, b_full, b_empty); break;
+    case 1: tma_consume<NT, 1, false>(a, l, sA, sB, a_full, a_empty, b_full, b_empty); break;
+    case 2: tma_consume<NT, 2, false>(a, l, sA, sB, a_full, a_empty, b_full, b_empty); break;
+    case 3: tma_consume<NT, 3, false>(a, l, sA, sB, a_full, a_empty, b_full, b_empty); break;
+    case 4: tma_consume<NT, 4, false>(a, l, sA, sB, a_full, a_empty, b_full, b_empty); break;
+    default: tma_consume<NT, 0, false>(a, l, sA, sB, a_full, a_empty, b_full, b_empty); break;
   }
 }
 
 // Reduction order shared by the producer, the consumers and the weight images:
 //   for ky, for xpar in [0, stride), for cc (64-channel block):   one activation box (all x shifts of that row)
 //     for kx = xpar, xpar + stride, ... < KW:                      one weight chunk, A start shifted by kx>>shift rows
-__global__ void __launch_bounds__(TM_THREADS, 1) conv2d_tma_kernel(const __grid_constant__ ConvTmaArgs a,
-                                                                   const __grid_constant__ CUtensorMap xmap,
-                                                                   const __grid_constant__ CUtensorMap xmap_lo) {
+template <bool LSTM>
+__device__ __forceinline__ void conv_tma_body(const ConvTmaArgs& a, const CUtensorMap& xmap, const CUtensorMap& xmap_lo,
+                                              const LstmArgs& l) {
   extern __shared__ __align__(1024) char smem[];
   const int b_half = a.n_tile * 128;                    // one term of one weight chunk
   const int b_bytes = a.split ? 2 * b_half : b_half;
@@ -205,9 +260,9 @@ __global__ void __launch_bounds__(TM_THREADS, 1) conv2d_tma_kernel(const __grid_
 
   if (warp < TM_CONSUMER_WARPS) {
     setmaxnreg_inc<232>();                               // 128 * 40 + 256 * 232 <= 64 K
-    if (a.n_tile == 256) tma_consume_act<256>(a, sA, sB, a_full, a_empty, b_full, b_empty);
-    else if (a.n_tile == 128) tma_consume_act<128>(a, sA, sB, a_full, a_empty, b_full, b_empty);
-    else tma_consume_act<64>(a, sA, sB, a_full, a_empty, b_full, b_empty);
+    if (a.n_tile == 256) tma_consume_act<256, LSTM>(a, l, sA, sB, a_full, a_empty, b_full, b_empty);
+    else if (a.n_tile == 128) tma_consume_act<128, LSTM>(a, l, sA, sB, a_full, a_empty, b_full, b_empty);
+    else tma_consume_act<64, LSTM>(a, l, sA, sB, a_full, a_empty, b_full, b_empty);
     return;
   }
   setmaxnreg_dec<40>();
@@ -251,6 +306,20 @@ __global__ void __launch_bounds__(TM_THREADS, 1) conv2d_tma_kernel(const __grid_
   }
 }
 
+__global__ void __launch_bounds__(TM_THREADS, 1) conv2d_tma_kernel(const __grid_constant__ ConvTmaArgs a,
+                                                                   const __grid_constant__ CUtensorMap xmap,
+                                                                   const __grid_constant__ CUtensorMap xmap_lo) {
+  conv_tma_body<false>(a, xmap, xmap_lo, LstmArgs{});
+}
+
+// the ConvLSTM gate convolution with the cell update in its epilogue (gate-interleaved weight image, see LstmArgs)
+__global__ void __launch_bounds__(TM_THREADS, 1) convlstm_tma_kernel(const __grid_constant__ ConvTmaArgs a,
+                                                                     const __grid_constant__ CUtensorMap xmap,
+                                                                     const __grid_constant__ CUtensorMap xmap_lo,
+                                                                     const __grid_constant__ LstmArgs l) {
+  conv_tma_body<true>(a, xmap, xmap_lo, l);
+}
+
 __device__ __forceinline__ int tm_reflect(int i, int n) {
   if (i < 0) i = -i;
   if (i >= n) i = 2 * (n - 1) - i;
@@ -259,11 +328,14 @@ __device__ __forceinline__ int tm_reflect(int i, int n) {
 
 // fp32 NCHW slice -> fp16 [N*phases][HP2][WP2][Cp] (Cp = channels padded to 64) with padding / upsampling /
 // phase split applied.  One block = 32 pixels of one row x 64 channels, transposed through shared memory.
+// Channels [0, c_write) of the slice land at channel c_off of each packed pixel (a whole repack: c_off = 0, c_write =
+// Cp, the padding channels written as zeros; a slice into a shared packed input: c_write = Cin, c_off % 8 == 0).
 __global__ void __launch_bounds__(256) conv_pack_input_kernel(const float* __restrict__ x, __half* __restrict__ xp,
                                                               B200ConvDesc d, int HP2, int WP2, int Cp, int phases,
-                                                              float scale, int64_t lo_off, int fold_cf) {
+                                                              float scale, int64_t lo_off, int fold_cf, int c_off,
+                                                              int c_write) {
   __shared__ float tile[64][33];
-  const int cblocks = Cp / 64;
+  const int cblocks = (c_write + 63) / 64;
   const int cb = blockIdx.z % cblocks, nph = blockIdx.z / cblocks;
   const int ph = nph % phases, n = nph / phases;
   const int yy = blockIdx.y, bx = blockIdx.x * 32;
@@ -328,14 +400,14 @@ __global__ void __launch_bounds__(256) conv_pack_input_kernel(const float* __res
   }
   __syncthreads();
   const int px = threadIdx.x >> 3, c8 = threadIdx.x & 7;
-  if (bx + px < WP2) {
+  if (bx + px < WP2 && cb * 64 + c8 * 8 < c_write) {
     float v[8];
 #pragma unroll
     for (int q = 0; q < 8; ++q) v[q] = tile[c8 * 8 + q][px] * scale;
     uint4 hi, lo;
     split2_f16(v[0], v[1], hi.x, lo.x); split2_f16(v[2], v[3], hi.y, lo.y);
     split2_f16(v[4], v[5], hi.z, lo.z); split2_f16(v[6], v[7], hi.w, lo.w);
-    const int64_t o = (((int64_t)nph * HP2 + yy) * WP2 + bx + px) * Cp + cb * 64 + c8 * 8;
+    const int64_t o = (((int64_t)nph * HP2 + yy) * WP2 + bx + px) * Cp + c_off + cb * 64 + c8 * 8;
     *reinterpret_cast<uint4*>(xp + o) = hi;
     if (lo_off) *reinterpret_cast<uint4*>(xp + lo_off + o) = lo;
   }
@@ -371,16 +443,23 @@ __global__ void conv_reflect_halo_kernel(__half* __restrict__ xp, int N, int H, 
 
 // weights [Cout][Cin][KH][KW] fp32 -> per cout tile, per (tap, channel block): [n_tile rows x 64 channels] fp16,
 // K-major, 128-byte swizzle, zero padded
-// (w_co, w_ci, w_tap = element strides of the weight tensor; split: chunk = [hi rows | lo rows], values pre-scaled)
+// (w_co, w_ci, w_tap = element strides of the weight tensor; split: chunk = [hi rows | lo rows], values pre-scaled;
+// lstm_c > 0: gate-interleaved rows for convlstm_tma_kernel, Cout = 4 * lstm_c: row 32b + 8k + r of cout tile nt holds
+// weight row k * lstm_c + nt * n_tile / 4 + 8b + r, i.e. gate k of that hidden channel)
 __global__ void conv_tma_weight_images_kernel(const float* __restrict__ w, char* __restrict__ img, int Cout, int Cin,
                                               int KH, int KW, int stride, int n_tile, int n_tiles_n, int cchunks,
                                               int64_t w_co, int64_t w_ci, int64_t w_tap, float scale, int split,
-                                              int fold_cf) {
+                                              int fold_cf, int lstm_c) {
   const int KHW = KH * KW, n_chunks = fold_cf ? KH : KHW * cchunks;
   const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;      // one 16-byte chunk each
   if (e >= (int64_t)n_tiles_n * n_tile * n_chunks * 8) return;
   const int c8 = (int)(e % 8), j = (int)((e / 8) % n_chunks), grow = (int)(e / (8 * n_chunks));
-  const int nt = grow / n_tile, lrow = grow % n_tile, row = nt * n_tile + lrow;
+  const int nt = grow / n_tile, lrow = grow % n_tile;
+  int row = nt * n_tile + lrow;
+  if (lstm_c) {
+    const int hc = nt * (n_tile >> 2) + (lrow >> 5) * 8 + (lrow & 7);
+    row = hc < lstm_c ? ((lrow >> 3) & 3) * lstm_c + hc : Cout;        // Cout: a zero row
+  }
   // chunk j -> (ky, xpar, cc, kx) in the kernel's reduction order
   int tap = 0, cc = 0;
   if (!fold_cf) {
@@ -473,11 +552,11 @@ static EncodeTiledFn encode_tiled() {
 }
 
 static int launch_weight_images(const B200ConvDesc* d, const TmaGeom& g, const float* w, int64_t w_co, int64_t w_ci,
-                                int64_t w_tap, float scale, int split, void* images, cudaStream_t st) {
+                                int64_t w_tap, float scale, int split, void* images, cudaStream_t st, int lstm_c = 0) {
   const int64_t total = (int64_t)g.n_tiles_n * g.n_tile * g.n_chunks * 8;
   conv_tma_weight_images_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(
       w, reinterpret_cast<char*>(images), d->Cout, d->Cin, d->KH, d->KW, d->stride, g.n_tile, g.n_tiles_n, g.cchunks, w_co,
-      w_ci, w_tap, scale, split, g.fold_cf);
+      w_ci, w_tap, scale, split, g.fold_cf, lstm_c);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
@@ -486,13 +565,15 @@ static int launch_weight_images(const B200ConvDesc* d, const TmaGeom& g, const f
 struct ChainOut { __half* yp = nullptr; int hp2 = 0, wp2 = 0, cp = 0, pad_h = 0, pad_w = 0, c_off = 0; };
 
 // x == nullptr: `base` already holds the packed input (written by the producing convolution's epilogue)
+// lstm != nullptr: the ConvLSTM gate layer (convlstm_tma_kernel; y, residual and chain unused)
 static int launch_conv_tma(const B200ConvDesc* d, const TmaGeom& g, const float* x, char* base, const void* w_images,
                            const float* bias, const float* residual, float* y, int split, float in_scale, cudaStream_t st,
-                           const ChainOut* chain = nullptr) {
+                           const ChainOut* chain = nullptr, const LstmArgs* lstm = nullptr) {
   B200_REQUIRE(g.HP2 <= 65535 && (int64_t)d->N * g.phases * g.cchunks <= 65535, "input too large for the repack grid");
   if (x) {
     conv_pack_input_kernel<<<dim3((g.WP2 + 31) / 32, g.HP2, d->N * g.phases * g.cchunks), 256, 0, st>>>(
-        x, reinterpret_cast<__half*>(base), *d, g.HP2, g.WP2, g.Cp, g.phases, in_scale, split ? g.pack_bytes / 2 : 0, g.fold_cf);
+        x, reinterpret_cast<__half*>(base), *d, g.HP2, g.WP2, g.Cp, g.phases, in_scale, split ? g.pack_bytes / 2 : 0, g.fold_cf,
+        0, g.Cp);
     B200_CHECK_LAUNCH();
   }
 
@@ -513,10 +594,11 @@ static int launch_conv_tma(const B200ConvDesc* d, const TmaGeom& g, const float*
   }
   if (!split) map_lo = map;
 
-  static bool attr_done = false;
-  if (!attr_done) {
-    B200_CHECK_CUDA(cudaFuncSetAttribute(conv2d_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TM_SMEM_BUDGET));
-    attr_done = true;
+  static bool attr_done = false, attr_lstm_done = false;
+  if (!(lstm ? attr_lstm_done : attr_done)) {
+    B200_CHECK_CUDA(cudaFuncSetAttribute(lstm ? (const void*)convlstm_tma_kernel : (const void*)conv2d_tma_kernel,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, TM_SMEM_BUDGET));
+    (lstm ? attr_lstm_done : attr_done) = true;
   }
   ConvTmaArgs a{};
   a.d = *d; a.w_img = reinterpret_cast<const char*>(w_images); a.bias = bias; a.res = residual; a.y = y;
@@ -560,7 +642,9 @@ static int launch_conv_tma(const B200ConvDesc* d, const TmaGeom& g, const float*
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  conv2d_tma_kernel<<<(unsigned)(tiles < sms ? tiles : sms), TM_THREADS, smem_bytes, st>>>(a, map, map_lo);
+  const unsigned grid = (unsigned)(tiles < sms ? tiles : sms);
+  if (lstm) convlstm_tma_kernel<<<grid, TM_THREADS, smem_bytes, st>>>(a, map, map_lo, *lstm);
+  else conv2d_tma_kernel<<<grid, TM_THREADS, smem_bytes, st>>>(a, map, map_lo);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
@@ -602,6 +686,31 @@ int b200_conv_tma_chainable(const B200ConvDesc* next) {
           next->in_c_total == next->Cin) ? 1 : 0;
 }
 
+// where the packed input of `d` lives: the caller's pre-packed buffer, or the (aligned) workspace the repack fills;
+// a pre-packed input with reflection padding gets its halo mirrored here
+static int tma_input_base(const B200ConvDesc* d, const TmaGeom& g, void* in_packed, void* workspace, int64_t workspace_bytes,
+                          const char* who, cudaStream_t st, char** base) {
+  if (in_packed) {
+    B200_REQUIRE(b200_conv_tma_chainable(d), "this convolution cannot take a pre-packed input");
+    B200_REQUIRE((reinterpret_cast<uintptr_t>(in_packed) & 255) == 0, "packed input must be 256-byte aligned");
+    *base = reinterpret_cast<char*>(in_packed);
+    if (d->pad_mode == 1 && (d->pad_h > 0 || d->pad_w > 0)) {
+      const int64_t threads = (int64_t)d->N * ((int64_t)g.HP2 * g.WP2 - (int64_t)d->H * d->W) * (g.Cp / 8);
+      conv_reflect_halo_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(
+          reinterpret_cast<__half*>(*base), d->N, d->H, d->W, d->pad_h, d->pad_w, g.Cp);
+      B200_CHECK_LAUNCH();
+    }
+    return B200_OK;
+  }
+  B200_REQUIRE(workspace, "null workspace");
+  *base = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
+  if (*base + g.pack_bytes > reinterpret_cast<char*>(workspace) + workspace_bytes) {
+    set_error("%s: workspace too small (%lld < %lld)", who, (long long)workspace_bytes, (long long)(g.pack_bytes + 256));
+    return B200_ERR_WORKSPACE;
+  }
+  return B200_OK;
+}
+
 int b200_conv2d_tma_chain(const B200ConvDesc* d, const float* x, void* in_packed, const void* w_images, const float* bias,
                           const float* residual, float* y, void* out_packed, const B200ConvDesc* next, int32_t next_c_off,
                           void* workspace, int64_t workspace_bytes, void* stream) {
@@ -612,19 +721,6 @@ int b200_conv2d_tma_chain(const B200ConvDesc* d, const float* x, void* in_packed
                d->out_c_off + d->Cout <= d->out_c_total, "channel slice out of range");
   if (residual) B200_REQUIRE(d->res_c_off >= 0 && d->res_c_off + d->Cout <= d->res_c_total, "residual slice out of range");
   if (!b200_device_supports_tc()) { set_error("b200_conv2d_tma_chain needs a compute-capability 9.x device"); return B200_ERR_UNSUPPORTED; }
-  char* base = nullptr;
-  if (in_packed) {
-    B200_REQUIRE(b200_conv_tma_chainable(d), "this convolution cannot take a pre-packed input");
-    B200_REQUIRE((reinterpret_cast<uintptr_t>(in_packed) & 255) == 0, "packed input must be 256-byte aligned");
-    base = reinterpret_cast<char*>(in_packed);
-  } else {
-    B200_REQUIRE(workspace, "null workspace");
-    base = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
-    if (base + g.pack_bytes > reinterpret_cast<char*>(workspace) + workspace_bytes) {
-      set_error("b200_conv2d_tma_chain: workspace too small (%lld < %lld)", (long long)workspace_bytes, (long long)(g.pack_bytes + 256));
-      return B200_ERR_WORKSPACE;
-    }
-  }
   ChainOut co;
   if (out_packed) {
     B200_REQUIRE(next && b200_conv_tma_chainable(next), "the consumer convolution cannot take a pre-packed input");
@@ -637,14 +733,64 @@ int b200_conv2d_tma_chain(const B200ConvDesc* d, const float* x, void* in_packed
     co.yp = reinterpret_cast<__half*>(out_packed); co.hp2 = gn.HP2; co.wp2 = gn.WP2; co.cp = gn.Cp;
     co.pad_h = next->pad_h; co.pad_w = next->pad_w; co.c_off = next_c_off;
   }
-  if (in_packed && d->pad_mode == 1 && (d->pad_h > 0 || d->pad_w > 0)) {
-    const int64_t threads = (int64_t)d->N * ((int64_t)g.HP2 * g.WP2 - (int64_t)d->H * d->W) * (g.Cp / 8);
-    conv_reflect_halo_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-        reinterpret_cast<__half*>(base), d->N, d->H, d->W, d->pad_h, d->pad_w, g.Cp);
-    B200_CHECK_LAUNCH();
-  }
-  return launch_conv_tma(d, g, in_packed ? nullptr : x, base, w_images, bias, residual, y, 0, 1.0f,
-                         reinterpret_cast<cudaStream_t>(stream), &co);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  char* base = nullptr;
+  if (int rc = tma_input_base(d, g, in_packed, workspace, workspace_bytes, "b200_conv2d_tma_chain", st, &base)) return rc;
+  return launch_conv_tma(d, g, in_packed ? nullptr : x, base, w_images, bias, residual, y, 0, 1.0f, st, &co);
+}
+
+int b200_conv_tma_pack_chain(const B200ConvDesc* next, const float* x, int32_t C, void* out_packed, int32_t next_c_off,
+                             void* stream) {
+  B200_REQUIRE(next && x && out_packed, "null pointer");
+  B200_REQUIRE(b200_conv_tma_chainable(next), "the consumer convolution cannot take a pre-packed input");
+  TmaGeom g;
+  if (int rc = tma_geometry(next, &g)) return rc;
+  B200_REQUIRE(C > 0 && next_c_off >= 0 && next_c_off + C <= next->Cin && (next_c_off & 7) == 0 && (C & 7) == 0,
+               "packed channel slice must lie inside the consumer's input and be a multiple of 8 channels");
+  B200_REQUIRE((reinterpret_cast<uintptr_t>(out_packed) & 255) == 0, "packed output must be 256-byte aligned");
+  B200_REQUIRE(g.HP2 <= 65535 && (int64_t)next->N * ((C + 63) / 64) <= 65535, "input too large for the repack grid");
+  B200ConvDesc s = *next;                                 // the source tensor: C channels at the consumer's input extent
+  s.Cin = C; s.in_c_total = C; s.in_c_off = 0;
+  conv_pack_input_kernel<<<dim3((g.WP2 + 31) / 32, g.HP2, next->N * ((C + 63) / 64)), 256, 0,
+                           reinterpret_cast<cudaStream_t>(stream)>>>(x, reinterpret_cast<__half*>(out_packed), s, g.HP2, g.WP2,
+                                                                      g.Cp, 1, 1.0f, 0, 0, next_c_off, C);
+  B200_CHECK_LAUNCH();
+  return B200_OK;
+}
+
+// the gate convolution of a ConvLSTM: Cout = 4C (C % 8 == 0), stride 1, no upsampling / activation / scale / residual,
+// the whole output (no slice)
+static int lstm_geometry(const B200ConvDesc* d, TmaGeom* g) {
+  if (int rc = tma_geometry(d, g)) return rc;
+  B200_REQUIRE(d->Cout % 32 == 0, "ConvLSTM gates: Cout must be 4 * C with C a multiple of 8");
+  B200_REQUIRE(d->stride == 1 && d->upsample == 1 && d->act == B200_ACT_NONE && d->out_scale == 1.0f &&
+               d->out_c_off == 0 && d->out_c_total == d->Cout && d->res_c_total == 0 && d->res_c_off == 0,
+               "ConvLSTM gates: stride 1, no upsampling, activation, output scale, output slice or residual");
+  return B200_OK;
+}
+
+int b200_convlstm_tma_weight_images(const B200ConvDesc* d, const float* w, void* images, void* stream) {
+  B200_REQUIRE(w && images, "null pointer");
+  TmaGeom g;
+  if (int rc = lstm_geometry(d, &g)) return rc;
+  const int KHW = d->KH * d->KW;
+  return launch_weight_images(d, g, w, (int64_t)d->Cin * KHW, KHW, 1, 1.0f, 0, images, reinterpret_cast<cudaStream_t>(stream),
+                              d->Cout / 4);
+}
+
+int b200_convlstm_tma(const B200ConvDesc* d, const float* x, void* in_packed, const void* w_images, const float* bias,
+                      const float* prev_cell, float* hidden, float* cell, void* workspace, int64_t workspace_bytes,
+                      void* stream) {
+  B200_REQUIRE(d && w_images && (x || in_packed) && hidden, "null pointer");
+  TmaGeom g;
+  if (int rc = lstm_geometry(d, &g)) return rc;
+  B200_REQUIRE(d->in_c_off >= 0 && d->in_c_off + d->Cin <= d->in_c_total, "channel slice out of range");
+  if (!b200_device_supports_tc()) { set_error("b200_convlstm_tma needs a compute-capability 9.x device"); return B200_ERR_UNSUPPORTED; }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  char* base = nullptr;
+  if (int rc = tma_input_base(d, g, in_packed, workspace, workspace_bytes, "b200_convlstm_tma", st, &base)) return rc;
+  const LstmArgs l{prev_cell, hidden, cell, d->Cout / 4};
+  return launch_conv_tma(d, g, in_packed ? nullptr : x, base, w_images, bias, nullptr, nullptr, 0, 1.0f, st, nullptr, &l);
 }
 
 /* ---- all-pairs correlation (RAFT CorrBlock level 0, src/models/stage_1/core/corr.py:56-64) as a 1x1 "convolution":

@@ -1,6 +1,9 @@
-"""`TransformNet` local refinement (Lai et al.) with the reference's constructor and state_dict keys
-(src/models/network_local.py:7-188).  Reflection padding, nearest upsampling, LeakyReLU, the residual
-adds and the ConvLSTM cell are fused into b200_conv2d / b200_convlstm_zero_state.  As in the reference
+"""`TransformNet` local refinement (Lai et al.) with the reference's constructor, state_dict keys and call
+signature (src/models/network_local.py:7-188): `forward(X, prev_state)` returns `(Y, (hidden, cell))`, and the
+returned state (fresh tensors) can be passed back as the next frame's `prev_state`, the recurrent form of the
+network; `None` is the zero state.  Reflection padding, nearest upsampling, LeakyReLU and the residual adds are
+fused into the convolutions; on the wgmma path the ConvLSTM cell update runs in the gate convolution's epilogue
+(b200_convlstm_tma), on the fp32 path in b200_convlstm_cell after the gate convolution.  As in the reference
 the norm layers are constructed (their buffers are part of the state_dict) but never applied
 (`self.norm in ["BN" or "IN"]`, network_local.py:136,169)."""
 import torch
@@ -63,17 +66,27 @@ class ConvLSTM(nn.Module):
         self.Gates = nn.Conv2d(input_size + hidden_size, 4 * hidden_size, kernel_size, padding=kernel_size // 2)
 
     def run(self, x, prev_state=None):
-        if prev_state is not None:
-            raise NotImplementedError("the stage-2 script always passes prev_state=None "
-                                      "(src/neural_filter_and_refinement.py:106)")
-        # zero previous hidden state: only the input half of the gate weights contributes
-        gw = self.Gates.weight
-        if getattr(self, "_w_in_key", None) != (gw.data_ptr(), gw._version):       # input half, sliced once
-            self._w_in = gw.detach()[:, :self.input_size].contiguous()
-            self._w_in_key = (gw.data_ptr(), gw._version)
-        w = self._w_in
-        gates = K.conv2d(x, w, self.Gates.bias.detach(), pad=self.Gates.padding)
-        return K.convlstm_zero_state(gates)
+        """One step -> fresh (hidden, cell) tensors.  `x` is a tensor, or on the wgmma path a `Chain` (input_size
+        channels without a state, input_size + hidden_size with one: the previous hidden state is packed behind x).
+        wgmma path: the gate convolution with the cell update in its epilogue (K.convlstm); fp32 path: the gate
+        convolution on cat(x, prev_hidden), then the cell kernel."""
+        gw, gb = self.Gates.weight, self.Gates.bias.detach()
+        tc = isinstance(x, K.Chain) or K.Chain.available()
+        if prev_state is None:
+            # zero previous hidden state: only the input half of the gate weights contributes
+            if getattr(self, "_w_in_key", None) != (gw.data_ptr(), gw._version):       # input half, sliced once
+                self._w_in = gw.detach()[:, :self.input_size].contiguous()
+                self._w_in_key = (gw.data_ptr(), gw._version)
+            if tc:
+                return K.convlstm(x, self._w_in, gb)
+            gates = K.conv2d(x, self._w_in, gb, pad=self.Gates.padding)
+            return K.convlstm_zero_state(gates)
+        if tc:
+            return K.convlstm(x, gw, gb, prev_state)
+        n, _, h, w = x.shape
+        hidden, cell = K._check_state(prev_state, (n, self.hidden_size, h, w), x.device)
+        gates = K.conv2d(torch.cat((x, hidden), 1), gw, gb, pad=self.Gates.padding)
+        return K.convlstm_cell(gates, cell)
 
 
 class TransformNet(nn.Module):
@@ -111,13 +124,15 @@ class TransformNet(nn.Module):
         self.conv2a.run(c1, "leaky", in_slice=(nf, 2 * nf), out=e2, out_c_off=0)
         self.conv2b.run(e1b, "leaky", out=e2, out_c_off=2 * nf)
         c2[:, 2 * nf:] = e2[:, :2 * nf]
-        if K.Chain.available() and prev_state is None:
+        if chained:
             # wgmma path: conv3 -> 5 residual blocks -> ConvLSTM gates run as one chain of packed fp16 inputs (the
-            # residuals stay fp32 tensors); eleven fp32 -> fp16 repack kernels less
-            hq, wq = rb_shape = (h // 4, w // 4)
+            # residuals stay fp32 tensors); eleven fp32 -> fp16 repack kernels less.  With a state the gates' input is
+            # [RB | prev_hidden]: the last block writes channels [0, 4nf), the ConvLSTM packs the hidden state behind
+            hq, wq = (h // 4, w // 4)
             chains = [K.Chain(n, 4 * nf, hq, wq, (3, 3), 1, dev, tag=f"tn_rb{i & 1}", pad_mode="reflect")
                       for i in range(len(self.ResBlocks))]
-            gates_in = K.Chain(n, 4 * nf, hq, wq, (3, 3), 1, dev, tag="tn_gates")            # zero padding (nn.Conv2d)
+            gates_in = (K.Chain(n, 4 * nf, hq, wq, (3, 3), 1, dev, tag="tn_gates") if prev_state is None  # zero padding
+                        else K.Chain(n, 8 * nf, hq, wq, (3, 3), 1, dev, tag="tn_gates_state"))        # (nn.Conv2d)
             rb = self.conv3.run(e2, "leaky", chain_out=chains[0] if chains else gates_in)
             for i, blk in enumerate(self.ResBlocks):
                 nxt = chains[i + 1] if i + 1 < len(chains) else gates_in

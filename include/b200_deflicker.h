@@ -488,6 +488,29 @@ int b200_conv2d_tma_chain(const B200ConvDesc* d, const float* x, void* in_packed
                           const float* bias, const float* residual, float* y, void* out_packed,
                           const B200ConvDesc* next, int32_t next_c_off, void* workspace,
                           int64_t workspace_bytes, void* stream);
+/* Packs an fp32 NCHW tensor x [next->N][C][next->H][next->W] as fp16 (saturating, like the repack) into the packed
+ * input of the chainable consumer `next`, at its input channels [next_c_off, next_c_off + C): another producer of a
+ * concatenated input, for a tensor no convolution writes (the ConvLSTM's previous hidden state).  Other channels of
+ * out_packed are left as they are.  Refused unless C and next_c_off are multiples of 8 and the slice lies inside
+ * next->Cin. */
+int b200_conv_tma_pack_chain(const B200ConvDesc* next, const float* x, int32_t C, void* out_packed,
+                             int32_t next_c_off, void* stream);
+/* ConvLSTM (network_local.py:18-53) on the tensor cores: the gate convolution `d` (the reference's Gates layer,
+ * Cout = 4C with C % 8 == 0, stride 1, act none, out_scale 1, no residual or output slice) with the cell update in
+ * its epilogue, so the 4C-channel gates tensor is never written:
+ *   cell = sigmoid(remember) * prev_cell + sigmoid(in) * tanh(cell_gate),  hidden = sigmoid(out) * tanh(cell)
+ * with the reference's gate order (chunk(4, 1): in, remember, out, cell) and each product and the sum rounded to
+ * fp32 as torch rounds them; prev_cell == NULL is the zero state (cell = sigmoid(in) * tanh(cell_gate)).
+ * hidden, cell (may be NULL), prev_cell: fp32 [N][C][OH][OW].  x / in_packed / workspace as in b200_conv2d_tma_chain;
+ * with a previous state the input is [x | prev_hidden] (Cin = 2C), e.g. a packed input whose channels [C, 2C) were
+ * filled by b200_conv_tma_pack_chain.  The weight images are gate-interleaved (32-column block b of an N tile holds
+ * the four gates of hidden channels 8b .. 8b+7, see DESIGN §4b): build them with b200_convlstm_tma_weight_images
+ * from the reference's Gates.weight unchanged ([4C][Cin][KH][KW]); they take b200_conv_tma_weight_image_bytes(d)
+ * bytes.  bias is the reference's Gates.bias unchanged. */
+int b200_convlstm_tma_weight_images(const B200ConvDesc* d, const float* w, void* images, void* stream);
+int b200_convlstm_tma(const B200ConvDesc* d, const float* x, void* in_packed, const void* w_images,
+                      const float* bias, const float* prev_cell, float* hidden, float* cell, void* workspace,
+                      int64_t workspace_bytes, void* stream);
 int b200_maxpool2(const float* x, float* y, int64_t planes, int32_t H, int32_t W, void* stream);
 int b200_upsample_bilinear2(const float* x, float* y, int32_t N, int32_t C, int32_t H, int32_t W,
                             int32_t out_c_total, int32_t out_c_off, void* stream);
@@ -499,7 +522,11 @@ int b200_add_relu(const float* a, const float* b, float* out, int64_t n, void* s
 /* mode 0: out = a*b (r*h into a concat buffer); mode 1: out = (1-a)*b + a*c (GRU state update) */
 int b200_gru_gate(const float* a, const float* b, const float* c, float* out, int64_t n_per_sample,
                   int64_t samples, int64_t out_sample_stride, int32_t mode, void* stream);
-/* ConvLSTM cell with prev_state=None: gates [N][4C][H][W] -> hidden, cell (may be NULL) */
+/* ConvLSTM cell on fp32 gates [N][4C][H][W] (pre-activation, chunk(4, 1) order) -> hidden, cell (may be NULL),
+ * [N][C][H][W]; the same expressions as b200_convlstm_tma's epilogue.  prev_cell == NULL is the zero state;
+ * b200_convlstm_zero_state(gates, ...) is b200_convlstm_cell(gates, NULL, ...). */
+int b200_convlstm_cell(const float* gates, const float* prev_cell, float* hidden, float* cell, int32_t N,
+                       int32_t C, int32_t H, int32_t W, void* stream);
 int b200_convlstm_zero_state(const float* gates, float* hidden, float* cell, int32_t N, int32_t C,
                              int32_t H, int32_t W, void* stream);
 /* RAFT.upsample_flow (core/raft.py:76-87): flow [N][2][H][W], mask [N][576][H][W] -> [N][2][8H][8W] */
