@@ -116,6 +116,8 @@ SIGNATURES = {
     "b200_producer_frame": (C.c_int, [_P, _I32, _I32, _P, _P]),
     "b200_producer_scratch_floats": (_I64, [_I32, _I32]),
     "b200_producer_flow_pair": (C.c_int, [_P, _P] + [_I32] * 7 + [_P, _P, _P, _I32, _I32, _P, _P]),
+    "b200_stage2_pack_input": (C.c_int, [_P, _I32, _I32, _I32, _P, _I32, _I32, _I32, _P, _I32, _I32, _P]),
+    "b200_stage2_emit": (C.c_int, [_P, _I64, _I32, _I32, _P, _I64, _I64, _I32, _I32, _P]),
     "b200_dp_adam_step": (C.c_int, [C.POINTER(DpComm), _P, _P, _I64, _I64, C.c_double, C.c_double, C.c_double, C.c_double,
                                     _P, _P, _P]),
     "b200_dp_slice": (C.c_int, [_I32, _I32, _I64, C.POINTER(_I64), C.POINTER(_I64)]),

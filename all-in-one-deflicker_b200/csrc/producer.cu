@@ -12,6 +12,7 @@
 // (tests/test_loader_oracle.py); tests/test_producer_gpu.py compares records and bitmaps with the reference's tensors.
 // Decoding image files and the float64 frame resize stay on the host, one frame at a time.
 #include "common.cuh"
+#include "resize_linear.cuh"
 
 namespace b200 {
 
@@ -33,20 +34,6 @@ __global__ void producer_frame_kernel(const float* __restrict__ frame, int H, in
   rec[p * B200_RECORD_FLOATS + 8] = v[8];
 }
 
-struct ResizeTap { int s0, s1; float w0, w1; };
-
-__device__ __forceinline__ ResizeTap resize_tap(int d, int dst, int src) {
-  const double scale = (double)src / (double)dst;
-  float f = (float)(((double)d + 0.5) * scale - 0.5);
-  int s = (int)floorf(f);
-  f = __fsub_rn(f, (float)s);
-  if (s < 0) { f = 0.f; s = 0; }
-  if (s >= src - 1) { f = 0.f; s = src - 1; }
-  ResizeTap t;
-  t.s0 = s; t.s1 = min(s + 1, src - 1); t.w1 = f; t.w0 = __fsub_rn(1.0f, f);
-  return t;
-}
-
 // dst (H, W, 2) <- src (h, w, 2), H <= h and W <= w; then the reference's scale factors
 __global__ void producer_resize_kernel(const float2* __restrict__ src, int h, int w, float2* __restrict__ dst, int H,
                                        int W, float sx, float sy) {
@@ -60,7 +47,7 @@ __global__ void producer_resize_kernel(const float2* __restrict__ src, int h, in
     o.x = __fmul_rn(__fadd_rn(__fadd_rn(__fadd_rn(a.x, b.x), c.x), d.x), 0.25f);
     o.y = __fmul_rn(__fadd_rn(__fadd_rn(__fadd_rn(a.y, b.y), c.y), d.y), 0.25f);
   } else {
-    const ResizeTap tx = resize_tap(x, W, w), ty = resize_tap(y, H, h);
+    const ResizeTap tx = resize_tap(x, W, w, true), ty = resize_tap(y, H, h, false);
     const float2 a0 = src[(int64_t)ty.s0 * w + tx.s0], a1 = src[(int64_t)ty.s0 * w + tx.s1];
     const float2 b0 = src[(int64_t)ty.s1 * w + tx.s0], b1 = src[(int64_t)ty.s1 * w + tx.s1];
     const float r0x = __fadd_rn(__fmul_rn(a0.x, tx.w0), __fmul_rn(a1.x, tx.w1));

@@ -220,6 +220,29 @@ int b200_producer_flow_pair(const float* flow12, const float* flow21, int32_t h,
                             int32_t first_frame, int32_t filter, float* scratch, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Stage-2 frame plumbing on the device — replaces, per frame, the host arithmetic of
+ *   load_image x2 + InputPadder.pad + torch.cat          src/models/utils.py, neural_filter_and_refinement.py:59-62
+ *   cv2.resize(tensor2img(t), org_size) + save_img       :69-72
+ * 8-bit images in, 8-bit images out.  cv2.resize is restated as OpenCV's own INTER_LINEAR code computes it
+ * (oracle/stage2_io_oracle.py resize_linear_f64 / resize_linear_f32, pinned against cv2.resize with its IPP
+ * back end switched off; where OpenCV dispatches float images to IPP the host results differ in the last bits).
+ * ------------------------------------------------------------------------------------------ */
+/* out [1][6][Hp][Wp] fp32: channels 0-2 = content / 255, channels 3-5 = atlas / 255 resized (Hs, Ws) -> (Hc, Wc),
+ * both replicate-padded to Hp = Hc rounded up to 32 (all rows at the bottom) and Wp = Wc rounded up to 32 (pad // 2
+ * columns on the left, the rest on the right).  content (Hc, Wc, Cc) and atlas (Hs, Ws, Cs) are contiguous uint8 HWC
+ * device images with 1 (grey, repeated), 3 or 4 (4th dropped) channels.  The division and the resize are float64 with
+ * fp32 weights, rounded to fp32 once, as load_image computes them. */
+int b200_stage2_pack_input(const uint8_t* content, int32_t Hc, int32_t Wc, int32_t Cc,
+                           const uint8_t* atlas, int32_t Hs, int32_t Ws, int32_t Cs, float* out,
+                           int32_t Hp, int32_t Wp, void* stream);
+/* src: 3 fp32 planes (Hp, Wp), plane_stride floats apart (a channel slice of a padded NCHW tensor), squeezed to
+ * (H, W) by the fp32 resize exactly as the reference squeezes the padded tensor, then
+ * clip(v * 255, 0, 255) truncated to uint8 (NaN gives 0), RGB -> BGR, written as rows of 3 W bytes at
+ * dst + dst_offset + y * dst_row_stride; no other byte of dst is touched. */
+int b200_stage2_emit(const float* src, int64_t plane_stride, int32_t Hp, int32_t Wp, uint8_t* dst,
+                     int64_t dst_offset, int64_t dst_row_stride, int32_t H, int32_t W, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Data-parallel optimiser step (frame-sharded loop, SURVEY.md §8e): reduce-scatter of the partial
  * [gradients || 8 losses] buffers + Adam + all-gather of the new parameters in ONE kernel over
  * NVLink peer memory.  Replaces  torch.distributed.all_reduce + optimizer.step()  of a data-parallel
