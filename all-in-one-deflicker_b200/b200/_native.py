@@ -101,6 +101,9 @@ SIGNATURES = {
     "b200_atlas_param_floats_for": (_I64, [C.POINTER(MlpDesc)]),
     "b200_atlas_workspace_bytes_for": (_I64, [C.POINTER(AtlasConfig), C.POINTER(MlpDesc)]),
     "b200_atlas_workspace_offsets_for": (C.c_int, [C.POINTER(AtlasConfig), C.POINTER(MlpDesc), _P, C.POINTER(_I64)]),
+    "b200_mlp_tc_image_offsets": (C.c_int, [C.POINTER(MlpDesc), _I64, _P, C.POINTER(_I64)]),
+    "b200_atlas_tc_image_offsets_for": (C.c_int, [C.POINTER(AtlasConfig), C.POINTER(MlpDesc), _P, _I32,
+                                                  C.POINTER(_I64)]),
     "b200_atlas_loss_grad_for": (C.c_int, [C.POINTER(AtlasConfig), C.POINTER(MlpDesc), C.POINTER(Video), _P, _P, _P, _P,
                                            _P, _I64, _P]),
     "b200_pretrain_loss_grad_for": (C.c_int, [C.POINTER(AtlasConfig), C.POINTER(MlpDesc), _I32, _I32, _I32, _P, _P, _P,

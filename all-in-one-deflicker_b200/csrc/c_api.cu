@@ -237,19 +237,26 @@ int64_t b200_mlp_workspace_bytes(const B200MlpDesc* d, int64_t rows, int trainin
   return need;
 }
 
-static int tc_call_prepare(const B200MlpDesc* d, int64_t rows, void* ws, int64_t ws_bytes, MlpShape* s, TcNet* net,
-                           int64_t* rows_pad, TcCallPlan* pl) {
+// the shape and the buffers of a stand-alone tensor-core call on `rows` rows in the workspace `ws`
+static int tc_call_plan(const B200MlpDesc* d, int64_t rows, const void* ws, MlpShape* s, TcNet* net, int64_t* rows_pad,
+                        TcCallPlan* pl) {
   B200_PROPAGATE(resolve_mlp(d, s));
   *net = tc_net_of(*s);
   B200_REQUIRE(*net != TcNet::None, "B200_PREC_TC serves the stage-1 architectures (mapping: 3-256x{2,4}-2 without encoding "
                "or 3-PE{1..10}-256x{2,4}-2; alpha: 3-PE5-256x6-1; atlas: 2-PE10-256x6-3 with skips 4, 7); use B200_PREC_FP32 "
                "for other shapes");
-  if (!b200_device_supports_tc()) { set_error("B200_PREC_TC needs a compute-capability 9.x device"); return B200_ERR_UNSUPPORTED; }
   B200_REQUIRE(rows > 0 && rows < (1ll << 26), "rows out of range: %lld", (long long)rows);
   B200_REQUIRE(ws != nullptr, "null workspace");
   *rows_pad = round_up(rows, kTileRows);
-  char* base = reinterpret_cast<char*>(round_up(reinterpret_cast<int64_t>(ws), 1024));
-  plan_tc_call(*s, *net, *rows_pad, base, pl);
+  plan_tc_call(*s, *net, *rows_pad, reinterpret_cast<char*>(round_up(reinterpret_cast<int64_t>(ws), 1024)), pl);
+  return B200_OK;
+}
+
+static int tc_call_prepare(const B200MlpDesc* d, int64_t rows, void* ws, int64_t ws_bytes, MlpShape* s, TcNet* net,
+                           int64_t* rows_pad, TcCallPlan* pl) {
+  B200_PROPAGATE(tc_call_plan(d, rows, ws, s, net, rows_pad, pl));
+  if (!b200_device_supports_tc()) { set_error("B200_PREC_TC needs a compute-capability 9.x device"); return B200_ERR_UNSUPPORTED; }
+  const char* base = reinterpret_cast<const char*>(pl->gmax2);      // the first buffer of the plan
   if (base + pl->bytes > reinterpret_cast<char*>(ws) + ws_bytes) {
     set_error("workspace too small: need %lld bytes", (long long)(pl->bytes + 2048));
     return B200_ERR_WORKSPACE;
@@ -410,6 +417,29 @@ int b200_atlas_workspace_offsets_for(const B200AtlasConfig* cfg, const B200MlpDe
   offsets[5] = reinterpret_cast<char*>(pl.d_y) - w;
   offsets[6] = reinterpret_cast<char*>(pl.map.y) - w;
   offsets[7] = reinterpret_cast<char*>(pl.atlas.y) - w;
+  return B200_OK;
+}
+
+int b200_mlp_tc_image_offsets(const B200MlpDesc* d, int64_t rows, const void* ws, int64_t* out) {
+  B200_REQUIRE(out != nullptr, "null pointer");
+  MlpShape s; TcNet net; int64_t rows_pad; TcCallPlan pl;
+  B200_PROPAGATE(tc_call_plan(d, rows, ws, &s, &net, &rows_pad, &pl));
+  const char* w = reinterpret_cast<const char*>(ws);
+  tc_single_image_offsets(s, net, rows_pad, pl.tc, w, out);
+  out[B200_TC_OFFSET_GMAX] = reinterpret_cast<char*>(pl.gmax2) - w;
+  return B200_OK;
+}
+
+int b200_atlas_tc_image_offsets_for(const B200AtlasConfig* cfg, const B200MlpDesc* mapping, const void* ws,
+                                    int32_t net, int64_t* out) {
+  B200_REQUIRE(cfg && ws && out, "null pointer");
+  B200_REQUIRE(cfg->precision == B200_PREC_TC, "the tensor-core images exist at B200_PREC_TC only");
+  B200_REQUIRE(net == 0 || net == 1, "net must be 0 (mapping) or 1 (atlas), got %d", net);
+  AtlasPlan pl;
+  B200_PROPAGATE(plan_atlas(cfg, mapping, reinterpret_cast<char*>(round_up(reinterpret_cast<int64_t>(ws), 256)), &pl));
+  const char* w = reinterpret_cast<const char*>(ws);
+  tc_step_image_offsets(pl.ms, pl.as, pl.tc, net == 1, w, out);
+  out[B200_TC_OFFSET_GMAX] = reinterpret_cast<char*>(pl.counters + 3) - w;     // tc_step_backward's gmax words
   return B200_OK;
 }
 

@@ -1655,6 +1655,35 @@ int64_t tc_single_workspace_bytes(const MlpShape& sh, TcNet net, int64_t rows) {
   return pl.bytes + 2048;
 }
 
+// ---------------------------------------------------------------------------------------------
+// diagnostics: where the images of one network lie, from the plans the kernels' launches use
+// ---------------------------------------------------------------------------------------------
+static void image_offsets(const NetImages& im, const char* ws, int64_t* out) {
+  auto at = [&](const void* p) { return p ? (int64_t)(reinterpret_cast<const char*>(p) - ws) : (int64_t)-1; };
+  out[0] = at(im.w_fwd); out[1] = at(im.w_bwd); out[2] = at(im.cst); out[3] = at(im.act);
+  out[4] = at(im.dz); out[5] = at(im.pe); out[6] = at(im.dzl); out[7] = at(im.bits);
+  out[8] = im.slot_stride; out[9] = im.term_stride; out[10] = im.w64_term_stride; out[11] = im.rows;
+  for (int l = 0; l < B200_MAX_LAYERS; ++l) {
+    out[12 + l] = im.w_fwd_layer[l];
+    out[12 + B200_MAX_LAYERS + l] = im.n_chunks_fwd[l];
+    out[12 + 2 * B200_MAX_LAYERS + l] = im.w_bwd_layer[l];
+  }
+}
+
+void tc_single_image_offsets(const MlpShape& sh, TcNet net, int64_t rows, char* tc_ws, const char* ws, int64_t* out) {
+  SinglePlan pl{};
+  plan_single(sh, net, rows, tc_ws, &pl);
+  image_offsets(pl.im, ws, out);
+}
+
+void tc_step_image_offsets(const MlpShape& ms, const MlpShape& as, const TcPlan& plan, bool atlas, const char* ws,
+                           int64_t* out) {
+  TcStep s{};
+  s.ms = &ms; s.as = &as; s.plan = &plan;
+  const TcLayout lay = layout_of(s);
+  image_offsets(atlas ? lay.atl : lay.map, ws, out);
+}
+
 static int check_single(const MlpShape& sh, TcNet net, const TcRows& r) {
   B200_PROPAGATE(ensure_attrs());
   B200_REQUIRE(net != TcNet::None && tc_net_of(sh) == net, "tensor-core IMLP: the shape is not the network it is "

@@ -95,4 +95,10 @@ struct PersistentWorkspaceScope {
 
 int tc_debug_wgrad(long long* cycles, int* shapes, int max_ctas);
 
+// diagnostics: the first B200_TC_OFFSET_GMAX entries of the b200_*_tc_image_offsets vector (see the header) for the
+// images of a stand-alone call whose tensor-core workspace starts at tc_ws, or of one network of the fused step
+void tc_single_image_offsets(const MlpShape& sh, TcNet net, int64_t rows, char* tc_ws, const char* ws, int64_t* out);
+void tc_step_image_offsets(const MlpShape& ms, const MlpShape& as, const TcPlan& plan, bool atlas, const char* ws,
+                           int64_t* out);
+
 }  // namespace b200

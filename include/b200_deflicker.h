@@ -185,6 +185,28 @@ int b200_atlas_workspace_offsets(const B200AtlasConfig* cfg, const void* ws, int
 int b200_atlas_workspace_offsets_for(const B200AtlasConfig* cfg, const B200MlpDesc* mapping,
                                      const void* ws, int64_t* offsets);
 
+/* Test / debugging aid: where the tensor-core path (B200_PREC_TC) keeps the operand images of one
+ * network inside a workspace, computed by the planning functions its launches use.  out receives
+ * B200_TC_OFFSET_FLOATS int64:
+ *   [0..7]   byte offsets from `ws` of: forward weight items, dgrad (W^T) weight items, forward
+ *            constants, activation images, dZ images, positional-encoding image, output-layer dZ
+ *            image, ReLU flag words (-1 where the network has no such buffer)
+ *   [8..11]  bytes from one activation / dZ slot to the next, from the hi to the lo term of those
+ *            images, from the hi to the lo term of the 64-wide images; rows of the images
+ *   [12..27] byte offset of layer l's forward weight items from [0]
+ *   [28..43] number of 64-wide k chunks (4 items each) of layer l's forward weight items
+ *   [44..59] byte offset of layer l's dgrad weight items from [1]
+ *   [60]     byte offset of the two int32 gmax words the backward took its gradient scales from
+ *            ([0] atlas-shaped networks, [1] mappings)
+ * b200_mlp_tc_image_offsets: the workspace of b200_mlp_forward / backward(d, ..., rows, B200_PREC_TC,
+ * ws, ...).  b200_atlas_tc_image_offsets_for: the workspace of b200_atlas_loss_grad_for(cfg, mapping,
+ * ..., ws, ...), net 0 = the mapping, 1 = the atlas. */
+#define B200_TC_OFFSET_GMAX 60
+#define B200_TC_OFFSET_FLOATS 61
+int b200_mlp_tc_image_offsets(const B200MlpDesc* d, int64_t rows, const void* ws, int64_t* out);
+int b200_atlas_tc_image_offsets_for(const B200AtlasConfig* cfg, const B200MlpDesc* mapping,
+                                    const void* ws, int32_t net, int64_t* out);
+
 /* One pre_train_mapping step (src/models/stage_1/unwrap_utils.py:182-195): rows ys / columns
  * xs (int64[batch]) of frame `frame`; gradients of the mapping block only; loss -> losses[0]. */
 int b200_pretrain_loss_grad(const B200AtlasConfig* cfg, int32_t larger_dim, int32_t T,
