@@ -74,6 +74,7 @@ class SegConfig(C.Structure):
 
 
 SEG_LOSS_FLOATS = 16
+SEG_OFFSET_FLOATS = 15
 
 _P = C.c_void_p
 _I64 = C.c_int64
@@ -128,6 +129,7 @@ SIGNATURES = {
     "b200_seg_param_floats": (_I64, [C.POINTER(SegConfig), C.POINTER(_I64)]),
     "b200_seg_workspace_bytes": (_I64, [C.POINTER(SegConfig)]),
     "b200_seg_loss_grad": (C.c_int, [C.POINTER(SegConfig), C.POINTER(Video), _P, _P, _P, _P, _P, _P, _I64, _P]),
+    "b200_seg_workspace_offsets": (C.c_int, [C.POINTER(SegConfig), _P, C.POINTER(_I64)]),
     "b200_mlp_pretrain_workspace_bytes": (_I64, [C.POINTER(MlpDesc), _I32]),
     "b200_mlp_pretrain_loss_grad": (C.c_int, [C.POINTER(MlpDesc), _I32, _F, _I32, _I32, _I32, _P, _P, _P, _P, _P, C.c_int,
                                               _P, _I64, _P]),

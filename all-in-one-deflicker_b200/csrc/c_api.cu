@@ -499,6 +499,13 @@ int b200_atlas_loss_grad_for(const B200AtlasConfig* cfg, const B200MlpDesc* mapp
   geo.half_frames = (float)((double)video->T / 2.0);
   geo.d_local = cfg->derivative_amount;
   geo.d_global = cfg->global_derivative_amount;
+  // The networks run whole 128-row tiles: rows of the flow-match groups past their compacted counts, and the padding
+  // slots of a frame shard, are evaluated but never written by the sampling kernel.  Zero rows keep them finite
+  // whatever the workspace held before (0 x NaN in a weight gradient would be NaN).  With the whole video resident the
+  // kernel writes every other row itself, padding included, so only the two flow-match groups need clearing.
+  const bool whole_video = video->t_begin == 0 && video->t_end == video->T;
+  B200_CHECK_CUDA(cudaMemsetAsync(pl.x_map + (whole_video ? (size_t)G_FWD * cap * 4 : 0), 0,
+                                  (size_t)(whole_video ? 2 : ng) * cap * 16, st));
   B200_PROPAGATE(launch_select_sample(indices, cfg->batch, *video, geo, cap, ng, pl.counters, pl.list, pl.x_map,
                                       pl.targets, st));
 

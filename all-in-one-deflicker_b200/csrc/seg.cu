@@ -322,6 +322,17 @@ int64_t b200_seg_workspace_bytes(const B200SegConfig* cfg) {
   return pl.bytes + 2048;
 }
 
+int b200_seg_workspace_offsets(const B200SegConfig* cfg, const void* ws, int64_t* out) {
+  B200_REQUIRE(cfg && ws && out, "null pointer");
+  SegPlan pl;
+  B200_PROPAGATE(plan_seg(cfg, reinterpret_cast<char*>(round_up(reinterpret_cast<int64_t>(ws), 1024)), &pl));
+  const char* w = reinterpret_cast<const char*>(ws);
+  const void* bufs[B200_SEG_OFFSET_FLOATS] = {pl.counters, pl.x_map, pl.targets, pl.x3, pl.xa, pl.xat, pl.uv1, pl.uv2,
+                                              pl.ar, pl.yat, pl.d_uv1, pl.d_uv2, pl.d_ar, pl.d_yat, pl.d_xat};
+  for (int i = 0; i < B200_SEG_OFFSET_FLOATS; ++i) out[i] = reinterpret_cast<const char*>(bufs[i]) - w;
+  return B200_OK;
+}
+
 int b200_seg_loss_grad(const B200SegConfig* cfg, const B200Video* video, const float* mask, const int64_t* indices,
                        const float* params, float* grads, float* losses, void* ws, int64_t ws_bytes, void* stream) {
   B200_REQUIRE(cfg && video && mask && indices && params && grads && losses, "null pointer");

@@ -408,6 +408,16 @@ int b200_seg_loss_grad(const B200SegConfig* cfg, const B200Video* video, const f
                        const int64_t* indices, const float* params, float* grads, float* losses,
                        void* ws, int64_t ws_bytes, void* stream);
 
+/* Test / debugging aid: byte offsets (from `ws`) of the intermediate buffers of b200_seg_loss_grad
+ * inside its workspace, for the configuration `cfg` (host only, no launch).  out receives
+ * B200_SEG_OFFSET_FLOATS int64, cap = batch rounded up to 128:
+ *   [0] counters (int32, as in the atlas step)  [1] x_map [9][cap][4]  [2] targets [cap][12]
+ *   [3] x3 [9][cap][3]  [4] xa [5][cap][3]  [5] xat [6][cap][2]  [6] uv1 [9][cap][2]
+ *   [7] uv2 [9][cap][2]  [8] ar [5][cap]  [9] yat [6][cap][3]  [10] d_uv1  [11] d_uv2  [12] d_ar
+ *   [13] d_yat  [14] d_xat (same shapes as the buffers they are the gradients of) */
+#define B200_SEG_OFFSET_FLOATS 15
+int b200_seg_workspace_offsets(const B200SegConfig* cfg, const void* ws, int64_t* out);
+
 /* One pre_train_mapping step (unwrap_utils.py:182-195) for ANY mapping-shaped IMLP (3 -> 2):
  * gradients of that network (its own flat layout, overwritten); loss -> losses[0]. */
 int64_t b200_mlp_pretrain_workspace_bytes(const B200MlpDesc* d, int32_t batch);
