@@ -73,6 +73,15 @@ class SegConfig(C.Structure):
                 ("mapping1", MlpDesc), ("mapping2", MlpDesc), ("alpha", MlpDesc), ("atlas", MlpDesc)]
 
 
+class PngPlan(C.Structure):
+    _fields_ = [("magic", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("n_blocks", C.c_int32),
+                ("n_chunks", C.c_int32), ("prefix_bytes", C.c_int32), ("suffix_bytes", C.c_int32),
+                ("max_chunk", C.c_int32), ("raw_bytes", C.c_int64), ("zlib_bytes", C.c_int64),
+                ("file_bytes", C.c_int64), ("plan_bytes", C.c_int64), ("block_raw_at", C.c_int64),
+                ("chunk_z_at", C.c_int64), ("prefix_at", C.c_int64), ("suffix_at", C.c_int64),
+                ("zlib_header", C.c_uint8 * 8)]
+
+
 SEG_LOSS_FLOATS = 16
 SEG_OFFSET_FLOATS = 15
 
@@ -122,6 +131,10 @@ SIGNATURES = {
     "b200_producer_flow_pair": (C.c_int, [_P, _P] + [_I32] * 7 + [_P, _P, _P, _I32, _I32, _P, _P]),
     "b200_stage2_pack_input": (C.c_int, [_P, _I32, _I32, _I32, _P, _I32, _I32, _I32, _P, _I32, _I32, _P]),
     "b200_stage2_emit": (C.c_int, [_P, _I64, _I32, _I32, _P, _I64, _I64, _I32, _I32, _P]),
+    "b200_png_plan_bytes": (_I64, [_I32, _I32, _I32, _I32]),
+    "b200_png_plan": (C.c_int, [_I32, _I32, _P, _P, _P, _I32, _P, _I32, _P, _I32, _P, _I32, _P, _I64]),
+    "b200_png_workspace_bytes": (_I64, [_I32, _I32]),
+    "b200_png_encode": (C.c_int, [C.POINTER(PngPlan), _P, _P, _P, _I64, _P, _I64, _P]),
     "b200_dp_adam_step": (C.c_int, [C.POINTER(DpComm), _P, _P, _I64, _I64, C.c_double, C.c_double, C.c_double, C.c_double,
                                     _P, _P, _P]),
     "b200_dp_slice": (C.c_int, [_I32, _I32, _I64, C.POINTER(_I64), C.POINTER(_I64)]),

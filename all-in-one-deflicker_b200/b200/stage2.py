@@ -4,7 +4,8 @@
 three 8-bit images the script writes out.  The filter network's input is built by b200_stage2_pack_input and the output
 images by b200_stage2_emit (csrc/stage2_io.cu); only uint8 crosses the bus, through pinned buffers.  The arithmetic is
 the script's, restated from OpenCV's own resize code (oracle/stage2_io_oracle.py); images that are not 8-bit go through
-the host arithmetic of src/models/utils.py instead.
+the host arithmetic of src/models/utils.py instead.  `Stage2.frame_png` goes one step further and returns the three PNG
+files the script writes, encoded on the device by b200.png (csrc/png_encode.cu).
 """
 from __future__ import annotations
 
@@ -12,6 +13,7 @@ import numpy as np
 import torch
 
 from . import _native as N
+from . import png
 
 
 def pad_geometry(h: int, w: int):
@@ -72,7 +74,8 @@ class Stage2:
     """The two networks and every device / pinned buffer of one frame geometry (re-made when the geometry changes).
 
     frame() returns {"filter", "final": uint8 BGR (H, W, 3), "concat": (H, 3 W, 3)} as numpy views of one of two
-    pinned buffers used in turn: a result stays valid until the call after next."""
+    pinned buffers used in turn: a result stays valid until the call after next.  frame_png() returns the same three
+    images as the bytes of their PNG files (cv2.imwrite at compression 0), with the same lifetime."""
 
     def __init__(self, filter_net, local_net, device):
         self.filter_net, self.local_net, self.device = filter_net, local_net, torch.device(device)
@@ -98,7 +101,20 @@ class Stage2:
         self._host = [torch.empty(5 * n, dtype=torch.uint8).pin_memory() for _ in range(2)]
         self._done = [torch.cuda.Event() for _ in range(2)]
         self._turn = 0
+        self._png_files = None
         self._geom = geom
+
+    def _png_buffers(self, hc, wc):
+        """Plans, workspace and output buffers of the three encodes, made on the first frame_png of a geometry."""
+        if self._png_files is not None:
+            return
+        dev = self.device
+        plans = [png.plan(hc, 3 * wc, dev), png.plan(hc, wc, dev), png.plan(hc, wc, dev)]
+        ends = np.cumsum([0] + [p.file_bytes for p in plans]).tolist()
+        self._png_files = list(zip(ends[:-1], ends[1:]))
+        self._png_ws = torch.empty(max(p.workspace_bytes for p in plans), dtype=torch.uint8, device=dev)
+        self._png = torch.empty(ends[-1], dtype=torch.uint8, device=dev)
+        self._png_host = [torch.empty(ends[-1], dtype=torch.uint8).pin_memory() for _ in range(2)]
 
     def _to_device(self, img, k):
         if torch.is_tensor(img) and img.is_cuda:
@@ -108,36 +124,60 @@ class Stage2:
         self._u8[k].copy_(self._stage[k], non_blocking=True)
         return self._u8[k]
 
-    @torch.no_grad()
-    def frame(self, content, atlas):
+    def _emit_frame(self, content, atlas):
+        """One trip up to the three 8-bit images in self._out (concat, filter, final, back to back)."""
         is_u8 = lambda a: (a.dtype == torch.uint8) if torch.is_tensor(a) else (np.asarray(a).dtype == np.uint8)
         shape3 = lambda a: tuple(a.shape) + (1,) * (3 - len(a.shape))
         hc, wc = content.shape[:2]
+        self._buffers((shape3(content), shape3(atlas)))
+        if is_u8(content) and is_u8(atlas):
+            x6 = pack_input(self._to_device(content, 0), self._to_device(atlas, 1), out=self._x6)
+        else:
+            as_np = lambda a: a.cpu().numpy() if torch.is_tensor(a) else a
+            x6 = host_input(as_np(content), as_np(atlas), self.device)
+        pred = self.filter_net(x6)
+        if self._o1 is None:
+            o2 = pred
+        else:
+            out, _ = self.local_net(torch.cat((pred, self._o1, pred, self._p1), dim=1), None)
+            o2 = pred + out
+        self._p1, self._o1 = pred, o2
+        n = hc * wc * 3
+        concat, filt, final = (self._out[a:b].view(hc, -1, 3) for a, b in ((0, 3 * n), (3 * n, 4 * n), (4 * n, 5 * n)))
+        for k, t in enumerate((x6[:, 0:3], x6[:, 3:6], pred)):
+            emit(t, concat, k * wc, wc)
+        emit(pred, filt, 0, wc)
+        emit(o2, final, 0, wc)
+        return concat, filt, final
+
+    def _to_host(self, src, hosts):
+        """src -> the pinned buffer of this turn, waited for; the buffer is reused two calls later."""
+        host, done = hosts[self._turn], self._done[self._turn]
+        self._turn ^= 1
+        host.copy_(src, non_blocking=True)
+        done.record()
+        done.synchronize()
+        return host.numpy()
+
+    @torch.no_grad()
+    def frame(self, content, atlas):
+        hc, wc = content.shape[:2]
         with torch.cuda.device(self.device):
-            self._buffers((shape3(content), shape3(atlas)))
-            if is_u8(content) and is_u8(atlas):
-                x6 = pack_input(self._to_device(content, 0), self._to_device(atlas, 1), out=self._x6)
-            else:
-                as_np = lambda a: a.cpu().numpy() if torch.is_tensor(a) else a
-                x6 = host_input(as_np(content), as_np(atlas), self.device)
-            pred = self.filter_net(x6)
-            if self._o1 is None:
-                o2 = pred
-            else:
-                out, _ = self.local_net(torch.cat((pred, self._o1, pred, self._p1), dim=1), None)
-                o2 = pred + out
-            self._p1, self._o1 = pred, o2
-            n = hc * wc * 3
-            concat, filt, final = (self._out[a:b].view(hc, -1, 3) for a, b in ((0, 3 * n), (3 * n, 4 * n), (4 * n, 5 * n)))
-            for k, t in enumerate((x6[:, 0:3], x6[:, 3:6], pred)):
-                emit(t, concat, k * wc, wc)
-            emit(pred, filt, 0, wc)
-            emit(o2, final, 0, wc)
-            host, done = self._host[self._turn], self._done[self._turn]
-            self._turn ^= 1
-            host.copy_(self._out, non_blocking=True)
-            done.record()
-            done.synchronize()
-        h = host.numpy()
+            self._emit_frame(content, atlas)
+            h = self._to_host(self._out, self._host)
+        n = hc * wc * 3
         return {"concat": h[:3 * n].reshape(hc, 3 * wc, 3), "filter": h[3 * n:4 * n].reshape(hc, wc, 3),
                 "final": h[4 * n:].reshape(hc, wc, 3)}
+
+    @torch.no_grad()
+    def frame_png(self, content, atlas):
+        """frame(), then the three images encoded as PNG files on the device and copied to the host in one copy:
+        {"concat", "filter", "final"} -> uint8 numpy views of the files' bytes."""
+        hc, wc = content.shape[:2]
+        with torch.cuda.device(self.device):
+            imgs = self._emit_frame(content, atlas)
+            self._png_buffers(hc, wc)
+            for img, (a, b) in zip(imgs, self._png_files):
+                png.encode(img, out=self._png[a:b], workspace=self._png_ws)
+            h = self._to_host(self._png, self._png_host)
+        return {k: h[a:b] for k, (a, b) in zip(("concat", "filter", "final"), self._png_files)}

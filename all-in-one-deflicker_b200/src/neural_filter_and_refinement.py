@@ -1,8 +1,10 @@
 """Stage 2 — neural filter (UNet) + local refinement (TransformNet) with the reference's CLI and output
 folders (src/neural_filter_and_refinement.py).  Like the reference it requires a GPU.
 
-The frames stay on the device (b200.stage2.Stage2): the host only decodes and encodes 8-bit PNGs, the next frame's
-decode on one thread and the previous frame's three writes on a small pool while the current frame is on the GPU."""
+The frames stay on the device (b200.stage2.Stage2), and so does the PNG encoding of the three output images
+(Stage2.frame_png: the files cv2.imwrite writes at compression 0, byte for byte): the host decodes the 8-bit input PNGs
+and writes finished files, the next frame's decode on one thread and the previous frame's three writes on a small pool
+while the current frame is on the GPU."""
 import argparse
 import concurrent.futures as cf
 import os
@@ -15,7 +17,6 @@ from types import SimpleNamespace
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 
-import cv2          # noqa: E402
 import numpy as np  # noqa: E402
 import torch        # noqa: E402
 from tqdm import tqdm  # noqa: E402
@@ -42,20 +43,21 @@ def _decode(path):
     return np.array(Image.open(path))
 
 
-def _write(img, path):
-    cv2.imwrite(path, img, [cv2.IMWRITE_PNG_COMPRESSION, 0])
+def _write(data, path):
+    with open(path, "wb") as f:
+        f.write(data)
 
 
 def run_frames(stage2, content_names, style_names, out_dirs, sync_io=False, progress=lambda it: it):
     """The frame loop: out_dirs = {"concat", "filter", "final"} -> folder.  Pipelined unless sync_io: frame i + 1 is
-    decoded and frame i - 1 written while frame i is on the GPU.  A frame's images are views of a buffer Stage2 reuses
+    decoded and frame i - 1 written while frame i is on the GPU.  A frame's files are views of a buffer Stage2 reuses
     two calls later, so frame i's writes are awaited before frame i + 2 starts.  Every thread is joined on return and
     on any exception."""
     n = len(content_names)
     stage2.reset()
     if sync_io:
         for i in progress(range(n)):
-            imgs = stage2.frame(_decode(content_names[i]), _decode(style_names[i]))
+            imgs = stage2.frame_png(_decode(content_names[i]), _decode(style_names[i]))
             for key, folder in out_dirs.items():
                 _write(imgs[key], "{}/{:05d}.png".format(folder, i))
         return
@@ -70,7 +72,7 @@ def run_frames(stage2, content_names, style_names, out_dirs, sync_io=False, prog
                 for w in f:
                     w.result()
             pending = pending[-1:]
-            imgs = stage2.frame(content, style)
+            imgs = stage2.frame_png(content, style)
             pending.append([writers.submit(_write, imgs[key], "{}/{:05d}.png".format(folder, i))
                             for key, folder in out_dirs.items()])
         for f in pending:

@@ -265,6 +265,54 @@ int b200_stage2_emit(const float* src, int64_t plane_stride, int32_t Hp, int32_t
                      int64_t dst_offset, int64_t dst_row_stride, int32_t H, int32_t W, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * PNG encoding of an 8-bit BGR image, byte for byte the file
+ *   cv2.imwrite(path, img, [cv2.IMWRITE_PNG_COMPRESSION, 0])        save_img, src/models/utils.py
+ * writes (libpng's adaptive row filters on RGB, zlib stored blocks).  What depends on the pixels — the row filters,
+ * the filtered bytes, the Adler-32 and the IDAT CRC-32s — is computed on the device; what depends on (H, W) only —
+ * zlib header, stored-block lengths, IDAT chunk lengths, the bytes before the first and after the last IDAT chunk —
+ * is a plan the caller builds once per shape from the layout of the writer's file of any image of that shape.
+ * ------------------------------------------------------------------------------------------ */
+#define B200_PNG_PLAN_MAGIC 0x504e4731     /* "PNG1" */
+#define B200_PNG_MAX_CHUNK 32768           /* longest IDAT chunk a plan may have (libpng writes 8192)      */
+#define B200_PNG_MAX_PREFIX 4096           /* longest run of bytes before the first / after the last IDAT  */
+#define B200_PNG_MAX_RAW (1ll << 30)       /* H (3 W + 1): filtered bytes of one image                     */
+/* Header of a plan; the tables follow it in the same buffer at the byte offsets *_at.  The plan is plain bytes: the
+ * caller keeps the host copy (b200_png_encode reads its header) and uploads the whole of it once. */
+typedef struct B200PngPlan {
+  int32_t magic;                   /* B200_PNG_PLAN_MAGIC                                           */
+  int32_t H, W;
+  int32_t n_blocks, n_chunks;      /* stored deflate blocks, IDAT chunks                            */
+  int32_t prefix_bytes, suffix_bytes;
+  int32_t max_chunk;               /* longest IDAT chunk                                            */
+  int64_t raw_bytes;               /* H (3 W + 1): filtered rows, each led by its filter byte       */
+  int64_t zlib_bytes;              /* 2 + 5 n_blocks + raw_bytes + 4                                */
+  int64_t file_bytes;              /* prefix + 12 n_chunks + zlib_bytes + suffix                    */
+  int64_t plan_bytes;              /* header and tables                                             */
+  int64_t block_raw_at;            /* uint32 [n_blocks + 1]: raw offset of each block, then raw_bytes */
+  int64_t chunk_z_at;              /* uint32 [n_chunks + 1]: zlib offset of each chunk, then zlib_bytes */
+  int64_t prefix_at, suffix_at;    /* the bytes before the first IDAT chunk / after the last        */
+  uint8_t zlib_header[8];          /* CMF, FLG; the rest 0                                          */
+} B200PngPlan;
+/* bytes of a plan with these table sizes; -1 (message) when a size is out of range */
+int64_t b200_png_plan_bytes(int32_t n_blocks, int32_t n_chunks, int32_t prefix_bytes, int32_t suffix_bytes);
+/* Host only.  Validates a layout and writes the plan into `plan` (host memory, plan_capacity bytes):
+ * zlib_header[2]; block_heads[b] the stored blocks' first bytes (0, the last 1: BFINAL, BTYPE 00) and block_lens[b]
+ * their lengths (<= 65535, summing to H (3 W + 1)); chunk_lens[c] the IDAT lengths (1 .. B200_PNG_MAX_CHUNK,
+ * summing to the zlib stream's length); prefix = signature, IHDR (8-bit RGB, H x W, not interlaced), any other
+ * chunk before the first IDAT; suffix = the chunks after the last, ending with IEND. */
+int b200_png_plan(int32_t H, int32_t W, const uint8_t* zlib_header, const uint8_t* block_heads,
+                  const int32_t* block_lens, int32_t n_blocks, const int32_t* chunk_lens, int32_t n_chunks,
+                  const uint8_t* prefix, int32_t prefix_bytes, const uint8_t* suffix, int32_t suffix_bytes,
+                  void* plan, int64_t plan_capacity);
+/* device workspace of one encode (the filtered rows and per-row Adler-32 sums); -1 (message) for a bad size */
+int64_t b200_png_workspace_bytes(int32_t H, int32_t W);
+/* Encodes the contiguous uint8 BGR device image (plan->H, plan->W, 3) into out[0, plan->file_bytes).
+ * plan = the host plan, plan_device = its upload (8-byte aligned).  Two launches, no allocation, no
+ * synchronisation; workspace_bytes and out_capacity are checked against the plan. */
+int b200_png_encode(const B200PngPlan* plan, const void* plan_device, const uint8_t* image, void* workspace,
+                    int64_t workspace_bytes, uint8_t* out, int64_t out_capacity, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Data-parallel optimiser step (frame-sharded loop, SURVEY.md §8e): reduce-scatter of the partial
  * [gradients || 8 losses] buffers + Adam + all-gather of the new parameters in ONE kernel over
  * NVLink peer memory.  Replaces  torch.distributed.all_reduce + optimizer.step()  of a data-parallel
