@@ -151,6 +151,8 @@ SIGNATURES = {
     "b200_eval_maps_workspace_bytes": (_I64, [C.POINTER(MlpDesc), _I64]),
     "b200_eval_maps": (C.c_int, [C.POINTER(MlpDesc), _P, C.POINTER(Video), _I32, _I64, _I64, _F, _F, C.c_int, _P, _P, _P,
                                  _P, _I64, _P]),
+    "b200_frame_sse_workspace_bytes": (_I64, [_I32, _I32]),
+    "b200_frame_sse": (C.c_int, [C.POINTER(Video), _I32, _P, _P, _P, _I64, _P]),
     "b200_render_workspace_bytes": (_I64, [_I64]),
     "b200_render": (C.c_int, [_P, _I32, _I32, _I32, _I32, _I64, _I64, _P, _P, C.c_int, _P, _I64, _P]),
     "b200_corr_pyramid_floats": (_I64, [_I32, _I32]),

@@ -68,6 +68,14 @@ class DeviceVideo:
     def num_pixels(self):
         return self.H * self.W * self.T
 
+    def frame_rgb(self, f: int) -> torch.Tensor:
+        """The fp32 frame f as held in channels 0..2 of its resident records: an (H, W, 3) device tensor (a copy)."""
+        if not self.t_begin <= f < self.t_end:
+            raise N.B200Error(f"frame {f} is not resident (frames [{self.t_begin}, {self.t_end}))")
+        HW = self.H * self.W
+        rec = self.records[(f - self.t_begin) * HW * N.RECORD_FLOATS:(f - self.t_begin + 1) * HW * N.RECORD_FLOATS]
+        return rec.view(HW, N.RECORD_FLOATS)[:, :3].reshape(self.H, self.W, 3)
+
     def mask_fwd_host(self) -> torch.Tensor:
         """The forward consistency masks as the reference's (H, W, T, 1) fp32 CPU tensor, unpacked from the bitmap."""
         n = self.num_pixels
@@ -124,21 +132,31 @@ class DeviceVideo:
         return cls(H, W, T, t_begin, t_end, records, bits_f, bits_b)
 
 
+def video_files(data_folder):
+    """The frame files of a video folder in frame order (load_input_data_single's listing)."""
+    from pathlib import Path
+    data_folder = Path(data_folder)
+    return sorted(list(data_folder.glob("*.jpg")) + list(data_folder.glob("*.png")))
+
+
 def _from_files(cls, data_folder, vid_root, vid_name, resy: int, resx: int, maximum_number_of_frames: int, device,
-                filter_optical_flow: bool = True, t_begin: int = 0, t_end: Optional[int] = None):
+                filter_optical_flow: bool = True, t_begin: int = 0, t_end: Optional[int] = None,
+                decode_all: bool = True):
     """The stage-1 input producer on the device (SURVEY.md §8f rank 1): what `load_input_data_single`
     (unwrap_utils.py:105-163) returns, built frame by frame and pair by pair straight into the pixel records and the
     validity bitmaps — the eight (H, W, ., T) host tensors are never allocated.  The host decodes one image file at
     a time (PIL + the reference's float64 cv2.resize, unwrap_utils.py:124-131) and reads the RAFT .npy flows; the
     differences, the flow resize (cv2.resize-exact, swapped scale factors), the remap-exact forward/backward
     consistency masks and the packing run in libb200deflicker.so (csrc/producer.cu).  Returns (DeviceVideo,
-    frames) with `frames` the decoded (H, W, 3, T) fp32 host tensor the PSNR of evaluate.py:740-743 needs."""
+    frames) with `frames` the decoded (H, W, 3, T) fp32 host tensor the PSNR of evaluate.py:740-743 needs.
+    With `decode_all` False only the resident frames [t_begin, t_end) are decoded and `frames` is None: a frame
+    shard's evaluation reads its frames from the records (DeviceVideo.frame_rgb)."""
     import cv2
     from pathlib import Path
     from PIL import Image
-    data_folder, vid_root = Path(data_folder), Path(vid_root)
+    vid_root = Path(vid_root)
     flow_dir = vid_root / f"{vid_name}_flow"
-    files = sorted(list(data_folder.glob("*.jpg")) + list(data_folder.glob("*.png")))
+    files = video_files(data_folder)
     T = int(min(maximum_number_of_frames, len(files)))
     t_end = T if t_end is None else t_end
     lib, st = N.lib(), N.current_stream()
@@ -148,15 +166,16 @@ def _from_files(cls, data_folder, vid_root, vid_name, resy: int, resx: int, maxi
     words = (HW * T + 31) // 32 + 1
     bits_f = torch.zeros(words, dtype=torch.int32, device=device)
     bits_b = torch.zeros(words, dtype=torch.int32, device=device)
-    frames = torch.zeros((H, W, 3, T))
+    frames = torch.zeros((H, W, 3, T)) if decode_all else None
     pin = torch.zeros(HW * 3, dtype=torch.float32).pin_memory()
     frame_dev = torch.empty(HW * 3, dtype=torch.float32, device=device)
-    for i in range(T):
+    for i in range(T) if decode_all else range(t_begin, t_end):
         im = np.array(Image.open(str(files[i]))).astype(np.float64) / 255.
         if im.ndim == 2:
             im = np.tile(im[:, :, None], [1, 1, 3])
         fr = torch.from_numpy(cv2.resize(im[:, :, :3], (W, H))).float()        # float64 -> fp32, as the reference's assignment
-        frames[:, :, :, i] = fr
+        if decode_all:
+            frames[:, :, :, i] = fr
         if t_begin <= i < t_end:
             pin.copy_(fr.reshape(-1))
             frame_dev.copy_(pin, non_blocking=True)
@@ -644,6 +663,30 @@ def psnr(a: torch.Tensor, b: torch.Tensor) -> float:
     """10 log10(1/MSE) in float64 (skimage peak_signal_noise_ratio, data_range=1; evaluate.py:740-743)."""
     err = torch.mean((a.double() - b.double()) ** 2).item()
     return float(10.0 * math.log10(1.0 / err))
+
+
+def frame_sse(video: DeviceVideo, f: int, rgb: torch.Tensor, out: Optional[torch.Tensor] = None,
+              ws: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """b200_frame_sse: float64 sum of (rgb - frame f)^2 over the H*W*3 values, with frame f read from the resident
+    records; `rgb` an (H, W, 3) fp32 device tensor.  Returns the 1-element float64 device tensor `out` (valid once the
+    stream reaches this point).  `out` and `ws` (b200_frame_sse_workspace_bytes) may be passed for graph capture."""
+    lib = N.lib()
+    rgb = rgb.contiguous()
+    if rgb.dtype != torch.float32 or rgb.numel() != video.H * video.W * 3 or rgb.device.type != "cuda":
+        raise N.B200Error(f"rgb must be an fp32 ({video.H}, {video.W}, 3) device tensor")
+    if out is None:
+        out = torch.empty(1, dtype=torch.float64, device=rgb.device)
+    if ws is None:
+        ws = torch.empty(int(lib.b200_frame_sse_workspace_bytes(video.H, video.W)), dtype=torch.uint8, device=rgb.device)
+    N.check(lib.b200_frame_sse(C.byref(video.struct), int(f), N.ptr(rgb), N.ptr(out), N.ptr(ws), ws.numel(),
+                               N.current_stream()), "b200_frame_sse")
+    return out
+
+
+def psnr_device(video: DeviceVideo, f: int, rgb: torch.Tensor) -> float:
+    """psnr(frame f, rgb) with the squared error summed on the device against frame f's resident records."""
+    sse = float(frame_sse(video, f, rgb).item())
+    return float(10.0 * math.log10(1.0 / (sse / (video.H * video.W * 3))))
 
 
 def frame_range(rank: int, world: int, T: int):

@@ -12,7 +12,7 @@ from PIL import Image
 from src.models.stage_1.core.raft import RAFT
 from src.models.stage_1.core.utils.utils import InputPadder
 
-device = torch.device("cuda:0")
+device = torch.device("cuda")      # the current device: cuda:LOCAL_RANK on a rank of a multi-GPU pre-pass
 REFINEMENT_ITERS = 20
 
 

@@ -13,6 +13,8 @@ parser.add_argument('--video_name', type=str, default=None)
 parser.add_argument('--video_frame_folder', type=str, default=None)
 parser.add_argument('--fps', type=int, default=10)
 parser.add_argument('--gpu', type=int, default=0)
+parser.add_argument('--gpus', type=int, default=1,
+                    help="run the flow pre-pass and stage 1 on this many GPUs of the node (stage 2 runs on one)")
 parser.add_argument('--class_name', type=str, default=None)
 parser.add_argument('--ckpt_filter', type=str, default="./pretrained_weights/neural_filter.pth")
 parser.add_argument('--ckpt_local', type=str, default="./pretrained_weights/local_refinement_net.pth")
@@ -63,6 +65,9 @@ if __name__ == "__main__":
         # the two-layer variant (reference test.py:39); it needs the mattes of data/test/<name>_seg
         stage1 = [sys.executable, os.path.join(HERE, "src", "stage1_neural_atlas_seg.py"), "--vid_name", name,
                   "--class_name", args.class_name, "--gpu", str(args.gpu)]
+    if args.gpus > 1:
+        # stage 1 re-runs itself under torchrun on cuda:0..N-1; stage 2 then runs on cuda:0, rank 0's device
+        stage1 += ["--gpus", str(args.gpus)]
     rc = subprocess.call(stage1)
     if rc != 0:
         sys.exit(rc)

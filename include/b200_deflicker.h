@@ -499,6 +499,19 @@ int b200_eval_maps(const B200MlpDesc* mapping, const float* mapping_params, cons
                    float* flow_error, void* ws, int64_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Squared error of one rendered frame — the numerator of the evaluation's per-frame PSNR
+ * (src/models/stage_1/evaluate.py:740-743) against the fp32 frame held in channels 0..2 of the
+ * frame's resident records.  `rgb`: (H, W, 3) fp32 on the device; `*out` (device) receives the
+ * float64 sum over the H*W*3 values of (rgb - record)^2.  The summation order depends on H*W only
+ * (per-CTA partials, then one CTA; no atomics): bit-identical across calls, graph replays and
+ * ranks, and graph-capturable.  A frame outside [t_begin, t_end) is refused with B200_ERR_INVALID,
+ * a workspace below b200_frame_sse_workspace_bytes(H, W) with B200_ERR_WORKSPACE.
+ * ------------------------------------------------------------------------------------------ */
+int64_t b200_frame_sse_workspace_bytes(int32_t H, int32_t W);
+int b200_frame_sse(const B200Video* video, int32_t frame, const float* rgb, double* out, void* ws,
+                   int64_t ws_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * RAFT correlation — replaces CorrBlock (src/models/stage_1/core/corr.py:16-64) with an all-pairs pyramid, and
  * AlternateCorrBlock (corr.py:67-91) with the on-the-fly b200_corr_alt_* calls below, which take the place of the
  * reference's unshipped alt_cuda_corr extension.
