@@ -1,9 +1,10 @@
-"""Multi-GPU launch of the flow pre-pass and the stage-1 scripts on one node.
+"""Multi-GPU launch of the flow pre-pass, the stage-1 scripts and stage 2 on one node.
 
 A script started with `--gpus N` (N > 1) and no launcher re-runs itself under `torch.distributed.run`; a script that
 finds torchrun's WORLD_SIZE / RANK / LOCAL_RANK joins an NCCL process group on cuda:LOCAL_RANK.  The helpers below are
-what every rank of such a run shares: the pair and frame blocks, one random stream, the one-time replica check and
-the per-frame values gathered in frame order.  Everything but `init` / `finish` also runs on a gloo group."""
+what every rank of such a run shares: the pair and frame blocks, one random stream, the one-time replica check, the
+per-frame values gathered in frame order and the tensors sent point to point to rank 0.  Everything but `init` /
+`finish` also runs on a gloo group."""
 from __future__ import annotations
 
 import hashlib
@@ -141,3 +142,22 @@ def collect_on_root(items, counts, numel: int, sink, device, pg=None):
         for _ in range(counts[r]):
             dist.recv(buf, src=r, group=pg)
             sink(buf.to("cpu", copy=True))          # buf is reused for the next payload
+
+
+def send_to_root(t: torch.Tensor, pg=None):
+    """Start sending the device tensor `t` to rank 0: its device buffer under NCCL, a CPU copy under gloo.  Returns
+    (work, buffer); the buffer must stay alive and unchanged until work.wait() has returned.  Under NCCL the wait makes
+    the current stream wait for the send, so the buffer's memory may then go to later work on that stream."""
+    import torch.distributed as dist
+    buf = t if dist.get_backend(pg) == "nccl" else t.cpu()
+    return dist.isend(buf, dst=0, group=pg), buf
+
+
+def recv_on_root(shape, src: int, device, pg=None, dtype=torch.float32) -> torch.Tensor:
+    """A new `dtype` tensor of `shape` on `device`, received from rank `src` (what it passed to send_to_root): into a
+    device buffer under NCCL, whose transfer the current stream then waits for, through a CPU buffer under gloo."""
+    import torch.distributed as dist
+    on_device = dist.get_backend(pg) == "nccl"
+    buf = torch.empty(shape, dtype=dtype, device=device if on_device else "cpu")
+    dist.recv(buf, src=src, group=pg)
+    return buf if on_device else buf.to(device)

@@ -14,7 +14,7 @@ parser.add_argument('--video_frame_folder', type=str, default=None)
 parser.add_argument('--fps', type=int, default=10)
 parser.add_argument('--gpu', type=int, default=0)
 parser.add_argument('--gpus', type=int, default=1,
-                    help="run the flow pre-pass and stage 1 on this many GPUs of the node (stage 2 runs on one)")
+                    help="run the flow pre-pass, stage 1 and stage 2 on this many GPUs of the node")
 parser.add_argument('--class_name', type=str, default=None)
 parser.add_argument('--ckpt_filter', type=str, default="./pretrained_weights/neural_filter.pth")
 parser.add_argument('--ckpt_local', type=str, default="./pretrained_weights/local_refinement_net.pth")
@@ -65,12 +65,13 @@ if __name__ == "__main__":
         # the two-layer variant (reference test.py:39); it needs the mattes of data/test/<name>_seg
         stage1 = [sys.executable, os.path.join(HERE, "src", "stage1_neural_atlas_seg.py"), "--vid_name", name,
                   "--class_name", args.class_name, "--gpu", str(args.gpu)]
+    stage2 = [sys.executable, os.path.join(HERE, "src", "neural_filter_and_refinement.py"), "--video_name", name,
+              "--fps", str(args.fps), "--ckpt_filter", args.ckpt_filter, "--ckpt_local", args.ckpt_local]
     if args.gpus > 1:
-        # stage 1 re-runs itself under torchrun on cuda:0..N-1; stage 2 then runs on cuda:0, rank 0's device
+        # both stages re-run themselves under torchrun on cuda:0..N-1
         stage1 += ["--gpus", str(args.gpus)]
+        stage2 += ["--gpus", str(args.gpus)]
     rc = subprocess.call(stage1)
     if rc != 0:
         sys.exit(rc)
-    sys.exit(subprocess.call([sys.executable, os.path.join(HERE, "src", "neural_filter_and_refinement.py"),
-                              "--video_name", name, "--fps", str(args.fps), "--ckpt_filter", args.ckpt_filter,
-                              "--ckpt_local", args.ckpt_local]))
+    sys.exit(subprocess.call(stage2))
