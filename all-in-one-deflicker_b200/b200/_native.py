@@ -143,6 +143,7 @@ SIGNATURES = {
     "b200_seg_workspace_bytes": (_I64, [C.POINTER(SegConfig)]),
     "b200_seg_loss_grad": (C.c_int, [C.POINTER(SegConfig), C.POINTER(Video), _P, _P, _P, _P, _P, _P, _I64, _P]),
     "b200_seg_workspace_offsets": (C.c_int, [C.POINTER(SegConfig), _P, C.POINTER(_I64)]),
+    "b200_seg_tc_image_offsets": (C.c_int, [C.POINTER(SegConfig), _P, _I32, C.POINTER(_I64)]),
     "b200_mlp_pretrain_workspace_bytes": (_I64, [C.POINTER(MlpDesc), _I32]),
     "b200_mlp_pretrain_loss_grad": (C.c_int, [C.POINTER(MlpDesc), _I32, _F, _I32, _I32, _I32, _P, _P, _P, _P, _P, C.c_int,
                                               _P, _I64, _P]),

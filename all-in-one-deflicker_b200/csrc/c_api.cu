@@ -421,13 +421,7 @@ int b200_atlas_workspace_offsets_for(const B200AtlasConfig* cfg, const B200MlpDe
 }
 
 int b200_mlp_tc_image_offsets(const B200MlpDesc* d, int64_t rows, const void* ws, int64_t* out) {
-  B200_REQUIRE(out != nullptr, "null pointer");
-  MlpShape s; TcNet net; int64_t rows_pad; TcCallPlan pl;
-  B200_PROPAGATE(tc_call_plan(d, rows, ws, &s, &net, &rows_pad, &pl));
-  const char* w = reinterpret_cast<const char*>(ws);
-  tc_single_image_offsets(s, net, rows_pad, pl.tc, w, out);
-  out[B200_TC_OFFSET_GMAX] = reinterpret_cast<char*>(pl.gmax2) - w;
-  return B200_OK;
+  return tc_call_image_offsets(d, rows, ws, ws, out);
 }
 
 int b200_atlas_tc_image_offsets_for(const B200AtlasConfig* cfg, const B200MlpDesc* mapping, const void* ws,
@@ -715,6 +709,16 @@ int mlp_forward_rows(const B200MlpDesc* d, const float* params, const float* x, 
 int mlp_backward_rows(const B200MlpDesc* d, const float* params, const float* x, const float* dy, float* dparams,
                       float* dx, const TcRows& live, int precision, void* ws, int64_t ws_bytes, cudaStream_t st) {
   return mlp_backward_impl(d, params, x, dy, dparams, dx, live.rows(), &live, precision, ws, ws_bytes, st);
+}
+
+int tc_call_image_offsets(const B200MlpDesc* d, int64_t rows, const void* call_ws, const void* origin, int64_t* out) {
+  B200_REQUIRE(out != nullptr && origin != nullptr, "null pointer");
+  MlpShape s; TcNet net; int64_t rows_pad; TcCallPlan pl;
+  B200_PROPAGATE(tc_call_plan(d, rows, call_ws, &s, &net, &rows_pad, &pl));
+  const char* w = reinterpret_cast<const char*>(origin);
+  tc_single_image_offsets(s, net, rows_pad, pl.tc, w, out);
+  out[B200_TC_OFFSET_GMAX] = reinterpret_cast<char*>(pl.gmax2) - w;
+  return B200_OK;
 }
 
 }  // namespace b200

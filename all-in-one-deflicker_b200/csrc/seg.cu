@@ -47,7 +47,15 @@ struct SegPlan {
   int64_t bytes = 0;
 };
 
-static const int kNetRows[4] = {G_COUNT, G_COUNT, A_COUNT, SEG_ATLAS_ROWS};   // row groups each network evaluates
+static const int kNetRows[4] = {G_COUNT, G_COUNT, A_COUNT, SEG_ATLAS_ROWS};   // most row groups each network evaluates
+
+// Row groups network k (mapping1, mapping2, alpha, atlas) evaluates in a trip under `cfg`: without the global rigidity
+// term the mappings' two D-offset groups are neither produced nor evaluated.  The trip's launches and the image
+// diagnostic both take their row counts from here.
+static int seg_net_groups(const B200SegConfig* cfg, int k) {
+  if (k < 2) return cfg->with_global ? G_COUNT : G_YMG;
+  return k == 2 ? A_COUNT : SEG_ATLAS_ROWS;
+}
 
 static int plan_seg(const B200SegConfig* cfg, char* base, SegPlan* pl) {
   B200_REQUIRE(cfg && cfg->batch > 0 && cfg->batch <= 16384, "samples_batch must be in [1, 16384]");
@@ -333,6 +341,18 @@ int b200_seg_workspace_offsets(const B200SegConfig* cfg, const void* ws, int64_t
   return B200_OK;
 }
 
+int b200_seg_tc_image_offsets(const B200SegConfig* cfg, const void* ws, int32_t net, int64_t* out) {
+  B200_REQUIRE(cfg && ws && out, "null pointer");
+  B200_REQUIRE(net >= 0 && net < 4, "net must be 0..3 (mapping1, mapping2, alpha, atlas), got %d", net);
+  const B200MlpDesc* descs[4] = {&cfg->mapping1, &cfg->mapping2, &cfg->alpha, &cfg->atlas};
+  SegPlan pl;
+  B200_PROPAGATE(plan_seg(cfg, reinterpret_cast<char*>(round_up(reinterpret_cast<int64_t>(ws), 1024)), &pl));
+  B200_REQUIRE(pl.net[net].prec == B200_PREC_TC, "network %d runs on the fp32 kernels under this configuration (precision "
+               "%d, tensor-core architecture %d): it has no tensor-core images", net, cfg->precision,
+               b200_mlp_tc_architecture(descs[net]));
+  return tc_call_image_offsets(descs[net], (int64_t)seg_net_groups(cfg, net) * pl.cap, pl.net[net].ws, ws, out);
+}
+
 int b200_seg_loss_grad(const B200SegConfig* cfg, const B200Video* video, const float* mask, const int64_t* indices,
                        const float* params, float* grads, float* losses, void* ws, int64_t ws_bytes, void* stream) {
   B200_REQUIRE(cfg && video && mask && indices && params && grads && losses, "null pointer");
@@ -358,8 +378,7 @@ int b200_seg_loss_grad(const B200SegConfig* cfg, const B200Video* video, const f
   geo.half_frames = (float)((double)video->T / 2.0);
   geo.d_local = cfg->derivative_amount;
   geo.d_global = cfg->global_derivative_amount;
-  // without the global rigidity term the two D-offset groups are neither produced nor evaluated
-  const int n_groups = cfg->with_global ? G_COUNT : G_YMG;
+  const int n_groups = seg_net_groups(cfg, 0);
   B200_PROPAGATE(launch_select_sample(indices, B, *video, geo, cap, n_groups, pl.counters, nullptr, pl.x_map, pl.targets, st,
                                       mask));
   const int64_t map_rows = (int64_t)n_groups * cap;
@@ -372,10 +391,9 @@ int b200_seg_loss_grad(const B200SegConfig* cfg, const B200Video* video, const f
   // live rows of each network's batch: the resident samples in every group, the compacted flow-match rows in the two
   // flow groups; the tensor-core launches visit only the tiles holding them
   TcRows live[4];
-  const int n_net_groups[4] = {n_groups, n_groups, A_COUNT, SEG_ATLAS_ROWS};
   const int g_fwd[4] = {G_FWD, G_FWD, A_FWD, -1}, g_bwd[4] = {G_BWD, G_BWD, A_BWD, -1};
   for (int k = 0; k < 4; ++k) {
-    live[k].cap = cap; live[k].groups = n_net_groups[k]; live[k].counters = pl.counters;
+    live[k].cap = cap; live[k].groups = seg_net_groups(cfg, k); live[k].counters = pl.counters;
     live[k].g_fwd = g_fwd[k]; live[k].g_bwd = g_bwd[k];
   }
   for (int k = 0; k < 3; ++k)

@@ -100,5 +100,8 @@ int tc_debug_wgrad(long long* cycles, int* shapes, int max_ctas);
 void tc_single_image_offsets(const MlpShape& sh, TcNet net, int64_t rows, char* tc_ws, const char* ws, int64_t* out);
 void tc_step_image_offsets(const MlpShape& ms, const MlpShape& as, const TcPlan& plan, bool atlas, const char* ws,
                            int64_t* out);
+// the whole vector for b200_mlp_forward / backward(d, ..., rows, B200_PREC_TC, call_ws, ...), as byte offsets from
+// `origin` (call_ws itself, or the start of a workspace that holds call_ws as a slice)
+int tc_call_image_offsets(const B200MlpDesc* d, int64_t rows, const void* call_ws, const void* origin, int64_t* out);
 
 }  // namespace b200

@@ -206,6 +206,14 @@ int b200_atlas_workspace_offsets_for(const B200AtlasConfig* cfg, const B200MlpDe
 int b200_mlp_tc_image_offsets(const B200MlpDesc* d, int64_t rows, const void* ws, int64_t* out);
 int b200_atlas_tc_image_offsets_for(const B200AtlasConfig* cfg, const B200MlpDesc* mapping,
                                     const void* ws, int32_t net, int64_t* out);
+/* The same vector for one network of a b200_seg_loss_grad(cfg, ..., ws, ...) workspace (declared
+ * with B200SegConfig below): net 0 = mapping1, 1 = mapping2, 2 = alpha, 3 = atlas.  Each network's
+ * images lie in its own slice of `ws`, planned for the rows the trip passes it (groups x cap, cap =
+ * batch rounded up to 128: 9 or, without the global rigidity term, 7 groups for the mappings, 5
+ * for alpha, 6 for the atlas); [11] is that row count.  Offsets are from `ws`.  A network the
+ * configuration runs on the fp32 kernels has no images: the call fails and says so. */
+struct B200SegConfig;
+int b200_seg_tc_image_offsets(const struct B200SegConfig* cfg, const void* ws, int32_t net, int64_t* out);
 
 /* One pre_train_mapping step (src/models/stage_1/unwrap_utils.py:182-195): rows ys / columns
  * xs (int64[batch]) of frame `frame`; gradients of the mapping block only; loss -> losses[0]. */
