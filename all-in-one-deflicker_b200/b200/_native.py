@@ -165,6 +165,13 @@ SIGNATURES = {
     "b200_corr_alt_floats": (_I64, [_I32, _I32, _I32]),
     "b200_corr_alt_build": (C.c_int, [_P, _P, _I32, _I32, _I32, _P, _P]),
     "b200_corr_alt_lookup": (C.c_int, [_P, _P, _P, _I32, _I32, _I32, _I32, _I32, _P]),
+    "b200_corr_build_batch": (C.c_int, [_P, _P, _I32, _I32, _I32, _I32, _P, _P]),
+    "b200_corr_pool_levels_batch": (C.c_int, [_P, _I32, _I32, _I32, _P]),
+    "b200_corr_build_tc_batch_workspace_bytes": (C.c_int64, [_I32, _I32, _I32, _I32]),
+    "b200_corr_build_tc_batch": (C.c_int, [_P, _P, _I32, _I32, _I32, _I32, _P, _P, C.c_int64, _P]),
+    "b200_corr_lookup_batch": (C.c_int, [_P, _P, _P, _I32, _I32, _I32, _I32, _P]),
+    "b200_corr_alt_build_batch": (C.c_int, [_P, _P, _I32, _I32, _I32, _I32, _P, _P]),
+    "b200_corr_alt_lookup_batch": (C.c_int, [_P, _P, _P, _I32, _I32, _I32, _I32, _I32, _P]),
     "b200_conv2d": (C.c_int, [C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P]),
     "b200_conv_tma_workspace_bytes": (C.c_int64, [C.POINTER(ConvDesc)]),
     "b200_conv_tma_weight_image_bytes": (C.c_int64, [C.POINTER(ConvDesc)]),

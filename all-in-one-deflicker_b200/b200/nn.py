@@ -313,26 +313,35 @@ def corr_build(fmap1, fmap2, impl="tc", out=None):
     impl 'tc': wgmma with (hi, lo) fp16 operand pairs (fp32-grade, like the reference's fp32 matmul);
     'simt': fp32 CUDA-core GEMM."""
     _check(fmap1); _check(fmap2)
-    b, c, h, w = fmap1.shape
-    if b != 1:
+    if fmap1.shape[0] != 1:
         raise N.B200Error("correlation kernels take batch 1 (the reference runs one frame pair at a time)")
+    return corr_build_batch(fmap1, fmap2, impl, out).view(-1)
+
+
+def corr_build_batch(fmap1, fmap2, impl="tc", out=None):
+    """fmaps (B, C, H8, W8) -> (B, b200_corr_pyramid_floats) pyramids, each the bits corr_build returns for its pair."""
+    _check(fmap1); _check(fmap2)
+    b, c, h, w = fmap1.shape
+    if fmap2.shape != fmap1.shape:
+        raise N.B200Error("corr_build: fmap1 and fmap2 differ in shape")
     n_pyr = int(N.lib().b200_corr_pyramid_floats(h, w))
-    pyr = out if out is not None else torch.empty(n_pyr, dtype=torch.float32, device=fmap1.device)
-    if pyr.numel() != n_pyr:
+    pyr = out if out is not None else torch.empty(b, n_pyr, dtype=torch.float32, device=fmap1.device)
+    _check(pyr)
+    if pyr.numel() != b * n_pyr:
         raise N.B200Error("corr_build: `out` has the wrong size")
     if impl == "tc":
-        nbytes = N.lib().b200_corr_build_tc_workspace_bytes(c, h, w)
+        nbytes = N.lib().b200_corr_build_tc_batch_workspace_bytes(b, c, h, w)
         if nbytes <= 0:
-            raise N.B200Error("b200_corr_build_tc_workspace_bytes: bad arguments")
+            raise N.B200Error("b200_corr_build_tc_batch_workspace_bytes: bad arguments")
         ws = torch.empty(nbytes, dtype=torch.uint8, device=fmap1.device)
-        N.check(N.lib().b200_corr_build_tc(N.ptr(fmap1), N.ptr(fmap2), c, h, w, N.ptr(pyr), N.ptr(ws), nbytes,
-                                           N.current_stream()), "b200_corr_build_tc")
+        N.check(N.lib().b200_corr_build_tc_batch(N.ptr(fmap1), N.ptr(fmap2), b, c, h, w, N.ptr(pyr), N.ptr(ws), nbytes,
+                                                 N.current_stream()), "b200_corr_build_tc_batch")
     elif impl == "simt":
-        N.check(N.lib().b200_corr_build(N.ptr(fmap1), N.ptr(fmap2), c, h, w, N.ptr(pyr), N.current_stream()),
-                "b200_corr_build")
+        N.check(N.lib().b200_corr_build_batch(N.ptr(fmap1), N.ptr(fmap2), b, c, h, w, N.ptr(pyr), N.current_stream()),
+                "b200_corr_build_batch")
     else:
         raise N.B200Error(f"unknown correlation builder {impl!r}")
-    return pyr
+    return pyr.view(b, n_pyr)
 
 
 def corr_lookup(pyr, coords, radius=4):
@@ -344,23 +353,44 @@ def corr_lookup(pyr, coords, radius=4):
     return out
 
 
+def corr_lookup_batch(pyr, coords, radius=4):
+    """coords (B, 2, H8, W8) on the (B, pyramid floats) pyramids of corr_build_batch -> (B, 4 (2r+1)^2, H8, W8), one
+    launch for the batch."""
+    _check(pyr); _check(coords)
+    b, _, h, w = coords.shape
+    if pyr.numel() != b * int(N.lib().b200_corr_pyramid_floats(h, w)):
+        raise N.B200Error("corr_lookup_batch: the pyramids were built for another batch or geometry")
+    out = torch.empty(b, 4 * (2 * radius + 1) ** 2, h, w, dtype=torch.float32, device=coords.device)
+    N.check(N.lib().b200_corr_lookup_batch(N.ptr(pyr), N.ptr(coords), N.ptr(out), b, h, w, radius, N.current_stream()),
+            "b200_corr_lookup_batch")
+    return out
+
+
 def corr_alt_build(fmap1, fmap2, out=None):
     """fmaps (1, C, H8, W8) -> the state of the on-the-fly correlation (b200_corr_alt_floats floats: fmap1 and the
     four average-pooled levels of fmap2, pixel-major).  No all-pairs volume: O(C * H8 * W8) memory."""
     _check(fmap1); _check(fmap2)
-    b, c, h, w = fmap1.shape
-    if b != 1 or fmap2.shape != fmap1.shape:
+    if fmap1.shape[0] != 1 or fmap2.shape != fmap1.shape:
         raise N.B200Error("correlation kernels take batch 1 (the reference runs one frame pair at a time)")
+    return corr_alt_build_batch(fmap1, fmap2, out).view(-1)
+
+
+def corr_alt_build_batch(fmap1, fmap2, out=None):
+    """fmaps (B, C, H8, W8) -> (B, b200_corr_alt_floats) states, each the bits corr_alt_build returns for its pair."""
+    _check(fmap1); _check(fmap2)
+    b, c, h, w = fmap1.shape
+    if fmap2.shape != fmap1.shape:
+        raise N.B200Error("corr_alt_build: fmap1 and fmap2 differ in shape")
     n = int(N.lib().b200_corr_alt_floats(c, h, w))
     if n <= 0:
         raise N.B200Error(f"corr_alt_build: feature maps of {c} channels at {h}x{w} are not supported")
-    state = out if out is not None else torch.empty(n, dtype=torch.float32, device=fmap1.device)
+    state = out if out is not None else torch.empty(b, n, dtype=torch.float32, device=fmap1.device)
     _check(state)
-    if state.numel() != n:
+    if state.numel() != b * n:
         raise N.B200Error("corr_alt_build: `out` has the wrong size")
-    N.check(N.lib().b200_corr_alt_build(N.ptr(fmap1), N.ptr(fmap2), c, h, w, N.ptr(state), N.current_stream()),
-            "b200_corr_alt_build")
-    return state
+    N.check(N.lib().b200_corr_alt_build_batch(N.ptr(fmap1), N.ptr(fmap2), b, c, h, w, N.ptr(state), N.current_stream()),
+            "b200_corr_alt_build_batch")
+    return state.view(b, n)
 
 
 def corr_alt_lookup(state, coords, dim, radius=4):
@@ -373,6 +403,18 @@ def corr_alt_lookup(state, coords, dim, radius=4):
     out = torch.empty(b, 4 * (2 * radius + 1) ** 2, h, w, dtype=torch.float32, device=coords.device)
     N.check(N.lib().b200_corr_alt_lookup(N.ptr(state), N.ptr(coords), N.ptr(out), dim, b, h, w, radius,
                                          N.current_stream()), "b200_corr_alt_lookup")
+    return out
+
+
+def corr_alt_lookup_batch(state, coords, dim, radius=4):
+    """corr_alt_lookup for B pairs at once: coords (B, 2, H8, W8) on the (B, floats) states of corr_alt_build_batch."""
+    _check(state); _check(coords)
+    b, _, h, w = coords.shape
+    if state.numel() != b * int(N.lib().b200_corr_alt_floats(dim, h, w)):
+        raise N.B200Error("corr_alt_lookup_batch: the states were built for another batch or geometry")
+    out = torch.empty(b, 4 * (2 * radius + 1) ** 2, h, w, dtype=torch.float32, device=coords.device)
+    N.check(N.lib().b200_corr_alt_lookup_batch(N.ptr(state), N.ptr(coords), N.ptr(out), dim, b, h, w, radius,
+                                               N.current_stream()), "b200_corr_alt_lookup_batch")
     return out
 
 

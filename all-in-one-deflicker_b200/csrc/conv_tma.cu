@@ -823,9 +823,21 @@ int64_t b200_corr_build_tc_workspace_bytes(int32_t dim, int32_t H8, int32_t W8) 
   return 2 * g.pack_bytes + 2 * (int64_t)g.n_tiles_n * g.n_chunks * g.n_tile * 128 + corr_pooled_floats(dim, H8, W8) * 4 + 2048;
 }
 
+int64_t b200_corr_build_tc_batch_workspace_bytes(int32_t batch, int32_t dim, int32_t H8, int32_t W8) {
+  return batch >= 1 ? b200_corr_build_tc_workspace_bytes(dim, H8, W8) : -1;   // the samples reuse one workspace
+}
+
 int b200_corr_build_tc(const float* fmap1, const float* fmap2, int32_t dim, int32_t H8, int32_t W8, float* pyramid,
                        void* workspace, int64_t workspace_bytes, void* stream) {
-  B200_REQUIRE(fmap1 && fmap2 && pyramid && workspace && dim > 0 && H8 >= 8 && W8 >= 8, "bad arguments");
+  return b200_corr_build_tc_batch(fmap1, fmap2, 1, dim, H8, W8, pyramid, workspace, workspace_bytes, stream);
+}
+
+// B pairs, one after the other in one workspace (stream order serialises them): each sample's fmap1 becomes its own
+// weight images, so a sample's launches are exactly the single-pair ones and conv2d_tma_kernel is not re-instantiated.
+// At 640x360 one sample's level-0 GEMM already fills the device (~675 tiles).
+int b200_corr_build_tc_batch(const float* fmap1, const float* fmap2, int32_t batch, int32_t dim, int32_t H8, int32_t W8,
+                             float* pyramid, void* workspace, int64_t workspace_bytes, void* stream) {
+  B200_REQUIRE(fmap1 && fmap2 && pyramid && workspace && batch >= 1 && dim > 0 && H8 >= 8 && W8 >= 8, "bad arguments");
   if (!b200_device_supports_tc()) { set_error("b200_corr_build_tc needs a compute-capability 9.x device"); return B200_ERR_UNSUPPORTED; }
   B200ConvDesc d; corr_desc(dim, H8, W8, &d);
   TmaGeom g;
@@ -836,28 +848,34 @@ int b200_corr_build_tc(const float* fmap1, const float* fmap2, int32_t dim, int3
   char* base = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
   char* images = base + 2 * g.pack_bytes;                  // pack_bytes is a multiple of 128
   const int HW = H8 * W8;
-  if (int rc = launch_weight_images(&d, g, fmap1, /*co*/ 1, /*ci*/ HW, /*tap*/ 0, 16.0f, 1, images, st)) return rc;
-  if (int rc = launch_conv_tma(&d, g, fmap2, base, images, nullptr, nullptr, pyramid, 1, 16.0f, st)) return rc;
-  // Levels 1..3 (corr.py:27-31: avg_pool2d of the previous level over the TARGET pixel grid).  Average pooling is linear
-  // in fmap2, so level l = fmap1^T . avgpool^l(fmap2): three small GEMMs on pooled 33 MB feature maps with the same
-  // fmap1 weight images, instead of three passes that re-read the 4.2 GB level-0 volume (1.7 of 3.5 ms at 1080p).
+  const int64_t fmap_floats = (int64_t)dim * HW, pyr_floats = b200_corr_pyramid_floats(H8, W8);
   const int64_t image_bytes = 2 * (int64_t)g.n_tiles_n * g.n_chunks * g.n_tile * 128;
-  float* pooled = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(images + image_bytes) + 255) & ~(uintptr_t)255);
-  const float* src = fmap2;
-  float* out = pyramid + (int64_t)HW * HW;
-  int h = H8, w = W8;
-  for (int l = 1; l < 4; ++l) {
-    if (int rc = launch_avgpool2(src, pooled, dim, h, w, st)) return rc;
-    h /= 2; w /= 2;
-    if (h < 1 || w < 1) break;
-    B200ConvDesc dl = d;
-    dl.H = h; dl.W = w;                                   // queries (output channels) stay at full resolution
-    TmaGeom gl;
-    if (int rc = tma_geometry(&dl, &gl)) return rc;
-    if (int rc = launch_conv_tma(&dl, gl, pooled, base, images, nullptr, nullptr, out, 1, 16.0f, st)) return rc;
-    out += (int64_t)HW * h * w;
-    src = pooled;
-    pooled += (((int64_t)dim * h * w + 63) / 64) * 64;
+  for (int b = 0; b < batch; ++b) {
+    const float* f1 = fmap1 + b * fmap_floats;
+    const float* f2 = fmap2 + b * fmap_floats;
+    float* pyr = pyramid + b * pyr_floats;
+    if (int rc = launch_weight_images(&d, g, f1, /*co*/ 1, /*ci*/ HW, /*tap*/ 0, 16.0f, 1, images, st)) return rc;
+    if (int rc = launch_conv_tma(&d, g, f2, base, images, nullptr, nullptr, pyr, 1, 16.0f, st)) return rc;
+    // Levels 1..3 (corr.py:27-31: avg_pool2d of the previous level over the TARGET pixel grid).  Average pooling is
+    // linear in fmap2, so level l = fmap1^T . avgpool^l(fmap2): three small GEMMs on pooled 33 MB feature maps with the
+    // same fmap1 weight images, instead of three passes that re-read the 4.2 GB level-0 volume (1.7 of 3.5 ms at 1080p).
+    float* pooled = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(images + image_bytes) + 255) & ~(uintptr_t)255);
+    const float* src = f2;
+    float* out = pyr + (int64_t)HW * HW;
+    int h = H8, w = W8;
+    for (int l = 1; l < 4; ++l) {
+      if (int rc = launch_avgpool2(src, pooled, dim, h, w, st)) return rc;
+      h /= 2; w /= 2;
+      if (h < 1 || w < 1) break;
+      B200ConvDesc dl = d;
+      dl.H = h; dl.W = w;                                   // queries (output channels) stay at full resolution
+      TmaGeom gl;
+      if (int rc = tma_geometry(&dl, &gl)) return rc;
+      if (int rc = launch_conv_tma(&dl, gl, pooled, base, images, nullptr, nullptr, out, 1, 16.0f, st)) return rc;
+      out += (int64_t)HW * h * w;
+      src = pooled;
+      pooled += (((int64_t)dim * h * w + 63) / 64) * 64;
+    }
   }
   return B200_OK;
 }

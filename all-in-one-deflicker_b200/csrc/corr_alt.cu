@@ -28,9 +28,12 @@ static int64_t alt_smem_bytes(int radius) {
   return ((int64_t)ALT_TQ * wm * wm + ALT_TQ * ALT_CS + ALT_UMAX * ALT_CS) * 4;
 }
 
-// [dim][n] (channel-major encoder output) -> [n][dim]
-__global__ void alt_transpose_kernel(const float* __restrict__ x, float* __restrict__ y, int dim, int64_t n) {
+// [dim][n] (channel-major encoder output) -> [n][dim]; sample blockIdx.z of x is x_stride floats on, of y y_stride
+__global__ void alt_transpose_kernel(const float* __restrict__ x, float* __restrict__ y, int dim, int64_t n,
+                                     int64_t x_stride, int64_t y_stride) {
   __shared__ float t[32][33];
+  x += blockIdx.z * x_stride;
+  y += blockIdx.z * y_stride;
   const int64_t p0 = (int64_t)blockIdx.x * 32;
   const int c0 = blockIdx.y * 32;
   for (int k = threadIdx.y; k < 32; k += 8) {
@@ -46,9 +49,12 @@ __global__ void alt_transpose_kernel(const float* __restrict__ x, float* __restr
   }
 }
 
-// level l from level l-1, both pixel-major: F.avg_pool2d(2, stride=2) with avgpool2_kernel's (a + b + c + d) * 0.25
-__global__ void alt_pool_kernel(const float* __restrict__ x, float* __restrict__ y, int dim, int H, int W) {
+// level l from level l-1, both pixel-major: F.avg_pool2d(2, stride=2) with avgpool2_kernel's (a + b + c + d) * 0.25;
+// sample blockIdx.y is `stride` floats on in both
+__global__ void alt_pool_kernel(const float* __restrict__ x, float* __restrict__ y, int dim, int H, int W, int64_t stride) {
   const int OH = H / 2, OW = W / 2;
+  x += blockIdx.y * stride;
+  y += blockIdx.y * stride;
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (int64_t)OH * OW * dim) return;
   const int c = (int)(i % dim);
@@ -60,11 +66,12 @@ __global__ void alt_pool_kernel(const float* __restrict__ x, float* __restrict__
 }
 
 struct AltArgs {
-  const float* f1;               // [H1*W1][dim]
+  const float* f1;               // [H1*W1][dim]  (sample 0; sample b's state is b * state_floats further on)
   const float* level[4];         // [LH*LW][dim]
   int LH[4], LW[4];
-  const float* coords;           // [1][2][H1][W1]  (x, y)
-  float* out;                    // [1][4*(2r+1)^2][H1][W1]
+  int64_t state_floats;          // b200_corr_alt_floats(dim, H1, W1)
+  const float* coords;           // [B][2][H1][W1]  (x, y)
+  float* out;                    // [B][4*(2r+1)^2][H1][W1]
   int H1, W1, dim, radius;
   float scale;                   // 1 / sqrt(dim)
 };
@@ -121,7 +128,7 @@ __device__ __forceinline__ void alt_row_chunk(const float4 (&f)[4], const float*
   }
 }
 
-// One CTA = a 16x4 tile of query pixels at one level.
+// One CTA = a 16x4 tile of query pixels at one level (blockIdx.y) of one sample (blockIdx.z).
 //  1. each query pixel's window: the integer positions its taps' corners touch (floor of the first and the last tap's
 //     coordinate, one more; at most 2r+4 per axis), clipped to the level;
 //  2. the dot products at those positions, 16 channels at a time: fmap1 chunks of the tile, and the union of the
@@ -144,7 +151,11 @@ __global__ void __launch_bounds__(ALT_THREADS) corr_alt_lookup_kernel(AltArgs a)
   const int64_t plane = (int64_t)a.H1 * a.W1;
   const int W = a.LW[l], H = a.LH[l];
   const float inv = 1.0f / (float)(1 << l);
-  const float* lvl = a.level[l];
+  const int64_t sample = (int64_t)blockIdx.z * a.state_floats;
+  const float* f1 = a.f1 + sample;
+  const float* lvl = a.level[l] + sample;
+  const float* coords = a.coords + (int64_t)blockIdx.z * 2 * plane;
+  float* out = a.out + (int64_t)blockIdx.z * 4 * taps * plane;
   if (threadIdx.x == 0) { s_u[0] = s_u[1] = INT_MAX; s_u[2] = s_u[3] = INT_MIN; }
   __syncthreads();
   if (threadIdx.x < ALT_TQ) {
@@ -153,7 +164,7 @@ __global__ void __launch_bounds__(ALT_THREADS) corr_alt_lookup_kernel(AltArgs a)
     float cx = 0.f, cy = 0.f;
     if (px < a.W1 && py < a.H1) {
       const int64_t pix = (int64_t)py * a.W1 + px;
-      cx = a.coords[pix]; cy = a.coords[plane + pix];
+      cx = coords[pix]; cy = coords[plane + pix];
       const float x0 = alt_sample(cx, inv, -r, W), x1 = alt_sample(cx, inv, r, W);
       const float y0 = alt_sample(cy, inv, -r, H), y1 = alt_sample(cy, inv, r, H);
       if (isfinite(x0) && isfinite(x1) && isfinite(y0) && isfinite(y1)) {
@@ -180,7 +191,7 @@ __global__ void __launch_bounds__(ALT_THREADS) corr_alt_lookup_kernel(AltArgs a)
         static_assert(ALT_TQ * 4 == ALT_THREADS, "one float4 of the fmap1 chunk per thread");
         const int p = threadIdx.x >> 2, k = threadIdx.x & 3, px = tx0 + p % ALT_TX, py = ty0 + p / ALT_TX;
         float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (px < a.W1 && py < a.H1) v = __ldg(reinterpret_cast<const float4*>(a.f1 + ((int64_t)py * a.W1 + px) * dim + c0) + k);
+        if (px < a.W1 && py < a.H1) v = __ldg(reinterpret_cast<const float4*>(f1 + ((int64_t)py * a.W1 + px) * dim + c0) + k);
         reinterpret_cast<float4*>(sf1 + p * ALT_CS)[k] = v;
       }
       if (staged) {
@@ -214,7 +225,7 @@ __global__ void __launch_bounds__(ALT_THREADS) corr_alt_lookup_kernel(AltArgs a)
     const int64_t pix = (int64_t)py * a.W1 + px;
     const int i = tap / wn, j = tap % wn;
     const float ix = alt_sample(s_cx[p], inv, i - r, W), iy = alt_sample(s_cy[p], inv, j - r, H);
-    float* dst = a.out + (int64_t)(l * taps + tap) * plane + pix;
+    float* dst = out + (int64_t)(l * taps + tap) * plane + pix;
     if (!isfinite(ix) || !isfinite(iy)) { *dst = nanf(""); continue; }
     const float fx0 = floorf(ix), fy0 = floorf(iy);
     const float tx = ix - fx0, ty = iy - fy0;
@@ -223,7 +234,7 @@ __global__ void __launch_bounds__(ALT_THREADS) corr_alt_lookup_kernel(AltArgs a)
       if (!(xf >= 0.f && xf <= (float)(W - 1) && yf >= 0.f && yf <= (float)(H - 1))) return 0.f;   // zero padding
       const int xi = (int)xf, yi = (int)yf, dx = xi - wx, dy = yi - wy;
       if (dx >= 0 && dx < nx && dy >= 0 && dy < ny) return sdot[(dy * wm + dx) * ALT_TQ + p] * a.scale;
-      return alt_dot_global(a.f1 + pix * a.dim, lvl + ((int64_t)yi * W + xi) * a.dim, a.dim) * a.scale;
+      return alt_dot_global(f1 + pix * a.dim, lvl + ((int64_t)yi * W + xi) * a.dim, a.dim) * a.scale;
     };
     const float nw = at(fy0, fx0), ne = at(fy0, fx0 + 1.f), sw = at(fy0 + 1.f, fx0), se = at(fy0 + 1.f, fx0 + 1.f);
     *dst = nw * ((1.f - tx) * (1.f - ty)) + ne * (tx * (1.f - ty)) + sw * ((1.f - tx) * ty) + se * (tx * ty);
@@ -269,22 +280,30 @@ int64_t b200_corr_alt_floats(int32_t dim, int32_t H8, int32_t W8) {
 
 int b200_corr_alt_build(const float* fmap1, const float* fmap2, int32_t dim, int32_t H8, int32_t W8, float* state,
                         void* stream) {
+  return b200_corr_alt_build_batch(fmap1, fmap2, 1, dim, H8, W8, state, stream);
+}
+
+int b200_corr_alt_build_batch(const float* fmap1, const float* fmap2, int32_t batch, int32_t dim, int32_t H8, int32_t W8,
+                              float* state, void* stream) {
   int64_t off[5];
   B200_REQUIRE(fmap1 && fmap2 && state, "b200_corr_alt_build: null pointer");
-  B200_REQUIRE(alt_layout(dim, H8, W8, off) > 0, "b200_corr_alt_build: dim must be a positive multiple of %d and H8, W8 >= 8 "
+  B200_REQUIRE(batch >= 1 && batch <= 65535, "b200_corr_alt_build: batch must be 1..65535 (got %d)", batch);
+  const int64_t floats = alt_layout(dim, H8, W8, off);
+  B200_REQUIRE(floats > 0, "b200_corr_alt_build: dim must be a positive multiple of %d and H8, W8 >= 8 "
                "(got dim %d, %dx%d)", ALT_CC, dim, H8, W8);
   B200_REQUIRE(reinterpret_cast<uintptr_t>(state) % 16 == 0, "b200_corr_alt_build: state must be 16-byte aligned");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int64_t n = (int64_t)H8 * W8;
-  const dim3 grid((unsigned)((n + 31) / 32), (unsigned)((dim + 31) / 32));
-  alt_transpose_kernel<<<grid, dim3(32, 8), 0, st>>>(fmap1, state + off[0], dim, n);
+  const dim3 grid((unsigned)((n + 31) / 32), (unsigned)((dim + 31) / 32), (unsigned)batch);
+  alt_transpose_kernel<<<grid, dim3(32, 8), 0, st>>>(fmap1, state + off[0], dim, n, dim * n, floats);
   B200_CHECK_LAUNCH();
-  alt_transpose_kernel<<<grid, dim3(32, 8), 0, st>>>(fmap2, state + off[1], dim, n);
+  alt_transpose_kernel<<<grid, dim3(32, 8), 0, st>>>(fmap2, state + off[1], dim, n, dim * n, floats);
   B200_CHECK_LAUNCH();
   int h = H8, w = W8;
   for (int l = 1; l < 4; ++l) {
     const int64_t total = (int64_t)(h / 2) * (w / 2) * dim;
-    alt_pool_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(state + off[l], state + off[l + 1], dim, h, w);
+    alt_pool_kernel<<<dim3((unsigned)((total + 255) / 256), (unsigned)batch), 256, 0, st>>>(state + off[l], state + off[l + 1],
+                                                                                          dim, h, w, floats);
     B200_CHECK_LAUNCH();
     h /= 2; w /= 2;
   }
@@ -293,12 +312,19 @@ int b200_corr_alt_build(const float* fmap1, const float* fmap2, int32_t dim, int
 
 int b200_corr_alt_lookup(const float* state, const float* coords, float* out, int32_t dim, int32_t batch, int32_t H8,
                          int32_t W8, int32_t radius, void* stream) {
+  B200_REQUIRE(batch == 1, "b200_corr_alt_lookup: batch must be 1 (got %d)", batch);
+  return b200_corr_alt_lookup_batch(state, coords, out, dim, batch, H8, W8, radius, stream);
+}
+
+int b200_corr_alt_lookup_batch(const float* state, const float* coords, float* out, int32_t dim, int32_t batch, int32_t H8,
+                               int32_t W8, int32_t radius, void* stream) {
   int64_t off[5];
   B200_REQUIRE(state && coords && out, "b200_corr_alt_lookup: null pointer");
-  B200_REQUIRE(batch == 1, "b200_corr_alt_lookup: batch must be 1 (got %d)", batch);
+  B200_REQUIRE(batch >= 1 && batch <= 65535, "b200_corr_alt_lookup: batch must be 1..65535 (got %d)", batch);
   B200_REQUIRE(radius >= 1 && radius <= ALT_MAX_RADIUS, "b200_corr_alt_lookup: radius must be 1..%d (got %d)",
                ALT_MAX_RADIUS, radius);
-  B200_REQUIRE(alt_layout(dim, H8, W8, off) > 0, "b200_corr_alt_lookup: dim must be a positive multiple of %d and "
+  const int64_t floats = alt_layout(dim, H8, W8, off);
+  B200_REQUIRE(floats > 0, "b200_corr_alt_lookup: dim must be a positive multiple of %d and "
                "H8, W8 >= 8 (got dim %d, %dx%d)", ALT_CC, dim, H8, W8);
   B200_REQUIRE(reinterpret_cast<uintptr_t>(state) % 16 == 0, "b200_corr_alt_lookup: state must be 16-byte aligned");
   B200_PROPAGATE(ensure_alt_attrs());
@@ -309,10 +335,12 @@ int b200_corr_alt_lookup(const float* state, const float* coords, float* out, in
     a.level[l] = state + off[l + 1]; a.LH[l] = h; a.LW[l] = w;
     h /= 2; w /= 2;
   }
+  a.state_floats = floats;
   a.coords = coords; a.out = out; a.H1 = H8; a.W1 = W8; a.dim = dim; a.radius = radius;
   a.scale = 1.0f / sqrtf((float)dim);
   const unsigned tiles = (unsigned)(((W8 + ALT_TX - 1) / ALT_TX) * ((H8 + ALT_TY - 1) / ALT_TY));
-  corr_alt_lookup_kernel<<<dim3(tiles, 4), ALT_THREADS, (size_t)alt_smem_bytes(radius), reinterpret_cast<cudaStream_t>(stream)>>>(a);
+  corr_alt_lookup_kernel<<<dim3(tiles, 4, (unsigned)batch), ALT_THREADS, (size_t)alt_smem_bytes(radius),
+                           reinterpret_cast<cudaStream_t>(stream)>>>(a);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }

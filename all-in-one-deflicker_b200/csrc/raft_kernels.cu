@@ -29,7 +29,8 @@ int launch_avgpool2(const float* x, float* y, int64_t planes, int H, int W, cuda
 }
 
 struct LookupArgs {
-  const float* level[4]; int LH[4], LW[4];
+  const float* level[4]; int LH[4], LW[4];   // sample 0's levels; sample b's lie sample_floats further on
+  int64_t sample_floats;    // b200_corr_pyramid_floats(H1, W1)
   const float* coords;      // [B][2][H1][W1]  (x, y)
   float* out;               // [B][4*81][H1][W1]
   int B, H1, W1, radius;
@@ -64,7 +65,7 @@ __global__ void corr_lookup_kernel(LookupArgs a) {
   const float fx0 = floorf(ix), fy0 = floorf(iy);
   const int x0 = (int)fx0, y0 = (int)fy0;
   const float tx = ix - fx0, ty = iy - fy0;
-  const float* src = a.level[l] + ((int64_t)b * plane + pix) * H * W;
+  const float* src = a.level[l] + (int64_t)b * a.sample_floats + pix * H * W;
   auto at = [&](int yy, int xx) -> float { return (xx >= 0 && xx < W && yy >= 0 && yy < H) ? __ldg(src + (int64_t)yy * W + xx) : 0.f; };
   // ATen grid_sampler_2d: nw*(1-tx)(1-ty) + ne*tx(1-ty) + sw*(1-tx)ty + se*tx*ty
   const float v = at(y0, x0) * ((1.f - tx) * (1.f - ty)) + at(y0, x0 + 1) * (tx * (1.f - ty)) +
@@ -99,7 +100,7 @@ __global__ void __launch_bounds__(256) corr_lookup_tiled_kernel(LookupArgs a) {
     const int64_t pix = pix0 + p;
     float v = 0.f;
     if (pix < plane && xx >= 0 && xx < W && yy >= 0 && yy < H)
-      v = __ldg(a.level[l] + ((int64_t)b * plane + pix) * H * W + (int64_t)yy * W + xx);
+      v = __ldg(a.level[l] + (int64_t)b * a.sample_floats + pix * H * W + (int64_t)yy * W + xx);
     win[p][k] = v;
   }
   __syncthreads();
@@ -125,7 +126,7 @@ __global__ void __launch_bounds__(256) corr_lookup_tiled_kernel(LookupArgs a) {
       nw = wp[0]; ne = wp[1]; sw = wp[LKW]; se = wp[LKW + 1];
     } else if (fabsf(fx0) < 1.0e9f && fabsf(fy0) < 1.0e9f) {
       const int x0 = (int)fx0, y0 = (int)fy0;
-      const float* src = a.level[l] + ((int64_t)b * plane + pix) * H * W;
+      const float* src = a.level[l] + (int64_t)b * a.sample_floats + pix * H * W;
       auto at = [&](int yy, int xx) -> float { return (xx >= 0 && xx < W && yy >= 0 && yy < H) ? __ldg(src + (int64_t)yy * W + xx) : 0.f; };
       nw = at(y0, x0); ne = at(y0, x0 + 1); sw = at(y0 + 1, x0); se = at(y0 + 1, x0 + 1);
     } else {
@@ -147,35 +148,59 @@ int64_t b200_corr_pyramid_floats(int32_t H8, int32_t W8) {
   return total;
 }
 
+
 int b200_corr_build(const float* fmap1, const float* fmap2, int32_t dim, int32_t H8, int32_t W8, float* pyramid, void* stream) {
-  B200_REQUIRE(fmap1 && fmap2 && pyramid && dim > 0 && H8 >= 8 && W8 >= 8, "bad arguments");
+  return b200_corr_build_batch(fmap1, fmap2, 1, dim, H8, W8, pyramid, stream);
+}
+
+int b200_corr_build_batch(const float* fmap1, const float* fmap2, int32_t batch, int32_t dim, int32_t H8, int32_t W8,
+                          float* pyramid, void* stream) {
+  B200_REQUIRE(fmap1 && fmap2 && pyramid && batch >= 1 && dim > 0 && H8 >= 8 && W8 >= 8, "bad arguments");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int HW = H8 * W8;
-  // level 0: corr[p1][p2] = <f1[:, p1], f2[:, p2]> / sqrt(dim)        (corr.py:56-64)
-  B200_PROPAGATE(simt_gemm_nn_scaled(fmap1, fmap2, pyramid, HW, HW, dim, 1.0f / sqrtf((float)dim), st));
-  return b200_corr_pool_levels(pyramid, H8, W8, stream);
+  const int64_t fmap_floats = (int64_t)dim * HW, pyr_floats = b200_corr_pyramid_floats(H8, W8);
+  for (int b = 0; b < batch; ++b) {
+    // level 0: corr[p1][p2] = <f1[:, p1], f2[:, p2]> / sqrt(dim)        (corr.py:56-64)
+    B200_PROPAGATE(simt_gemm_nn_scaled(fmap1 + b * fmap_floats, fmap2 + b * fmap_floats, pyramid + b * pyr_floats, HW, HW,
+                                       dim, 1.0f / sqrtf((float)dim), st));
+  }
+  return b200_corr_pool_levels_batch(pyramid, batch, H8, W8, stream);
 }
 
 /* levels 1..3 of the pyramid from level 0: 2x2 average pooling over the target image (corr.py:22-25) */
 int b200_corr_pool_levels(float* pyramid, int32_t H8, int32_t W8, void* stream) {
-  B200_REQUIRE(pyramid && H8 >= 8 && W8 >= 8, "bad arguments");
+  return b200_corr_pool_levels_batch(pyramid, 1, H8, W8, stream);
+}
+
+int b200_corr_pool_levels_batch(float* pyramid, int32_t batch, int32_t H8, int32_t W8, void* stream) {
+  B200_REQUIRE(pyramid && batch >= 1 && H8 >= 8 && W8 >= 8, "bad arguments");
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int HW = H8 * W8;
-  float* cur = pyramid;
-  int h = H8, w = W8;
-  for (int l = 1; l < 4; ++l) {
-    float* nxt = cur + (int64_t)HW * h * w;
-    const int64_t total = (int64_t)HW * (h / 2) * (w / 2);
-    avgpool2_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(cur, nxt, HW, h, w);
-    B200_CHECK_LAUNCH();
-    cur = nxt; h /= 2; w /= 2;
+  const int64_t pyr_floats = b200_corr_pyramid_floats(H8, W8);
+  for (int b = 0; b < batch; ++b) {
+    float* cur = pyramid + b * pyr_floats;
+    int h = H8, w = W8;
+    for (int l = 1; l < 4; ++l) {
+      float* nxt = cur + (int64_t)HW * h * w;
+      const int64_t total = (int64_t)HW * (h / 2) * (w / 2);
+      avgpool2_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(cur, nxt, HW, h, w);
+      B200_CHECK_LAUNCH();
+      cur = nxt; h /= 2; w /= 2;
+    }
   }
   return B200_OK;
 }
 
 int b200_corr_lookup(const float* pyramid, const float* coords, float* out, int32_t batch, int32_t H8, int32_t W8,
                      int32_t radius, void* stream) {
-  B200_REQUIRE(pyramid && coords && out && batch == 1 && radius >= 1 && radius <= 8, "bad arguments (batch must be 1)");
+  B200_REQUIRE(batch == 1, "bad arguments (batch must be 1)");
+  return b200_corr_lookup_batch(pyramid, coords, out, batch, H8, W8, radius, stream);
+}
+
+int b200_corr_lookup_batch(const float* pyramid, const float* coords, float* out, int32_t batch, int32_t H8, int32_t W8,
+                           int32_t radius, void* stream) {
+  B200_REQUIRE(pyramid && coords && out && batch >= 1 && batch <= 65535 && radius >= 1 && radius <= 8,
+               "bad arguments (batch 1..65535, radius 1..8)");
   LookupArgs a{};
   const float* cur = pyramid;
   int h = H8, w = W8;
@@ -183,6 +208,7 @@ int b200_corr_lookup(const float* pyramid, const float* coords, float* out, int3
     a.level[l] = cur; a.LH[l] = h; a.LW[l] = w;
     cur += (int64_t)H8 * W8 * h * w; h /= 2; w /= 2;
   }
+  a.sample_floats = b200_corr_pyramid_floats(H8, W8);
   a.coords = coords; a.out = out; a.B = batch; a.H1 = H8; a.W1 = W8; a.radius = radius;
   const int win = 2 * radius + 1;
   const int64_t total = (int64_t)batch * H8 * W8 * 4 * win * win;

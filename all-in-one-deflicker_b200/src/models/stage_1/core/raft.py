@@ -57,49 +57,66 @@ class RAFT(nn.Module):
         finally:
             K.set_conv_precision(prev)
 
-    def initialize_flow(self, img):
-        n, _, h, w = img.shape
-        c = coords_grid(n, h // 8, w // 8).to(img.device)
-        return c, c.clone()
-
     @torch.no_grad()
     def forward(self, image1, image2, iters=12, flow_init=None, upsample=True, test_mode=False):
+        """core/raft.py:93-148 for a batch of B frame pairs (B, 3, H, W); every sample's flow has the bits of the
+        same pair run alone."""
         image1 = (2 * (image1 / 255.0) - 1.0).contiguous()
         image2 = (2 * (image2 / 255.0) - 1.0).contiguous()
         with self._autocast():
             fmap1, fmap2 = self.fnet([image1, image2])
-        return self._refine(fmap1, fmap2, image1, iters, flow_init, test_mode)
+            cnet = self.cnet(image1)
+        return self._refine(fmap1, fmap2, cnet, iters, flow_init, test_mode)
 
     @torch.no_grad()
     def forward_both(self, image1, image2, iters=12):
-        """Flow 1->2 and 2->1 of one frame pair with the feature encoder run once (SURVEY §8f rank 2: the
-        reference's pre-pass, preprocess_optical_flow.py:29-30, calls the model twice and re-encodes both frames).
-        Each direction is exactly `forward(a, b, iters, test_mode=True)`: same feature maps, same arithmetic."""
-        image1 = (2 * (image1 / 255.0) - 1.0).contiguous()
-        image2 = (2 * (image2 / 255.0) - 1.0).contiguous()
-        with self._autocast():
-            fmap1, fmap2 = self.fnet([image1, image2])
-        out12 = self._refine(fmap1, fmap2, image1, iters, None, True)
-        out21 = self._refine(fmap2, fmap1, image2, iters, None, True)
-        return out12, out21
+        """Flow 1->2 and 2->1 of one frame pair: forward_sequence on the two frames."""
+        return self.forward_sequence(torch.cat([image1, image2]), iters)
 
-    def _refine(self, fmap1, fmap2, image1, iters, flow_init, test_mode):
-        """core/raft.py:109-148.  In test mode the `iters` refinement iterations (lookup -> update block -> coordinate
-        update, ~100 launches each plus tensor glue) are captured once per geometry in ONE CUDA graph and replayed:
-        the correlation block's state (pyramid or feature-map levels), hidden state, context and coordinates live in
-        buffers owned by this module."""
+    @torch.no_grad()
+    def forward_sequence(self, images, iters=12, pad_to=None):
+        """K + 1 consecutive frames (K + 1, 3, H, W) -> ((flow_low, flow_up) of the K forward flows k -> k + 1,
+        (flow_low, flow_up) of the K backward flows k + 1 -> k), each (K, 2, ...).  fnet and cnet run once per frame
+        (the reference's pre-pass, preprocess_optical_flow.py:29-30, encodes each interior frame four times), and the 2K
+        refinements run as one batch in the captured graph.  Each flow is `forward(a, b, iters, test_mode=True)` bit
+        for bit.  `pad_to`: refine a batch of 2 * pad_to flows (>= K; the extra ones repeat the last flow and are
+        dropped), so that a shorter window reuses the graph, and its correlation buffer, of the full-length one."""
+        k = images.shape[0] - 1
+        if k < 1:
+            raise ValueError("forward_sequence needs at least two frames")
+        kp = k if pad_to is None else pad_to
+        if kp < k:
+            raise ValueError(f"pad_to={pad_to} is smaller than the {k} pairs given")
+        x = (2 * (images / 255.0) - 1.0).contiguous()
+        with self._autocast():
+            fmaps = self.fnet(x)
+            ctx = self.cnet(x)
+        fmap1 = torch.cat([fmaps[:-1], fmaps[1:]])
+        fmap2 = torch.cat([fmaps[1:], fmaps[:-1]])
+        cnet = torch.cat([ctx[:-1], ctx[1:]])
+        del fmaps, ctx                             # the refinement's peak memory holds only the batched copies
+        if kp > k:
+            fmap1, fmap2, cnet = (torch.cat([t, t[-1:].expand(2 * (kp - k), *t.shape[1:])]) for t in (fmap1, fmap2, cnet))
+        lo, up = self._refine(fmap1, fmap2, cnet, iters, None, True)
+        return (lo[:k], up[:k]), (lo[k:2 * k], up[k:2 * k])
+
+    def _refine(self, fmap1, fmap2, cnet, iters, flow_init, test_mode):
+        """core/raft.py:109-148 from the feature maps and the context encoder's output.  In test mode the `iters`
+        refinement iterations (lookup -> update block -> coordinate update, ~100 launches each plus tensor glue) are
+        captured once per geometry (batch included) in ONE CUDA graph and replayed: the correlation block's state
+        (pyramids or feature-map levels), hidden state, context and coordinates live in buffers owned by this module."""
         use_graph = test_mode and getattr(self.args, "cuda_graph", True) and fmap1.is_cuda
-        block = corr_block_class(self.args, fmap1.shape[-2], fmap1.shape[-1],
+        n, _, h8, w8 = fmap1.shape
+        block = corr_block_class(self.args, h8, w8,
                                  torch.cuda.get_device_properties(fmap1.device).total_memory if fmap1.is_cuda else None)
         key = (tuple(fmap1.shape), int(iters), fmap1.device, block)
         st = self._graph_state.get(key) if use_graph else None
         corr_fn = block(fmap1.float(), fmap2.float(), radius=self.args.corr_radius,
                         out=st["corr"] if st is not None else None)
-        with self._autocast():
-            cnet = self.cnet(image1)
         net, inp = torch.split(cnet, [self.hidden_dim, self.context_dim], dim=1)
         net, inp = torch.tanh(net).contiguous(), torch.relu(inp).contiguous()
-        coords0, coords1 = self.initialize_flow(image1)
+        coords0 = coords_grid(n, h8, w8).to(fmap1.device)
+        coords1 = coords0.clone()
         if flow_init is not None:
             coords1 = coords1 + flow_init
         if use_graph:

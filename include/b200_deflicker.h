@@ -525,32 +525,49 @@ int b200_frame_sse(const B200Video* video, int32_t frame, const float* rgb, doub
  * reference's unshipped alt_cuda_corr extension.
  * fmaps: [dim][H8*W8] fp32 (batch 1).  pyramid: level 0 [H8*W8][H8][W8], then 3 avg-pooled levels,
  * b200_corr_pyramid_floats() floats in total.
+ * The *_batch forms take B pairs: fmaps [B][dim][H8*W8], pyramids [B][b200_corr_pyramid_floats(H8, W8)], coords
+ * [B][2][H8][W8], outputs [B][4*(2r+1)^2][H8][W8].  Every sample's bits equal those of the single-pair call on it;
+ * the single-pair calls are their B = 1 case (and refuse any other batch).  Lookups run the batch in one launch.
  * ------------------------------------------------------------------------------------------ */
 int64_t b200_corr_pyramid_floats(int32_t H8, int32_t W8);
 int b200_corr_build(const float* fmap1, const float* fmap2, int32_t dim, int32_t H8, int32_t W8,
                     float* pyramid, void* stream);
-/* CorrBlock.__call__ (corr.py:33-54): coords [1][2][H8][W8] (x, y) -> out [1][4*(2r+1)^2][H8][W8] */
+int b200_corr_build_batch(const float* fmap1, const float* fmap2, int32_t batch, int32_t dim, int32_t H8, int32_t W8,
+                          float* pyramid, void* stream);
 /* levels 1..3 from level 0 (2x2 average pooling over the target image, corr.py:22-25); called by both builders */
 int b200_corr_pool_levels(float* pyramid, int32_t H8, int32_t W8, void* stream);
+int b200_corr_pool_levels_batch(float* pyramid, int32_t batch, int32_t H8, int32_t W8, void* stream);
 /* Tensor-core builder: level 0 on wgmma with both feature maps split into (hi, lo) fp16 pairs (3 products per
  * element, fp32 accumulation: fp32-grade like the reference's fp32 matmul), operands fed by TMA; then the pooling.
- * workspace: b200_corr_build_tc_workspace_bytes(dim, H8, W8) bytes. */
+ * workspace: b200_corr_build_tc_workspace_bytes(dim, H8, W8) bytes.  The batched form builds the samples one after
+ * the other in the same workspace: b200_corr_build_tc_batch_workspace_bytes(batch, dim, H8, W8) bytes. */
 int64_t b200_corr_build_tc_workspace_bytes(int32_t dim, int32_t H8, int32_t W8);
 int b200_corr_build_tc(const float* fmap1, const float* fmap2, int32_t dim, int32_t H8, int32_t W8, float* pyramid,
                        void* workspace, int64_t workspace_bytes, void* stream);
+int64_t b200_corr_build_tc_batch_workspace_bytes(int32_t batch, int32_t dim, int32_t H8, int32_t W8);
+int b200_corr_build_tc_batch(const float* fmap1, const float* fmap2, int32_t batch, int32_t dim, int32_t H8, int32_t W8,
+                             float* pyramid, void* workspace, int64_t workspace_bytes, void* stream);
+/* CorrBlock.__call__ (corr.py:33-54): coords [1][2][H8][W8] (x, y) -> out [1][4*(2r+1)^2][H8][W8]; radius 1..8 */
 int b200_corr_lookup(const float* pyramid, const float* coords, float* out, int32_t batch,
                      int32_t H8, int32_t W8, int32_t radius, void* stream);
+int b200_corr_lookup_batch(const float* pyramid, const float* coords, float* out, int32_t batch,
+                           int32_t H8, int32_t W8, int32_t radius, void* stream);
 /* On-the-fly correlation (AlternateCorrBlock): no all-pairs volume.  The state holds fmap1 and fmap2's four 2x2
  * average-pooled levels, pixel-major ([pixels][dim]): b200_corr_alt_floats(dim, H8, W8) floats (-1 for a geometry
  * the kernels do not take: dim a positive multiple of 16, H8, W8 >= 8), 16-byte aligned, owned by the caller.
  * The lookup forms each window's dot products / sqrt(dim) when it is looked up and returns what b200_corr_lookup
  * returns on the pyramid of the same fmaps, up to fp32 rounding (layout, taps, padding, NaN rules are the same);
- * batch 1, radius 1..8.  Both calls are stream-ordered, allocate nothing and can be captured in a CUDA graph. */
+ * batch 1, radius 1..8.  Both calls are stream-ordered, allocate nothing and can be captured in a CUDA graph.
+ * The *_batch forms take B pairs with states [B][b200_corr_alt_floats(dim, H8, W8)], one launch per kernel. */
 int64_t b200_corr_alt_floats(int32_t dim, int32_t H8, int32_t W8);
 int b200_corr_alt_build(const float* fmap1, const float* fmap2, int32_t dim, int32_t H8, int32_t W8, float* state,
                         void* stream);
 int b200_corr_alt_lookup(const float* state, const float* coords, float* out, int32_t dim, int32_t batch, int32_t H8,
                          int32_t W8, int32_t radius, void* stream);
+int b200_corr_alt_build_batch(const float* fmap1, const float* fmap2, int32_t batch, int32_t dim, int32_t H8, int32_t W8,
+                              float* state, void* stream);
+int b200_corr_alt_lookup_batch(const float* state, const float* coords, float* out, int32_t dim, int32_t batch, int32_t H8,
+                               int32_t W8, int32_t radius, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Convolution and image operators of the RAFT update block (core/update.py:6-136) and of the
