@@ -4,6 +4,12 @@
 // (`get_optical_flow_loss_all`, loss_utils.py:283-295 with get_corresponding_flow_matches_all :360-382).
 // Four mapping evaluations per pixel — (x, y, t), (x, y-d, t), (x-d, y, t), (x+fx, y+fy, t+1) — as four row groups of
 // ONE b200_mlp_forward call, then one head kernel.
+//
+// The time coordinate of the first group is the render's (evaluate.py:656: a Python double, f / (T / 2.0) - 1, times an
+// fp32 ones_like): that group's output IS the reconstruction's uv_temp1, which the dashboards show and the rigidity
+// and flow terms subtract from.  The other three groups are built inside the loss functions from int64 frame indices
+// (loss_utils.py:232, :376-378), so their time goes through the fp32 division of norm_coord.  The two roundings differ
+// for many frames (T = 80: 36 of them, frame 78 among them).
 #include "atlas_internal.cuh"
 #include "loss_math.h"
 
@@ -12,7 +18,7 @@ namespace b200 {
 static char* carve_ev(char*& p, int64_t bytes) { char* r = p; p += round_up(bytes, 256); return r; }
 
 __global__ void eval_rows_kernel(B200Video vid, int frame, int64_t pix_begin, int64_t count, int64_t rows_pad, float hL,
-                                 float hT, float d, float* __restrict__ x3, float* __restrict__ valid) {
+                                 float hT, float t_render, float d, float* __restrict__ x3, float* __restrict__ valid) {
   const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= rows_pad) return;
   float r[4][3];
@@ -25,7 +31,7 @@ __global__ void eval_rows_kernel(B200Video vid, int frame, int64_t pix_begin, in
     const float fx = (float)x, fy = (float)y, ft = (float)frame;
     const float tn = norm_coord(ft, hT);
     const float* rec = vid.records + (((int64_t)(frame - vid.t_begin) * vid.H + y) * vid.W + x) * B200_RECORD_FLOATS;
-    r[0][0] = norm_coord(fx, hL); r[0][1] = norm_coord(fy, hL); r[0][2] = tn;
+    r[0][0] = norm_coord(fx, hL); r[0][1] = norm_coord(fy, hL); r[0][2] = t_render;
     r[1][0] = norm_coord(fx, hL); r[1][1] = norm_coord(fy - d, hL); r[1][2] = tn;
     r[2][0] = norm_coord(fx - d, hL); r[2][1] = norm_coord(fy, hL); r[2][2] = tn;
     r[3][0] = norm_coord(__fadd_rn(fx, rec[9]), hL); r[3][1] = norm_coord(__fadd_rn(fy, rec[10]), hL);
@@ -115,8 +121,9 @@ int b200_eval_maps(const B200MlpDesc* mapping, const float* mapping_params, cons
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int larger = video->W > video->H ? video->W : video->H;
   const float hL = (float)((double)larger / 2.0), hT = (float)((double)video->T / 2.0);
+  const float t_render = (float)((double)frame / ((double)video->T / 2.0) - 1.0);     // b200_render_for's t_norm
   const int64_t rp = pl.rows_pad;
-  eval_rows_kernel<<<(unsigned)((rp + 255) / 256), 256, 0, st>>>(*video, frame, pix_begin, count, rp, hL, hT,
+  eval_rows_kernel<<<(unsigned)((rp + 255) / 256), 256, 0, st>>>(*video, frame, pix_begin, count, rp, hL, hT, t_render,
                                                                   derivative_amount, pl.x3, pl.valid);
   B200_CHECK_LAUNCH();
   const int prec = (precision == B200_PREC_TC && b200_mlp_tc_architecture(mapping) > 0) ? B200_PREC_TC : B200_PREC_FP32;

@@ -523,8 +523,9 @@ int b200_seg_render(const B200SegConfig* cfg, const float* params, int32_t H, in
                     int64_t pix_begin, int64_t pix_end, float* rgb, uint8_t* rgb_u8, float* alpha, void* ws,
                     int64_t ws_bytes, void* stream) {
   B200_REQUIRE(cfg && params && ws && (rgb || rgb_u8 || alpha), "null pointer");
-  B200_REQUIRE(H > 0 && W > 0 && T > 0 && frame >= 0 && pix_begin >= 0 && pix_end > pix_begin && pix_end <= (int64_t)H * W,
+  B200_REQUIRE(H > 0 && W > 0 && T > 0 && pix_begin >= 0 && pix_end > pix_begin && pix_end <= (int64_t)H * W,
                "bad geometry");
+  B200_REQUIRE(frame >= 0 && frame < T, "frame %d is outside the video's %d frames", frame, T);
   const int64_t count = pix_end - pix_begin;
   SegRenderPlan pl;
   char* base = reinterpret_cast<char*>(round_up(reinterpret_cast<int64_t>(ws), 1024));

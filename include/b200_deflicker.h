@@ -485,7 +485,8 @@ int b200_mlp_pretrain_loss_grad(const B200MlpDesc* d, int32_t batch, float uv_ma
 
 /* Reconstruction of the seg variant (src/models/stage_1/evaluate.py:293-335): composite
  * rgb = rgb1*alpha + rgb2*(1-alpha) and alpha for pixels [pix_begin, pix_end) of frame f.
- * rgb [count][3], rgb_u8 (may be NULL), alpha [count] (may be NULL). */
+ * rgb [count][3], rgb_u8 (may be NULL), alpha [count] (may be NULL).  A frame outside [0, T) is
+ * refused with B200_ERR_INVALID, as b200_render refuses it. */
 int64_t b200_seg_render_workspace_bytes(const B200SegConfig* cfg, int64_t pixels);
 int b200_seg_render(const B200SegConfig* cfg, const float* params, int32_t H, int32_t W, int32_t T,
                     int32_t frame, int64_t pix_begin, int64_t pix_end, float* rgb,
