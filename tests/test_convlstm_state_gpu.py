@@ -30,12 +30,11 @@ from b200 import nn as K
 from convlstm_state_common import recurrence, recurrence_inputs, transformnet_forward_state
 from csrc_build import ensure_built
 from nets_common import seeded_weights
-from test_conv_kernels_gpu import _f16, plan, spec
+from conv_common import cell_reference, convlstm_reference
+from test_conv_kernels_gpu import plan, spec
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-U = 2.0 ** -24
-C_TC = 4.0
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -90,26 +89,8 @@ def _reference(x, wt, b, state):
     """float64 (hidden, cell) on the kernel's fp16 operands, and their elementwise bounds (module docstring)."""
     c = x.shape[1]
     if state is None:
-        xin, w_ = x, wt[:, :c]
-    else:
-        xin, w_ = torch.cat((x, state[0]), 1), wt
-    x16, w16 = _f16(xin), _f16(w_)
-    z = F.conv2d(x16, w16, b.double(), padding=1)
-    a = F.conv2d(x16.abs(), w16.abs(), b.double().abs(), padding=1)
-    r = xin.shape[1] * 9
-    ez = C_TC * U * math.sqrt(r) * a + 4 * U * z.abs()
-    zi, zr, zo, zg = z.chunk(4, 1)
-    ei, er, eo, eg = ez.chunk(4, 1)
-    si, sr, so, tg = torch.sigmoid(zi), torch.sigmoid(zr), torch.sigmoid(zo), torch.tanh(zg)
-    e_in, e_rem, e_out = ei / 4 + 8 * U * si, er / 4 + 8 * U * sr, eo / 4 + 8 * U * so
-    e_g = eg + 8 * U * tg.abs()
-    cp = torch.zeros_like(si) if state is None else state[1].double()
-    cell = sr * cp + si * tg
-    e_cell = cp.abs() * e_rem + tg.abs() * e_in + si * e_g + e_in * e_g + 4 * U * ((sr * cp).abs() + (si * tg).abs())
-    tc_ = torch.tanh(cell)
-    hidden = so * tc_
-    e_hidden = tc_.abs() * e_out + so * (e_cell + 8 * U * tc_.abs()) + e_out * e_cell + 4 * U * hidden.abs()
-    return hidden, cell, e_hidden, e_cell
+        return convlstm_reference(x, wt[:, :c], b, None)
+    return convlstm_reference(torch.cat((x, state[0]), 1), wt, b, state[1])
 
 
 def _gate_case(c, n, h, w, state):
@@ -183,16 +164,7 @@ def test_fp32_cell_kernel_against_float64(with_prev):
     gates = torch.randn(n, 4 * c, h, w, generator=g) * 4
     prev = torch.randn(n, c, h, w, generator=g) * 3 if with_prev else None
     hid, cell = K.convlstm_cell(gates.to(DEV), None if prev is None else prev.to(DEV))
-    z = gates.double()
-    zi, zr, zo, zg = z.chunk(4, 1)
-    si, sr, so, tg = torch.sigmoid(zi), torch.sigmoid(zr), torch.sigmoid(zo), torch.tanh(zg)
-    cp = torch.zeros_like(si) if prev is None else prev.double()
-    e_in, e_rem, e_out, e_g = 8 * U * si, 8 * U * sr, 8 * U * so, 8 * U * tg.abs()
-    ref_c = sr * cp + si * tg
-    e_c = cp.abs() * e_rem + tg.abs() * e_in + si * e_g + 4 * U * ((sr * cp).abs() + (si * tg).abs())
-    tc_ = torch.tanh(ref_c)
-    ref_h = so * tc_
-    e_h = tc_.abs() * e_out + so * (e_c + 8 * U * tc_.abs()) + 4 * U * ref_h.abs()
+    ref_h, ref_c, e_h, e_c = cell_reference(gates.double(), torch.zeros_like(gates.double()), prev)
     for what, got, ref, e in (("cell", cell, ref_c, e_c), ("hidden", hid, ref_h, e_h)):
         err = (got.cpu().double() - ref).abs()
         print(f"fp32 cell prev={with_prev} {what}: err / bound = {float((err / e.clamp_min(1e-300)).max()):.3f}")

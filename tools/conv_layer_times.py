@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """Per-convolution CUDA-event times of the update block, UNet and TransformNet at the aux-bench sizes, for
 both convolution arithmetics.  Diagnostic only (synchronises around every call)."""
+import inspect
 import json
 import os
 import sys
@@ -22,6 +23,8 @@ def main():
     rows = []
     orig = K.conv2d
 
+    sig = inspect.signature(orig)
+
     def timed_conv(x, w, *a, **kw):
         torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -29,12 +32,22 @@ def main():
         y = orig(x, w, *a, **kw)
         e1.record()
         torch.cuda.synchronize()
-        cin = w.shape[1]
-        macs = y.shape[0] * y.shape[2] * y.shape[3] * w.shape[0] * cin * w.shape[2] * w.shape[3]
-        rows.append({"net": tag[0], "prec": K.conv_precision(), "cin": cin, "cout": w.shape[0], "k": list(w.shape[2:]),
-                     "out_hw": list(y.shape[2:]), "pad": kw.get("pad_mode", "zeros"), "up": kw.get("upsample", 1),
-                     "stride": kw.get("stride", 1), "ms": round(e0.elapsed_time(e1), 4),
-                     "tflops": round(2 * macs / e0.elapsed_time(e1) / 1e9, 1)})
+        # the output geometry comes from the arguments: a chained producer with keep_fp32=False returns None
+        p = sig.bind(x, w, *a, **kw)
+        p.apply_defaults()
+        p = p.arguments
+        chained_in = isinstance(x, K.Chain)
+        n, h, wd = (x.n, x.h, x.w) if chained_in else (x.shape[0], x.shape[2], x.shape[3])
+        ph, pw = (p["pad"], p["pad"]) if isinstance(p["pad"], int) else p["pad"]
+        cout, cin, kh, kw = w.shape
+        oh = (h * p["upsample"] + 2 * ph - kh) // p["stride"] + 1
+        ow = (wd * p["upsample"] + 2 * pw - kw) // p["stride"] + 1
+        macs = n * oh * ow * cout * cin * kh * kw
+        ms = e0.elapsed_time(e1)
+        rows.append({"net": tag[0], "prec": K.conv_precision(), "cin": cin, "cout": cout, "k": [kh, kw],
+                     "out_hw": [oh, ow], "pad": p["pad_mode"], "up": p["upsample"], "stride": p["stride"],
+                     "chained_in": chained_in, "chain_out": p["chain_out"] is not None, "ms": round(ms, 4),
+                     "tflops": round(2 * macs / ms / 1e9, 1)})
         return y
 
     K.conv2d = timed_conv
