@@ -189,6 +189,7 @@ class Worst:
         print(f"{label}: largest error / bound {self.r[where]:.3g} ({where}); weight gradients {dw[0]:.3g} ({dw[1]})")
         bad = {k: v for k, v in self.r.items() if not v <= 1.0}
         assert not bad, (label, bad)
+        return self.r[where]
 
 
 def _mm3(a_hi, a_lo, b_hi, b_lo):
@@ -352,9 +353,14 @@ def check_backward(im, net, y_dev, dy_dev, s_g, worst):
         worst.add(f"dZ{l - 1}", f64(h) + f64(lo), ref, bound)
 
 
-def check_input_gradient(im, net, s_g, d_in, worst):
+def check_input_gradient(im, net, s_g, d_in, worst, base=None):
     """The atlas: dPE = dZ_0 W_0 (64 columns) on the tensor cores, then d(in)_e = sum_k b_k (dsin c - dcos s) with
-    the partner terms of the device's encoding image."""
+    the partner terms of the device's encoding image.
+
+    base: None when the kernel overwrites d_in with d(in) (stand-alone calls), or (value, bound), float64 [n, 2]
+    tensors, when it adds its gradient into a buffer that held `value` to within an absolute `bound`: the fused step
+    adds 0.5 d(in) (its atlas input is uv * 0.5 + 0.5) into the loss head's d_uv, with one fp32 rounding of the sum.
+    An infinite bound leaves a row only the finiteness check."""
     h, lo = im.dz(0)
     b_hi, b_lo = im.w_bwd(0)
     v, a = _mm3(f64(h), f64(lo), f64(b_hi[:64]), f64(b_lo[:64]))
@@ -369,7 +375,12 @@ def check_input_gradient(im, net, s_g, d_in, worst):
         s, c = pe[:n, e:40:4], pe[:n, 2 + e:40:4]
         ref = (bk * (ds * c - dc * s)).sum(1)
         bound = (bk * (es * c.abs() + ec * s.abs())).sum(1) + _bound(20, 10, (bk * ((ds * c).abs() + (dc * s).abs())).sum(1))
-        worst.add("d_in", d_in[:, e].double(), ref, bound + 1e-300)
+        got = d_in[:, e].double()
+        if base is None:
+            worst.add("d_in", got, ref, bound + 1e-300)
+        else:
+            worst.add("d_in + head", got, base[0][:, e] + 0.5 * ref,
+                      base[1][:, e] + 0.5 * bound + U * got.abs() + 1e-300)
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -462,3 +473,93 @@ def wg_units():
     ctas = N.lib().b200_debug_wgrad(cycles, shapes, 1024)
     assert ctas > 0 and ctas % 2 == 0
     return ctas            # 2 units per cluster of 2 CTAs
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# counted trips: the tiles a launch visits, host counts, hand-built batches on a small video
+# ---------------------------------------------------------------------------------------------------------------
+SMALL = dict(T=4, H=32, W=48)
+FRAME = 1                      # the resident samples' frame: it has both flow directions, rank 0 of 2 owns it
+B_SMALL = 400
+
+
+def tiles_of(n):
+    return -(-n // TM)
+
+
+def live_tiles(cap, groups, cnt, g_fwd, g_bwd):
+    """TileIter::init / global_tile on the host: the global tile indices a counted call visits."""
+    ct = cap // TM
+    gf = g_fwd if 0 <= g_fwd < groups else -1
+    gb = g_bwd if 0 <= g_bwd < groups else -1
+    t0 = min(ct, tiles_of(cnt[0]))
+    tf = min(ct, tiles_of(cnt[5])) if gf >= 0 else t0
+    tb = min(ct, tiles_of(cnt[6])) if gb >= 0 else t0
+    return [g * ct + t for g in range(groups) for t in range(tf if g == gf else (tb if g == gb else t0))]
+
+
+def desc_dims(d):
+    """Net's dims of a B200MlpDesc."""
+    skips = tuple(l for l in range(d.num_layers) if d.skip_mask >> l & 1)
+    return (d.input_dim, d.output_dim, d.num_layers, d.pe_freqs, skips)
+
+
+def host_counts(inds, data, t0, t1, H, W):
+    """counters[0], [5], [6]: resident samples of frames [t0, t1) and those of them with a valid forward / backward
+    flow."""
+    inds = inds.reshape(-1)
+    t = inds // (H * W)
+    yx = inds % (H * W)
+    here = (t >= t0) & (t < t1)
+    wf = data["mask_fwd"][yx // W, yx % W, t, 0] != 0
+    wb = data["mask_bwd"][yx // W, yx % W, t, 0] != 0
+    return int(here.sum()), int((here & wf).sum()), int((here & wb).sum())
+
+
+def run_trip(tr, it, replay=None):
+    """One trip on a workspace filled with 0xFF (eagerly, or by replaying the CUDA graph `replay`).  `it` is what
+    the trainer's loss_grad takes: the iteration (SegTrainer) or the global-term switch (AtlasTrainer)."""
+    tr._workspace().fill_(0xFF)
+    if replay is None:
+        tr.loss_grad(it)
+    else:
+        replay.replay()
+    torch.cuda.synchronize()
+
+
+def small_data(seed=5):
+    """32 x 48 x 4 video whose frame FRAME has the four flow-validity classes in turn: pixel p has a valid forward
+    flow iff p & 1, a valid backward flow iff p & 2."""
+    T, H, W = SMALL["T"], SMALL["H"], SMALL["W"]
+    data = synth.throughput_set(H, W, T, seed=seed)
+    p = torch.arange(H * W)
+    data["mask_fwd"][:, :, FRAME, 0] = (p & 1).float().view(H, W)
+    data["mask_bwd"][:, :, FRAME, 0] = ((p >> 1) & 1).float().view(H, W)
+    masks = (torch.rand(H, W, T, generator=torch.Generator().manual_seed(seed)) < 0.4).float()
+    return data, masks
+
+
+def small_batch(n_local, n_f, n_b, seed, resident=True):
+    """B_SMALL indices: n_local distinct pixels of frame FRAME of which n_f have a valid forward and n_b a valid
+    backward flow (none when not `resident`), the rest in frames 2 and 3 (rank 1's)."""
+    T, H, W = SMALL["T"], SMALL["H"], SMALL["W"]
+    n11 = max(0, n_f + n_b - n_local)
+    per_class = {3: n11, 1: n_f - n11, 2: n_b - n11, 0: n_local - n_f - n_b + n11}
+    assert min(per_class.values()) >= 0 and max(per_class.values()) <= H * W // 4, per_class
+    pix = [c + 4 * j for c, n in per_class.items() for j in range(n)]
+    g = torch.Generator().manual_seed(seed)
+    local = torch.tensor(pix, dtype=torch.long) + FRAME * H * W
+    rest = 2 * H * W + torch.randint(2 * H * W, (B_SMALL - n_local,), generator=g)
+    inds = torch.cat((local, rest))
+    return inds[torch.randperm(B_SMALL, generator=g)]
+
+
+def flow_counts(n_local, regime):
+    """(n_f, n_b) of a small batch with n_local resident rows: no forward-flow row ("no_fwd"), every resident row
+    forward-valid ("all_fwd"), or forward rows a multiple of 128 beside backward rows that are not."""
+    if regime == "no_fwd":
+        return 0, max(1, n_local // 3)
+    if regime == "all_fwd":
+        return n_local, n_local // 2
+    n_b = max(x for x in range(n_local, 0, -1) if x % TM)
+    return n_local // TM * TM, n_b

@@ -46,9 +46,11 @@ from b200 import _native as N
 from b200 import atlas as A
 from b200 import seg as SG
 from b200 import synth
-from tc_images_common import (DEV, GMAX, OFFSETS, TM, Images, Net, Worst, _need_tc, check_backward, check_forward,
-                              check_input_gradient, check_weight_gradients, check_weight_images, grad_scale,
-                              unit_splits, wg_units, wgrad_gemms)  # noqa: F401  (wg_units: a fixture)
+from tc_images_common import (B_SMALL, DEV, FRAME, GMAX, OFFSETS, SMALL, TM, Images, Net, Worst, _need_tc,
+                              check_backward, check_forward, check_input_gradient, check_weight_gradients,
+                              check_weight_images, desc_dims, flow_counts, grad_scale, host_counts, live_tiles,
+                              run_trip, small_batch, small_data, tiles_of, unit_splits, wg_units,
+                              wgrad_gemms)  # noqa: F401  (wg_units: a fixture)
 
 pytestmark = pytest.mark.gpu
 
@@ -58,49 +60,6 @@ ROLES = {"mapping1": (3, 6, 10, 3, 5, 6), "mapping2": (3, 7, 11, 3, 5, 6), "alph
          "atlas": (5, 9, 13, 2, -1, -1)}
 D_XAT = 14
 FULL = dict(T=80, H=432, W=768, B=10000)
-SMALL = dict(T=4, H=32, W=48)
-
-
-def tiles_of(n):
-    return -(-n // TM)
-
-
-def live_tiles(cap, groups, cnt, g_fwd, g_bwd):
-    """TileIter::init / global_tile on the host: the global tile indices a counted call visits."""
-    ct = cap // TM
-    gf = g_fwd if 0 <= g_fwd < groups else -1
-    gb = g_bwd if 0 <= g_bwd < groups else -1
-    t0 = min(ct, tiles_of(cnt[0]))
-    tf = min(ct, tiles_of(cnt[5])) if gf >= 0 else t0
-    tb = min(ct, tiles_of(cnt[6])) if gb >= 0 else t0
-    return [g * ct + t for g in range(groups) for t in range(tf if g == gf else (tb if g == gb else t0))]
-
-
-def _desc_dims(d):
-    skips = tuple(l for l in range(d.num_layers) if d.skip_mask >> l & 1)
-    return (d.input_dim, d.output_dim, d.num_layers, d.pe_freqs, skips)
-
-
-def host_counts(inds, data, t0, t1, H, W):
-    """counters[0], [5], [6]: resident samples of frames [t0, t1) and those of them with a valid forward / backward
-    flow."""
-    inds = inds.reshape(-1)
-    t = inds // (H * W)
-    yx = inds % (H * W)
-    here = (t >= t0) & (t < t1)
-    wf = data["mask_fwd"][yx // W, yx % W, t, 0] != 0
-    wb = data["mask_bwd"][yx // W, yx % W, t, 0] != 0
-    return int(here.sum()), int((here & wf).sum()), int((here & wb).sum())
-
-
-def run_trip(tr, it, replay=None):
-    """One trip on a workspace filled with 0xFF (eagerly, or by replaying the CUDA graph `replay`)."""
-    tr._workspace().fill_(0xFF)
-    if replay is None:
-        tr.loss_grad(it)
-    else:
-        replay.replay()
-    torch.cuda.synchronize()
 
 
 def check_trip(tr, it, want_counts, wg_units, label):
@@ -123,7 +82,7 @@ def check_trip(tr, it, want_counts, wg_units, label):
         groups = rows // cap
         assert groups == {0: 9 if cfg.with_global else 7, 1: 9 if cfg.with_global else 7, 2: 5, 3: 6}[k]
         i_in, i_out, i_dy, cols, g_fwd, g_bwd = ROLES[which]
-        net = Net(_desc_dims(tr.descs[which]), tr.params[tr.net_slice(which)])
+        net = Net(desc_dims(tr.descs[which]), tr.params[tr.net_slice(which)])
         tiles = live_tiles(cap, groups, cnt, g_fwd, g_bwd)
         n_tiles = rows // TM
         live = torch.zeros(n_tiles, dtype=torch.bool, device=DEV)
@@ -228,37 +187,6 @@ def test_fullsize_shard_layers(fullsize, world, rank, wg_units):
 # ---------------------------------------------------------------------------------------------------------------
 # hand-built batches on a small video
 # ---------------------------------------------------------------------------------------------------------------
-FRAME = 1                      # the resident samples' frame: it has both flow directions, rank 0 of 2 owns it
-B_SMALL = 400
-
-
-def small_data(seed=5):
-    """32 x 48 x 4 video whose frame FRAME has the four flow-validity classes in turn: pixel p has a valid forward
-    flow iff p & 1, a valid backward flow iff p & 2."""
-    T, H, W = SMALL["T"], SMALL["H"], SMALL["W"]
-    data = synth.throughput_set(H, W, T, seed=seed)
-    p = torch.arange(H * W)
-    data["mask_fwd"][:, :, FRAME, 0] = (p & 1).float().view(H, W)
-    data["mask_bwd"][:, :, FRAME, 0] = ((p >> 1) & 1).float().view(H, W)
-    masks = (torch.rand(H, W, T, generator=torch.Generator().manual_seed(seed)) < 0.4).float()
-    return data, masks
-
-
-def small_batch(n_local, n_f, n_b, seed, resident=True):
-    """B_SMALL indices: n_local distinct pixels of frame FRAME of which n_f have a valid forward and n_b a valid
-    backward flow (none when not `resident`), the rest in frames 2 and 3 (rank 1's)."""
-    T, H, W = SMALL["T"], SMALL["H"], SMALL["W"]
-    n11 = max(0, n_f + n_b - n_local)
-    per_class = {3: n11, 1: n_f - n11, 2: n_b - n11, 0: n_local - n_f - n_b + n11}
-    assert min(per_class.values()) >= 0 and max(per_class.values()) <= H * W // 4, per_class
-    pix = [c + 4 * j for c, n in per_class.items() for j in range(n)]
-    g = torch.Generator().manual_seed(seed)
-    local = torch.tensor(pix, dtype=torch.long) + FRAME * H * W
-    rest = 2 * H * W + torch.randint(2 * H * W, (B_SMALL - n_local,), generator=g)
-    inds = torch.cat((local, rest))
-    return inds[torch.randperm(B_SMALL, generator=g)]
-
-
 def _small_trainer(data, masks, t0, t1, config=None, seed=7):
     cfg = {"samples_batch": B_SMALL}
     cfg.update(config or {})
@@ -269,20 +197,11 @@ def _small_trainer(data, masks, t0, t1, config=None, seed=7):
     return tr
 
 
-def _flow_counts(n_local, regime):
-    if regime == "no_fwd":
-        return 0, max(1, n_local // 3)
-    if regime == "all_fwd":
-        return n_local, n_local // 2
-    n_b = max(x for x in range(n_local, 0, -1) if x % TM)
-    return n_local // TM * TM, n_b
-
-
 @pytest.mark.parametrize("regime", ["no_fwd", "all_fwd", "fwd_whole_tiles"])
 @pytest.mark.parametrize("n_local", [1, 127, 128, 129])
 def test_small_batch_layers(n_local, regime, wg_units):
     _need_tc()
-    n_f, n_b = _flow_counts(n_local, regime)
+    n_f, n_b = flow_counts(n_local, regime)
     data, masks = small_data()
     T, H, W = SMALL["T"], SMALL["H"], SMALL["W"]
     t0, t1 = A.frame_range(0, 2, T)
