@@ -192,6 +192,14 @@ class Worst:
         return self.r[where]
 
 
+F16_MAX_BITS = 0x7BFF   # 65504: where cvt.rn.satfinite clamps
+
+
+def check_unsaturated(worst, what, hi):
+    """No hi term of an image sits at +-65504: past it the 2-term split keeps only the lo term's 11 bits."""
+    worst.exact(f"no saturated hi term in {what}", not bool(((hi & 0x7FFF) == F16_MAX_BITS).any()))
+
+
 def _mm3(a_hi, a_lo, b_hi, b_lo):
     """sum_k a_hi b_hi + a_lo b_hi + a_hi b_lo  and the same of absolute values: [R, K] x [N, K] -> [R, N]."""
     v = (a_hi + a_lo) @ b_hi.T + a_hi @ b_lo.T
@@ -273,6 +281,7 @@ def check_forward(im, net, inp, y_dev, worst, y_rows=None):
     pe_full = None
     if net.pe:
         p_hi, p_lo = im.pe()
+        check_unsaturated(worst, "the encoding", p_hi)
         ref = encoding_ref(net, inp)
         pe_full = f64(p_hi) + f64(p_lo)
         worst.add("encoding", pe_full, ref, 4 * U * ref.abs() + SPLIT * ref.abs() + FLOOR)
@@ -297,6 +306,7 @@ def check_forward(im, net, inp, y_dev, worst, y_rows=None):
             bound = _bound(K, 3 * K / 16 + 1, a / S_W + bias.abs())
         flags = im.flags(l)
         h, lo = im.act(l)
+        check_unsaturated(worst, f"h{l}", h)
         img = f64(h) + f64(lo)
         sure = z.abs() > bound
         worst.exact(f"flags of layer {l}", torch.equal(flags[sure], z[sure] > 0))
@@ -325,6 +335,7 @@ def check_backward(im, net, y_dev, dy_dev, s_g, worst):
     """y_dev, dy_dev: [R, out] fp32 output and output gradient of the decoded rows (zero in padding rows)."""
     L, out = net.L, net.out
     d_hi, d_lo = im.dzl()
+    check_unsaturated(worst, "dZ output", d_hi)
     dzl = f64(d_hi) + f64(d_lo)
     y, dy = y_dev.double(), dy_dev.double()
     ref = s_g * dy * (1 - y * y)
@@ -338,6 +349,7 @@ def check_backward(im, net, y_dev, dy_dev, s_g, worst):
     a = s_g * (g.abs() @ W.abs())
     bound = mask * ((C_TC * U * (math.sqrt(out) + out) + SPLIT) * a + SPLIT * ref.abs() + FLOOR)
     h, lo = im.dz(L - 2)
+    check_unsaturated(worst, f"dZ{L - 2}", h)
     worst.add(f"dZ{L - 2}", f64(h) + f64(lo), ref, bound)
     # hidden layers: dZ_{l-1} = mask (dZ_l W_l), on the tensor cores with the W^T items
     for l in range(L - 2, 0, -1):
@@ -350,6 +362,7 @@ def check_backward(im, net, y_dev, dy_dev, s_g, worst):
         ref = v / S_W * mask
         bound = mask * (_bound(HID, 3 * HID / 16 + 1, a / S_W) + SPLIT * ref.abs() + FLOOR)
         h, lo = im.dz(l - 1)
+        check_unsaturated(worst, f"dZ{l - 1}", h)
         worst.add(f"dZ{l - 1}", f64(h) + f64(lo), ref, bound)
 
 

@@ -28,7 +28,8 @@ in tc_images_common.py mirror the kernels' swizzles.
     Where |z64| of a pre-activation exceeds its bound the flag must equal z64 > 0, and a zero flag must come with an
     exactly zero image.  The encoding is held to 4u of float64 sin / cos of the fp32 products x b_k (sinf / cosf are
     within 2 ulp), tanhf to 4u |y|, the output dZ image to dy (1 - y^2) with the device's y, and the gradient scale
-    s_g is recomputed from the gmax word the call used with the rule of `grad_scales`.
+    s_g is recomputed from the gmax word the call used with the rule of `grad_scales`.  No hi term of an activation,
+    encoding or dZ image may be +-65504: there the saturating split has lost its 22 bits.
 
 Stand-alone calls: the `IMLP` call for the six networks with tensor-core kernels at the row counts of
 test_wgrad_gpu.py and test_bwd_reductions_gpu.py (1, 127, 129, one tile per cluster of two SMs less / more one tile,
@@ -121,13 +122,20 @@ def _init_flat(net, g):
 @pytest.mark.parametrize("which", list(NETS))
 def test_imlp_layers(which, rows, wg_units):
     """The stand-alone IMLP call (b200_mlp_forward / backward at B200_PREC_TC): checks (a) to (d)."""
-    lib = N.lib()
     dims, xs, xo = NETS[which]
     g = torch.Generator().manual_seed(_seed(f"{which}/{rows}"))
     net = Net(dims, None)
     net.flat = _init_flat(net, g)
     x = (torch.rand(rows, net.in_dim, generator=g) * xs + xo).to(DEV)
     dy = torch.randn(rows, net.out, generator=g).to(DEV)
+    check_imlp(net, x, dy, wg_units, f"{which} rows {rows}")
+
+
+def check_imlp(net, x, dy, wg_units, label):
+    """Runs the stand-alone IMLP call of `net` on x and dy on a 0xFF workspace and applies checks (a) to (d).
+    Returns the decoded images and what the call wrote: dict(im, s_g, word, grads, d_in)."""
+    lib = N.lib()
+    rows = x.shape[0]
     nbytes = int(lib.b200_mlp_workspace_bytes(C.byref(net.desc), rows, 1))
     ws = torch.full((nbytes,), 0xFF, dtype=torch.uint8, device=DEV)     # NaN in every unwritten float / fp16 pair
     y = torch.empty(rows, net.out, device=DEV)
@@ -160,7 +168,8 @@ def test_imlp_layers(which, rows, wg_units):
     gemms = wgrad_gemms(net)
     n_split = unit_splits([(a, b, 1) for _, a, b in gemms], wg_units)
     check_weight_gradients(im, net, grads, s_g, rows_pad // TM, n_split, worst)
-    worst.report(f"{which} rows {rows}")
+    worst.report(label)
+    return dict(im=im, s_g=s_g, word=word, grads=grads, d_in=d_in)
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -232,9 +241,10 @@ def head_d_uv(tr, cfg, ws, ng, label):
     return as_dev(val), as_dev(bnd)
 
 
-def check_atlas_trip(tr, with_global, want_counts, wg_units, label):
+def check_atlas_trip(tr, with_global, want_counts, wg_units, label, keep=None):
     """Checks (a) to (d) of both networks of the trip `tr` just ran on a 0xFF workspace, the tiles each launch
-    visited, the counters, the gmax words and the summed d_uv of groups 0-2.  Returns the counters."""
+    visited, the counters, the gmax words and the summed d_uv of groups 0-2.  Returns the counters; appends
+    (network name, Images, s_g, gmax word) per network to the list `keep` when one is given."""
     lib = N.lib()
     cfg = tr._config(with_global)
     ws = tr._workspace()
@@ -292,6 +302,8 @@ def check_atlas_trip(tr, with_global, want_counts, wg_units, label):
         k = len(wgrad_gemms(net))
         check_weight_gradients(im, net, tr.grads[tr.net_slice(which)], s_g, len(tiles), n_split[first:first + k], worst)
         first += k
+        if keep is not None:
+            keep.append((which, im, s_g, word))
         worst_all = max(worst_all, worst.report(f"{label}, {which}: {len(tiles)} of {int(off[11]) // TM} tiles live"))
     print(f"{label}: largest error / bound over both networks {worst_all:.3g}, summed d_uv of groups 0-2 {summed:.3g}")
     return cnt
@@ -491,9 +503,15 @@ def test_pretrain_trip_layers(pe, B, wg_units):
     """b200_pretrain_loss_grad_for on a 0xFF workspace: the mapping alone on one group of B rows (its own work list);
     the other mapping groups, every atlas image and buffer, and the atlas block of the gradients stay untouched."""
     _need_tc()
-    lib = N.lib()
     data, _ = small_data()
     tr = _trainer(data, B_SMALL, pe=pe)
+    check_pretrain_trip(tr, B, wg_units, f"pre-training trip, {'plain' if pe == 0 else f'PE-{pe}'} mapping, B {B}")
+
+
+def check_pretrain_trip(tr, B, wg_units, label):
+    """One pre-training trip of B random pixels of the benchmark geometry on the mapping of `tr`, checked as
+    test_pretrain_trip_layers states.  Returns the mapping's Images, s_g and gmax word."""
+    lib = N.lib()
     H, W, T, f = FULL["H"], FULL["W"], FULL["T"], 37
     g = torch.Generator().manual_seed(B)
     ys, xs = torch.randint(H, (B,), generator=g).to(DEV), torch.randint(W, (B,), generator=g).to(DEV)
@@ -508,7 +526,6 @@ def test_pretrain_trip_layers(pe, B, wg_units):
                                             N.ptr(tr.params), N.ptr(tr.grads), N.ptr(tr.losses), N.ptr(ws), ws.numel(),
                                             N.current_stream()), "b200_pretrain_loss_grad_for")
     torch.cuda.synchronize()
-    label = f"pre-training trip, {'plain' if pe == 0 else f'PE-{pe}'} mapping, B {B}"
     assert bool((atl.view(torch.int32) == nan_bits).all()), f"{label}: the atlas gradients were written"
     cap = tiles_of(B) * TM
     wo = (C.c_int64 * 8)()
@@ -545,3 +562,4 @@ def test_pretrain_trip_layers(pe, B, wg_units):
     n_split = unit_splits([(a, b, 1) for _, a, b in wgrad_gemms(net)], wg_units)
     check_weight_gradients(im, net, tr.grads[tr.net_slice("mapping")], s_g, len(tiles), n_split, worst)
     worst.report(f"{label}: {len(tiles)} of {9 * cap // TM} tiles live")
+    return im, s_g, word
