@@ -98,6 +98,8 @@ SIGNATURES = {
     "b200_launch_count": (C.c_longlong, []),
     "b200_debug_wgrad": (C.c_int, [_P, _P, _I32]),
     "b200_set_kernel_timer": (C.c_int, [_P, _P, C.c_int]),
+    "b200_tc_release_tables": (C.c_int, [_P, _I64]),
+    "b200_tc_cached_tables": (C.c_int, []),
     "b200_mlp_layout": (_I64, [C.POINTER(MlpDesc), C.POINTER(_I64), C.POINTER(_I64)]),
     "b200_mlp_workspace_bytes": (_I64, [C.POINTER(MlpDesc), _I64, C.c_int]),
     "b200_mlp_forward": (C.c_int, [C.POINTER(MlpDesc), _P, _P, _P, _I64, C.c_int, C.c_int, _P, _I64, _P]),

@@ -11,7 +11,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-from typing import Dict, Optional
+from typing import Dict, List, Optional, Tuple
 
 import numpy as np
 import torch
@@ -141,7 +141,7 @@ def video_files(data_folder):
 
 def _from_files(cls, data_folder, vid_root, vid_name, resy: int, resx: int, maximum_number_of_frames: int, device,
                 filter_optical_flow: bool = True, t_begin: int = 0, t_end: Optional[int] = None,
-                decode_all: bool = True):
+                decode_all: bool = True, clip: Optional[Tuple[int, int]] = None):
     """The stage-1 input producer on the device (SURVEY.md §8f rank 1): what `load_input_data_single`
     (unwrap_utils.py:105-163) returns, built frame by frame and pair by pair straight into the pixel records and the
     validity bitmaps — the eight (H, W, ., T) host tensors are never allocated.  The host decodes one image file at
@@ -150,14 +150,22 @@ def _from_files(cls, data_folder, vid_root, vid_name, resy: int, resx: int, maxi
     consistency masks and the packing run in libb200deflicker.so (csrc/producer.cu).  Returns (DeviceVideo,
     frames) with `frames` the decoded (H, W, 3, T) fp32 host tensor the PSNR of evaluate.py:740-743 needs.
     With `decode_all` False only the resident frames [t_begin, t_end) are decoded and `frames` is None: a frame
-    shard's evaluation reads its frames from the records (DeviceVideo.frame_rgb)."""
+    shard's evaluation reads its frames from the records (DeviceVideo.frame_rgb).
+    With `clip` = (c0, c1) the video is frames [c0, c1) of the folder, T = c1 - c0 (maximum_number_of_frames is not
+    applied): what a folder holding only those frames gives, reading only the flows of pairs inside the clip."""
     import cv2
     from pathlib import Path
     from PIL import Image
     vid_root = Path(vid_root)
     flow_dir = vid_root / f"{vid_name}_flow"
     files = video_files(data_folder)
-    T = int(min(maximum_number_of_frames, len(files)))
+    if clip is None:
+        T = int(min(maximum_number_of_frames, len(files)))
+    else:
+        c0, c1 = int(clip[0]), int(clip[1])
+        if not 0 <= c0 < c1 <= len(files):
+            raise N.B200Error(f"clip [{c0}, {c1}) is outside the {len(files)} frames of {data_folder}")
+        files, T = files[c0:c1], c1 - c0
     t_end = T if t_end is None else t_end
     lib, st = N.lib(), N.current_stream()
     H, W = int(resy), int(resx)
@@ -483,6 +491,22 @@ class FlatTrainer:
         g.replay()
         return self.losses
 
+    def release(self):
+        """Free what the trainer holds on the device once it is done: its captured graphs, the tensor-core job tables
+        the library cached for its parameter buffer (b200_tc_release_tables) and its buffers.  The trainer cannot
+        be used afterwards.  A process that fits one trainer after another calls it before building the next."""
+        if self.device.type == "cuda":
+            torch.cuda.synchronize(self.device)
+            self._graphs.clear()
+            with torch.cuda.device(self.device):
+                rc = self.lib.b200_tc_release_tables(N.ptr(self.params), self.params.numel() * 4)
+            if rc < 0:
+                raise N.B200Error("b200_tc_release_tables: " + N.last_error())
+        self._graphs, self._scratch, self._ws, self._dp, self.video = {}, {}, None, None, None
+        for name in ("params", "grad_loss", "grads", "losses", "exp_avg", "exp_avg_sq", "step_count", "indices",
+                     "_pin_inds", "_pin_loss"):
+            setattr(self, name, None)
+
     def step_host(self, inds_cpu: torch.Tensor, it: int, use_graph: bool = True) -> np.ndarray:
         """End-to-end call with HOST buffers: pinned H2D of the index batch, one loop trip,
         D2H of the loss vector (the step's result).  Synchronous."""
@@ -694,3 +718,31 @@ def frame_range(rank: int, world: int, T: int):
     base, rem = divmod(T, world)
     t0 = rank * base + min(rank, rem)
     return t0, t0 + base + (1 if rank < rem else 0)
+
+
+def clip_plan(T: int, max_frames: int) -> List[Tuple[int, int]]:
+    """The clips a T-frame video is fitted in, one atlas each: K = ceil(T / max_frames) contiguous frame ranges in
+    frame order, none longer than max_frames, their lengths differing by at most one.  T <= max_frames: [(0, T)]."""
+    K = max(1, -(-int(T) // int(max_frames)))
+    return [frame_range(k, K, T) for k in range(K)]
+
+
+def video_clips(config: dict, n_frames: int) -> List[Tuple[int, int]]:
+    """clip_plan of an n_frames video under the config's maximum_number_of_frames.  Refused when there is more than
+    one clip and the config resumes from `checkpoint_path`, which holds one atlas."""
+    clips = clip_plan(n_frames, config["maximum_number_of_frames"])
+    if len(clips) > 1 and config.get("load_checkpoint"):
+        raise N.B200Error(f"--clips fits {len(clips)} atlases to this {n_frames}-frame video (maximum_number_of_frames "
+                          f"= {config['maximum_number_of_frames']}), but load_checkpoint resumes one atlas from "
+                          f"checkpoint_path ({config.get('checkpoint_path')}): set load_checkpoint to false")
+    return clips
+
+
+def rank_clips(clips: List[Tuple[int, int]], rank: int, world: int) -> List[Tuple[int, int]]:
+    """The clips rank `rank` of `world` fits: clip k for k = rank (mod world)."""
+    return clips[rank::world]
+
+
+def clip_name(clip: Tuple[int, int]) -> str:
+    """Folder of a clip's stage-1 files under results/<vid>/stage_1/."""
+    return "clip_%05d_%05d" % (clip[0], clip[1])

@@ -66,6 +66,15 @@ def shared_seed(pg=None) -> int:
     return obj[0]
 
 
+def patient_group():
+    """A gloo group of every rank whose collectives have no practical deadline, for the barrier that ends independent
+    work of uneven length (one atlas fit per clip): an NCCL barrier would be ended by its watchdog when one rank waits
+    longer than the group's timeout.  Collective: create it while the ranks are in step."""
+    import datetime
+    import torch.distributed as dist
+    return dist.new_group(backend="gloo", timeout=datetime.timedelta(days=365))
+
+
 def broadcast_params(params: torch.Tensor, pg=None):
     """Rank 0's parameters on every rank (after each rank's own pre-training).  Collective."""
     import torch.distributed as dist

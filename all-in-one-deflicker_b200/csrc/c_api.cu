@@ -602,6 +602,13 @@ int b200_debug_wgrad(long long* cycles_host, int32_t* shapes_host, int32_t max_c
   return tc_debug_wgrad(cycles_host, shapes_host, max_ctas);
 }
 
+int b200_tc_release_tables(const void* params, int64_t bytes) {
+  B200_REQUIRE(params && bytes > 0, "null or empty parameter buffer");
+  return tc_release_tables(params, reinterpret_cast<const char*>(params) + bytes);
+}
+
+int b200_tc_cached_tables(void) { return tc_cached_tables(); }
+
 int b200_dp_slice(int32_t world, int32_t rank, int64_t n_total, int64_t* begin, int64_t* count) {
   B200_REQUIRE(world >= 1 && world <= B200_MAX_RANKS && rank >= 0 && rank < world && n_total > 0 && begin && count,
                "bad slice request");

@@ -1559,6 +1559,33 @@ int tc_debug_wgrad(long long* cycles, int* shapes, int max_ctas) {
   return n;
 }
 
+// An entry is correct whenever its key matches (the key names every pointer and extent its tables hold), but it
+// outlives the buffers it names.  A process that fits one trainer after another (one atlas per clip of a long video)
+// would keep every earlier trainer's entries: device memory outside the caller's allocator, and a slot each towards
+// MAX_TABLES.  The owner of a parameter buffer frees its entries here once no graph that bakes them in is replayed.
+int tc_release_tables(const void* begin, const void* end) {
+  std::lock_guard<std::mutex> lock(g_tabs_mutex);
+  const int dev = current_device();
+  int n = 0;
+  for (size_t i = 0; i < g_tabs.size();) {
+    TcTables* t = g_tabs[i];
+    const void* p = t->key.params;
+    if (t->key.dev != dev || p < begin || p >= end) { ++i; continue; }
+    if (t->d_wg && t->d_wg == g_last_wg) { g_last_wg = nullptr; g_last_wg_n = 0; }
+    B200_CHECK_CUDA(cudaFree(t->d_prep));
+    B200_CHECK_CUDA(cudaFree(t->d_wg));
+    delete t;
+    g_tabs.erase(g_tabs.begin() + i);
+    ++n;
+  }
+  return n;
+}
+
+int tc_cached_tables() {
+  std::lock_guard<std::mutex> lock(g_tabs_mutex);
+  return (int)g_tabs.size();
+}
+
 // grid of a weight-gradient launch: as many clusters as fit on the device at once, at most one per work unit
 static int wgrad_grid(int n_items) { return WG_CLUSTER * min(n_items, wg_clusters()); }
 

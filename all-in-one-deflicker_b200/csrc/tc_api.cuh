@@ -94,6 +94,10 @@ struct PersistentWorkspaceScope {
 };
 
 int tc_debug_wgrad(long long* cycles, int* shapes, int max_ctas);
+// cached job tables: free the current device's entries whose parameter buffer starts in [begin, end) (returns how
+// many, or a negative error code), and the number of entries held
+int tc_release_tables(const void* begin, const void* end);
+int tc_cached_tables();
 
 // diagnostics: the first B200_TC_OFFSET_GMAX entries of the b200_*_tc_image_offsets vector (see the header) for the
 // images of a stand-alone call whose tensor-core workspace starts at tc_ws, or of one network of the fused step

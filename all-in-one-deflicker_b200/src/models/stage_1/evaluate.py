@@ -70,9 +70,13 @@ class ArtefactWriter:
 
 
 def evaluate_model_single(trainer, resx, resy, number_of_frames, video_frames, results_folder, iteration,
-                          vid_name=None, save_checkpoint=True, artefacts=False, writer=None):
+                          vid_name=None, save_checkpoint=True, artefacts=False, writer=None, output_folder=None,
+                          frame_offset=0):
+    """Frame f's reconstruction goes to `<output_folder>/%05d.png % (frame_offset + f)` (default `<results_folder>/output`,
+    offset 0): a clip of a longer video writes its frames where they lie in the video."""
+    output_folder = os.path.join(results_folder, "output") if output_folder is None else output_folder
     os.makedirs(os.path.join(results_folder, '%06d' % iteration), exist_ok=True)
-    os.makedirs(os.path.join(results_folder, "output"), exist_ok=True)
+    os.makedirs(output_folder, exist_ok=True)
     if save_checkpoint:      # evaluate.py:616-622 — same file name and keys
         torch.save({'F_atlas_state_dict': {k: v.cpu() for k, v in trainer.state_dict("atlas").items()},
                     'iteration': iteration,
@@ -84,7 +88,7 @@ def evaluate_model_single(trainer, resx, resy, number_of_frames, video_frames, r
     ends = {}
     for f in range(number_of_frames):
         img, u8 = trainer.render_frame(f, int(resy), int(resx), number_of_frames, want_u8=True)
-        cv2.imwrite(os.path.join(results_folder, 'output', '%05d.png' % f),
+        cv2.imwrite(os.path.join(output_folder, '%05d.png' % (frame_offset + f)),
                     cv2.cvtColor(u8.cpu().numpy(), cv2.COLOR_RGB2BGR))       # evaluate.py:732-733
         psnrs[f] = A.psnr(video_frames[:, :, :, f], img.cpu())               # :740-743
         if art is not None:                                                  # :668-779, maps computed on the device
@@ -104,13 +108,15 @@ def evaluate_model_single(trainer, resx, resy, number_of_frames, video_frames, r
 
 
 def evaluate_model(trainer, resx, resy, number_of_frames, video_frames, results_folder, iteration, mask_frames=None,
-                   vid_name=None, save_checkpoint=True):
+                   vid_name=None, save_checkpoint=True, output_folder=None, frame_offset=0):
     """Segmentation variant (evaluate.py:203-602): checkpoint with the reference's keys (:216-233), the composite
     reconstruction (:293-335) written to `output/`, the alpha mattes to `<iteration>/alpha/`, PSNR.  Texture editing,
-    atlas dumps and per-pixel loss videos are visualisation (out of scope)."""
+    atlas dumps and per-pixel loss videos are visualisation (out of scope).  `output_folder` and `frame_offset` as in
+    evaluate_model_single; the alpha mattes keep the clip's own frame numbers."""
+    output_folder = os.path.join(results_folder, "output") if output_folder is None else output_folder
     folder = os.path.join(results_folder, '%06d' % iteration)
     os.makedirs(os.path.join(folder, "alpha"), exist_ok=True)
-    os.makedirs(os.path.join(results_folder, "output"), exist_ok=True)
+    os.makedirs(output_folder, exist_ok=True)
     if save_checkpoint:
         cpu = lambda which: {k: v.cpu() for k, v in trainer.state_dict(which).items()}
         ck = {'F_atlas_state_dict': cpu("atlas"), 'iteration': iteration, 'model_F_mapping1_state_dict': cpu("mapping1"),
@@ -121,7 +127,8 @@ def evaluate_model(trainer, resx, resy, number_of_frames, video_frames, results_
     psnrs = np.zeros((number_of_frames, 1))
     for f in range(number_of_frames):
         img, alpha, u8 = trainer.render_frame(f, int(resy), int(resx), number_of_frames, want_u8=True)
-        cv2.imwrite(os.path.join(results_folder, 'output', '%05d.png' % f), cv2.cvtColor(u8.cpu().numpy(), cv2.COLOR_RGB2BGR))
+        cv2.imwrite(os.path.join(output_folder, '%05d.png' % (frame_offset + f)),
+                    cv2.cvtColor(u8.cpu().numpy(), cv2.COLOR_RGB2BGR))
         cv2.imwrite(os.path.join(folder, 'alpha', '%05d.png' % f), (alpha.cpu().numpy() * 255).astype(np.uint8))
         psnrs[f] = A.psnr(video_frames[:, :, :, f], img.cpu())
     open(os.path.join(folder, "PSNR_%f" % psnrs.mean()), "w").close()

@@ -5,6 +5,8 @@ layouts as the reference returns); `get_tuples` and `pre_train_mapping` are prov
 the latter running on the fused trainer.  `load_input_data` is the segmentation variant's loader (adds the
 bootstrapping masks).  `save_mask_flow` writes the reference's two overview videos with OpenCV.
 """
+from pathlib import Path
+
 import numpy as np
 import torch
 import cv2
@@ -75,16 +77,26 @@ def load_input_data_single(resy, resx, maximum_number_of_frames, data_folder, us
     return flows_mask, frames, flows_rev_mask, mask_frames, dx, dy, flows_rev, flows
 
 
-def load_mask_frames(resy, resx, number_of_frames, vid_root, vid_name):
-    """(resy, resx, T) bootstrapping masks from `<vid>_seg` (unwrap_utils.py:43,60,67-70).  The reference passes
-    cv2.INTER_NEAREST in the position of cv2.resize's `dst` argument, which OpenCV ignores: the masks are resized
-    with the default bilinear interpolation, and so they are here."""
-    mask_dir = vid_root / f'{vid_name}_seg'
+def mask_files(vid_root, vid_name, number_of_frames, clip=None):
+    """The matte files of `<vid>_seg` for frames [0, number_of_frames), or for the frames [c0, c1) of `clip`, in sorted
+    order.  Refused when the folder holds fewer."""
+    mask_dir = Path(vid_root) / f'{vid_name}_seg'
     files = sorted(list(mask_dir.glob('*.jpg')) + list(mask_dir.glob('*.png')))
-    if len(files) < number_of_frames:
-        raise FileNotFoundError(f"{mask_dir}: {len(files)} mask images for {number_of_frames} frames — the segmentation "
+    c0, c1 = (0, number_of_frames) if clip is None else clip
+    if len(files) < c1:
+        what = f"{number_of_frames} frames" if clip is None else f"clip_{c0:05d}_{c1:05d} (frames {c0} to {c1 - 1})"
+        raise FileNotFoundError(f"{mask_dir}: {len(files)} mask images for {what} — the segmentation "
                                 f"variant needs one matte per frame (the reference writes them with "
                                 f"src/preprocess_mask_portrait.py / preprocess_mask_rcnn.py)")
+    return files[c0:c1]
+
+
+def load_mask_frames(resy, resx, number_of_frames, vid_root, vid_name, clip=None):
+    """(resy, resx, T) bootstrapping masks from `<vid>_seg` (unwrap_utils.py:43,60,67-70).  The reference passes
+    cv2.INTER_NEAREST in the position of cv2.resize's `dst` argument, which OpenCV ignores: the masks are resized
+    with the default bilinear interpolation, and so they are here.  With `clip` = (c0, c1) (T = c1 - c0): the mattes
+    of frames c0..c1-1, as a folder holding only those would give."""
+    files = mask_files(vid_root, vid_name, number_of_frames, clip)
     masks = torch.zeros((resy, resx, number_of_frames))
     for i in range(number_of_frames):
         m = np.array(Image.open(str(files[i]))).astype(np.float64) / 255.

@@ -3,12 +3,16 @@ the reference script (src/stage1_neural_atlas.py:257-281); the optimisation loop
 (:151-231) runs as one replayed CUDA graph per iteration in libb200deflicker.so.
 
     python src/stage1_neural_atlas.py --vid_name NAME [--config config_flow_100.json] [--root data/test/]
-                                      [--down 4] [--gpu 0] [--gpus 1]
+                                      [--down 4] [--gpu 0] [--gpus 1] [--clips]
 
 With --gpus N > 1 the script re-runs itself under `python -m torch.distributed.run --nproc-per-node N`; under torchrun
 (any world size) every rank computes a block of the flow pairs, holds a block of the frames and evaluates those.
+
+With --clips a video longer than maximum_number_of_frames is fitted as clips (b200.atlas.clip_plan), one atlas each,
+the clips spread over the ranks under torchrun; see `fit_clips`.
 """
 import argparse
+import gc
 import glob
 import json
 import os
@@ -30,7 +34,10 @@ from src.models.stage_1.evaluate import evaluate_model_single  # noqa: E402
 from src.models.stage_1.unwrap_utils import pre_train_mapping, save_mask_flow  # noqa: E402
 
 
-def main(config, args):
+def main(config, args, clip=None, device=None):
+    """Fit the atlas of the video on `device` (default: the current CUDA device).  With `clip` = (c0, c1): the run
+    on a folder holding only frames [c0, c1) and their flows, its files under stage_1/clip_<c0>_<c1>/ except the
+    output frames, which go to stage_1/output/ at their frame numbers in the whole video."""
     frames_list = sorted(glob.glob(os.path.join(args.vid_path, "*g")))
     first = cv2.imread(frames_list[0])
     resx, resy = first.shape[1], first.shape[0]
@@ -38,16 +45,19 @@ def main(config, args):
         resx, resy = int(resx / args.down), int(resy / args.down)
     data_folder = Path(args.vid_path)
     vid_name, vid_root = data_folder.name, data_folder.parent
-    results_folder = Path(f'./results/{vid_name}/stage_1')
+    stage_folder = Path(f'./results/{vid_name}/stage_1')
+    results_folder = stage_folder if clip is None else stage_folder / A.clip_name(clip)
+    output = {} if clip is None else dict(output_folder=str(stage_folder / "output"), frame_offset=clip[0])
     results_folder.mkdir(parents=True, exist_ok=True)
     with open('%s/config.json' % results_folder, 'w') as f:
         json.dump(config, f, indent=4)
 
-    device = torch.device("cuda")
+    device = torch.device("cuda") if device is None else device
     # input producer on the device (the reference's load_input_data_single, unwrap_utils.py:105-163): frames, image
     # differences, resized flows and consistency masks go straight into HBM; `frames` is the decoded video for PSNR
     video, frames = A.DeviceVideo.from_files(data_folder, vid_root, vid_name, resy, resx,
-                                             config["maximum_number_of_frames"], device, filter_optical_flow=True)
+                                             config["maximum_number_of_frames"], device, filter_optical_flow=True,
+                                             clip=clip)
     T = frames.shape[3]
     writer = None
     if not args.no_artefacts:      # the reference's tensorboard log + overview videos (:99,109; unwrap_utils.py:200-231)
@@ -78,7 +88,22 @@ def main(config, args):
         trainer.step_host(inds, i)
         if i % evaluate_every == 0 and i > start_iteration:
             evaluate_model_single(trainer, resx, resy, T, frames, results_folder, i, vid_name,
-                                  artefacts=not args.no_artefacts, writer=writer)
+                                  artefacts=not args.no_artefacts, writer=writer, **output)
+    if writer is not None:
+        writer.close()
+    trainer.release()
+
+
+def fit_clips(config, args, clips, device, seed):
+    """Fit one atlas per clip of `clips` on `device`, in order, with no process group: clip k is `main(config, args,
+    clip)`, started from the CPU generator seeded with `seed`, so its files are those of a stand-alone run on a
+    folder holding only its frames.  Nothing of a clip is alive when the next one is loaded."""
+    for clip in clips:
+        torch.manual_seed(seed)
+        with torch.cuda.device(device):
+            main(config, args, clip, device)
+            gc.collect()
+            torch.cuda.empty_cache()
 
 
 def main_sharded(config, args, device, pg, phases=None):
@@ -165,20 +190,31 @@ if __name__ == "__main__":
                         help="skip the evaluation videos / tensorboard log (checkpoint, output frames and PSNR only)")
     parser.add_argument('--gpus', type=int, default=1,
                         help="fit on this many GPUs of the node, the video sharded by frame (started under torchrun)")
+    parser.add_argument('--clips', action='store_true',
+                        help="fit a video longer than maximum_number_of_frames as clips of at most that many frames, "
+                             "one atlas each (spread over the GPUs with --gpus)")
     args = parser.parse_args()
     from b200 import launch
     env = launch.torchrun_env()
     if env is None and args.gpus > 1:
         sys.exit(launch.relaunch(__file__, sys.argv[1:], args.gpus))
     args.vid_path = os.path.join(args.root, args.vid_name)
+    with open(os.path.join(HERE, "config", args.config)) as f:
+        config = json.load(f)
+    clips = A.video_clips(config, len(A.video_files(args.vid_path))) if args.clips else [None]
     if env is not None:
         from src.preprocess_optical_flow import preprocess_sharded
         device, pg = launch.init(env[2])
-        phases = launch.Phases(pg)
-        preprocess_sharded(args.vid_path, env[0], env[1])
-        phases.mark("prepass")
-        with open(os.path.join(HERE, "config", args.config)) as f:
-            main_sharded(json.load(f), args, device, pg, phases)
+        if len(clips) > 1:
+            preprocess_sharded(args.vid_path, env[0], env[1])
+            seed, done = launch.shared_seed(pg), launch.patient_group()
+            fit_clips(config, args, A.rank_clips(clips, env[0], env[1]), device, seed)
+            torch.distributed.barrier(group=done)
+        else:
+            phases = launch.Phases(pg)
+            preprocess_sharded(args.vid_path, env[0], env[1])
+            phases.mark("prepass")
+            main_sharded(config, args, device, pg, phases)
         launch.finish()
         sys.exit(0)
     os.environ["CUDA_VISIBLE_DEVICES"] = "%d" % args.gpu
@@ -189,5 +225,7 @@ if __name__ == "__main__":
     print(cmd)
     if subprocess.call(cmd, shell=True) != 0:
         raise RuntimeError("optical-flow pre-pass failed")
-    with open(os.path.join(HERE, "config", args.config)) as f:
-        main(json.load(f), args)
+    if len(clips) > 1:
+        fit_clips(config, args, clips, torch.device("cuda"), torch.initial_seed())
+    else:
+        main(config, args)

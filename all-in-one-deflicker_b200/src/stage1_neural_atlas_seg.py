@@ -3,17 +3,21 @@ CLI, config keys, on-disk inputs and outputs as the reference script (src/stage1
 loop body (:195-319) runs in libb200deflicker.so (b200_seg_loss_grad + b200_adam_step).
 
     python src/stage1_neural_atlas_seg.py --vid_name NAME --class_name portrait [--config config_flow_100.json]
-                                          [--root data/test/] [--down 1] [--gpu 0] [--gpus 1]
+                                          [--root data/test/] [--down 1] [--gpu 0] [--gpus 1] [--clips]
 
 With --gpus N > 1 the script re-runs itself under `python -m torch.distributed.run --nproc-per-node N`; under torchrun
 (any world size) every rank computes a block of the flow pairs, holds a block of the frames and their mattes and
 evaluates those frames.
+
+With --clips a video longer than maximum_number_of_frames is fitted as clips (b200.atlas.clip_plan), one atlas each,
+the clips spread over the ranks under torchrun; see `fit_clips`.
 
 The mattes of `<root>/<NAME>_seg/` are an input: the reference produces them with third-party models (CarveKit /
 detectron2 Mask-RCNN, src/preprocess_mask_*.py) that this repository does not ship; the script stops with a clear
 message when they are missing.
 """
 import argparse
+import gc
 import glob
 import json
 import os
@@ -33,10 +37,14 @@ from b200 import _native as N  # noqa: E402
 from b200 import atlas as A    # noqa: E402
 from b200 import seg as SG     # noqa: E402
 from src.models.stage_1.evaluate import evaluate_model  # noqa: E402
-from src.models.stage_1.unwrap_utils import load_mask_frames, pre_train_mapping  # noqa: E402
+from src.models.stage_1.unwrap_utils import load_mask_frames, mask_files, pre_train_mapping  # noqa: E402
 
 
-def main(config, args):
+def main(config, args, clip=None, device=None):
+    """Fit the two-layer atlas of the video on `device` (default: the current CUDA device).  With `clip` = (c0, c1):
+    the run on a folder holding only frames [c0, c1), their flows and their mattes, its files under
+    stage_1/clip_<c0>_<c1>/ except the output frames, which go to stage_1/output/ at their frame numbers in the whole
+    video."""
     frames_list = sorted(glob.glob(os.path.join(args.vid_path, "*g")))
     first = cv2.imread(frames_list[0])
     resx, resy = first.shape[1], first.shape[0]
@@ -44,16 +52,19 @@ def main(config, args):
         resx, resy = int(resx / args.down), int(resy / args.down)
     data_folder = Path(args.vid_path)
     vid_name, vid_root = data_folder.name, data_folder.parent
-    results_folder = Path(f'./results/{vid_name}/stage_1')
+    stage_folder = Path(f'./results/{vid_name}/stage_1')
+    results_folder = stage_folder if clip is None else stage_folder / A.clip_name(clip)
+    output = {} if clip is None else dict(output_folder=str(stage_folder / "output"), frame_offset=clip[0])
     results_folder.mkdir(parents=True, exist_ok=True)
     with open('%s/config.json' % results_folder, 'w') as f:
         json.dump(config, f, indent=4)
 
-    device = torch.device("cuda")
+    device = torch.device("cuda") if device is None else device
     video, frames = A.DeviceVideo.from_files(data_folder, vid_root, vid_name, resy, resx,
-                                             config["maximum_number_of_frames"], device, filter_optical_flow=True)
+                                             config["maximum_number_of_frames"], device, filter_optical_flow=True,
+                                             clip=clip)
     T = frames.shape[3]
-    mask_frames = load_mask_frames(resy, resx, T, vid_root, vid_name)
+    mask_frames = load_mask_frames(resy, resx, T, vid_root, vid_name, clip=clip)
     precision = N.PREC_TC if N.lib().b200_device_supports_tc() else N.PREC_FP32
     trainer = SG.SegTrainer(video, SG.pack_mask_frames(mask_frames, device), config, precision=precision, device=device,
                             resx=resx)
@@ -80,7 +91,28 @@ def main(config, args):
         inds = torch.randint(n_pixels, (samples, 1))       # same CPU-generator draw as the reference (:204)
         trainer.step_host(inds, i)
         if i % evaluate_every == 0 and i > start_iteration:
-            evaluate_model(trainer, resx, resy, T, frames, results_folder, i, mask_frames, vid_name)
+            evaluate_model(trainer, resx, resy, T, frames, results_folder, i, mask_frames, vid_name, **output)
+    trainer.release()
+
+
+def fit_clips(config, args, clips, device, seed):
+    """Fit one two-layer atlas per clip of `clips` on `device`, in order, with no process group: clip k is
+    `main(config, args, clip)`, started from the CPU generator seeded with `seed`, so its files are those of a
+    stand-alone run on a folder holding only its frames and mattes.  Nothing of a clip is alive when the next one is
+    loaded."""
+    for clip in clips:
+        torch.manual_seed(seed)
+        with torch.cuda.device(device):
+            main(config, args, clip, device)
+            gc.collect()
+            torch.cuda.empty_cache()
+
+
+def check_clip_mattes(vid_path, clips):
+    """Refuse, naming the first clip concerned, a matte folder that holds fewer mattes than the video has frames."""
+    data_folder = Path(vid_path)
+    for clip in clips:
+        mask_files(data_folder.parent, data_folder.name, clip[1] - clip[0], clip)
 
 
 def main_sharded(config, args, device, pg):
@@ -150,6 +182,9 @@ if __name__ == "__main__":
     parser.add_argument('--class_name', type=str, default="portrait")
     parser.add_argument('--gpus', type=int, default=1,
                         help="fit on this many GPUs of the node, the video sharded by frame (started under torchrun)")
+    parser.add_argument('--clips', action='store_true',
+                        help="fit a video longer than maximum_number_of_frames as clips of at most that many frames, "
+                             "one atlas each (spread over the GPUs with --gpus)")
     args = parser.parse_args()
     from b200 import launch
     env = launch.torchrun_env()
@@ -157,6 +192,9 @@ if __name__ == "__main__":
         sys.exit(launch.relaunch(__file__, sys.argv[1:], args.gpus))
     args.vid_path = os.path.join(args.root, args.vid_name)
     seg_dir = args.vid_path.rstrip("/") + "_seg"
+    with open(os.path.join(HERE, "config", args.config)) as f:
+        config = json.load(f)
+    clips = A.video_clips(config, len(A.video_files(args.vid_path))) if args.clips else [None]
     if env is not None:
         if not glob.glob(os.path.join(seg_dir, "*g")):
             raise FileNotFoundError(f"{seg_dir} holds no mattes: produce them with the reference's mask pre-pass "
@@ -164,8 +202,13 @@ if __name__ == "__main__":
         from src.preprocess_optical_flow import preprocess_sharded
         device, pg = launch.init(env[2])
         preprocess_sharded(args.vid_path, env[0], env[1])
-        with open(os.path.join(HERE, "config", args.config)) as f:
-            main_sharded(json.load(f), args, device, pg)
+        if len(clips) > 1:
+            check_clip_mattes(args.vid_path, clips)
+            seed, done = launch.shared_seed(pg), launch.patient_group()
+            fit_clips(config, args, A.rank_clips(clips, env[0], env[1]), device, seed)
+            torch.distributed.barrier(group=done)
+        else:
+            main_sharded(config, args, device, pg)
         launch.finish()
         sys.exit(0)
     os.environ["CUDA_VISIBLE_DEVICES"] = args.gpu
@@ -177,5 +220,8 @@ if __name__ == "__main__":
     if not glob.glob(os.path.join(seg_dir, "*g")):
         raise FileNotFoundError(f"{seg_dir} holds no mattes: produce them with the reference's mask pre-pass "
                                 f"(class '{args.class_name}') or any segmentation tool, one image per frame")
-    with open(os.path.join(HERE, "config", args.config)) as f:
-        main(json.load(f), args)
+    if len(clips) > 1:
+        check_clip_mattes(args.vid_path, clips)
+        fit_clips(config, args, clips, torch.device("cuda"), torch.initial_seed())
+    else:
+        main(config, args)

@@ -16,6 +16,8 @@ parser.add_argument('--gpu', type=int, default=0)
 parser.add_argument('--gpus', type=int, default=1,
                     help="run the flow pre-pass, stage 1 and stage 2 on this many GPUs of the node")
 parser.add_argument('--class_name', type=str, default=None)
+parser.add_argument('--clips', action='store_true',
+                    help="stage 1 fits a video longer than maximum_number_of_frames as clips, one atlas each")
 parser.add_argument('--ckpt_filter', type=str, default="./pretrained_weights/neural_filter.pth")
 parser.add_argument('--ckpt_local', type=str, default="./pretrained_weights/local_refinement_net.pth")
 
@@ -71,6 +73,9 @@ if __name__ == "__main__":
         # both stages re-run themselves under torchrun on cuda:0..N-1
         stage1 += ["--gpus", str(args.gpus)]
         stage2 += ["--gpus", str(args.gpus)]
+    if args.clips:
+        # stage 2 runs over the whole video's output frames as it is
+        stage1 += ["--clips"]
     rc = subprocess.call(stage1)
     if rc != 0:
         sys.exit(rc)

@@ -65,6 +65,13 @@ long long b200_launch_count(void);
  * 3 * max_ctas entries; returns the number of CTAs or -1.  Synchronises the device. */
 int b200_debug_wgrad(long long* cycles_host, int32_t* shapes_host, int32_t max_ctas);
 int b200_set_kernel_timer(void* ev_start, void* ev_stop, int tag);
+/* The tensor-core job tables that calls on a persistent workspace cache (the fused step, pre-training, the
+ * segmentation step and render) are keyed by the workspace, parameter and gradient pointers and the row geometry, and
+ * are held until released.  b200_tc_release_tables frees the current device's entries whose parameters lie in
+ * [params, params + bytes): the owner of that parameter buffer calls it when it is done, after the last replay of any
+ * CUDA graph captured over those calls.  Returns the number freed.  b200_tc_cached_tables: entries held now. */
+int b200_tc_release_tables(const void* params, int64_t bytes);
+int b200_tc_cached_tables(void);
 
 /* ------------------------------------------------------------------------------------------
  * IMLP  — replaces  src/models/stage_1/implicit_neural_networks.py:15-81  (class IMLP)
