@@ -73,6 +73,15 @@ class SegConfig(C.Structure):
                 ("mapping1", MlpDesc), ("mapping2", MlpDesc), ("alpha", MlpDesc), ("atlas", MlpDesc)]
 
 
+class WarpPair(C.Structure):
+    _fields_ = [("frame0", C.c_void_p), ("frame1", C.c_void_p), ("fwd", C.c_void_p), ("bwd", C.c_void_p),
+                ("H", C.c_int32), ("W", C.c_int32), ("Hf", C.c_int32), ("Wf", C.c_int32), ("bits", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
+WARP_MAX_PAIRS = 32
+
+
 class PngPlan(C.Structure):
     _fields_ = [("magic", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("n_blocks", C.c_int32),
                 ("n_chunks", C.c_int32), ("prefix_bytes", C.c_int32), ("suffix_bytes", C.c_int32),
@@ -156,6 +165,8 @@ SIGNATURES = {
                                  _P, _I64, _P]),
     "b200_frame_sse_workspace_bytes": (_I64, [_I32, _I32]),
     "b200_frame_sse": (C.c_int, [C.POINTER(Video), _I32, _P, _P, _P, _I64, _P]),
+    "b200_warp_error_workspace_bytes": (_I64, [C.POINTER(WarpPair), _I32]),
+    "b200_warp_error": (C.c_int, [C.POINTER(WarpPair), _I32, _P, _P, _P, _P, _I64, _P]),
     "b200_render_workspace_bytes": (_I64, [_I64]),
     "b200_render": (C.c_int, [_P, _I32, _I32, _I32, _I32, _I64, _I64, _P, _P, C.c_int, _P, _I64, _P]),
     "b200_corr_pyramid_floats": (_I64, [_I32, _I32]),

@@ -6,6 +6,7 @@
 // pixels, then a shuffle / shared-memory tree), then one CTA that sums the partials in the same tree.  No atomics, so
 // the result is bit-identical across calls, CUDA-graph replays, devices and ranks.
 #include "atlas_internal.cuh"
+#include "cta_sum.cuh"
 
 namespace b200 {
 
@@ -15,21 +16,6 @@ constexpr int kSseMaxBlocks = 1024;
 static int sse_blocks(int64_t pixels) {
   const int64_t b = (pixels + kSseThreads - 1) / kSseThreads;
   return (int)(b < kSseMaxBlocks ? b : kSseMaxBlocks);
-}
-
-// Sum of `v` over the CTA, valid in thread 0.  Fixed order: xor-shuffle tree in each warp, then warp 0 over the warps.
-__device__ __forceinline__ double cta_sum(double v, double* sh) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (lane == 0) sh[warp] = v;
-  __syncthreads();
-  if (warp == 0) {
-    v = lane < kSseThreads / 32 ? sh[lane] : 0.0;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  }
-  return v;
 }
 
 __global__ void __launch_bounds__(kSseThreads) frame_sse_partial_kernel(const float* __restrict__ records,
@@ -46,7 +32,7 @@ __global__ void __launch_bounds__(kSseThreads) frame_sse_partial_kernel(const fl
     acc += d1 * d1;
     acc += d2 * d2;
   }
-  acc = cta_sum(acc, sh);
+  acc = cta_sum<kSseThreads>(acc, sh);
   if (threadIdx.x == 0) partials[blockIdx.x] = acc;
 }
 
@@ -55,7 +41,7 @@ __global__ void __launch_bounds__(kSseThreads) frame_sse_final_kernel(const doub
   __shared__ double sh[kSseThreads / 32];
   double acc = 0.0;
   for (int i = threadIdx.x; i < n; i += kSseThreads) acc += partials[i];
-  acc = cta_sum(acc, sh);
+  acc = cta_sum<kSseThreads>(acc, sh);
   if (threadIdx.x == 0) *out = acc;
 }
 

@@ -17,24 +17,6 @@
 
 namespace b200 {
 
-// single IEEE operations in either arithmetic: the compiler must not contract a product and a sum into an fma
-__device__ __forceinline__ float mul(float a, float b) { return __fmul_rn(a, b); }
-__device__ __forceinline__ float add(float a, float b) { return __fadd_rn(a, b); }
-__device__ __forceinline__ double mul(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ double add(double a, double b) { return __dadd_rn(a, b); }
-
-// Bilinear sample of one channel at destination (y, x); `at(row, col)` reads the source in the arithmetic type T.
-template <typename T, typename At>
-__device__ __forceinline__ T resize_sample(At at, int h, int w, int H, int W, int y, int x) {
-  if (h == H && w == W) return at(y, x);
-  if (h == 2 * H && w == 2 * W)
-    return mul(add(add(add(at(2 * y, 2 * x), at(2 * y, 2 * x + 1)), at(2 * y + 1, 2 * x)), at(2 * y + 1, 2 * x + 1)), (T)0.25);
-  const ResizeTap tx = resize_tap(x, W, w, true), ty = resize_tap(y, H, h, false);
-  const T r0 = add(mul(at(ty.s0, tx.s0), (T)tx.w0), mul(at(ty.s0, tx.s1), (T)tx.w1));
-  const T r1 = add(mul(at(ty.s1, tx.s0), (T)tx.w0), mul(at(ty.s1, tx.s1), (T)tx.w1));
-  return add(mul(r0, (T)ty.w0), mul(r1, (T)ty.w1));
-}
-
 // 8-bit HWC image with 1, 3 or 4 channels read as the reference reads it: grey repeated, a 4th channel dropped
 struct U8Image {
   const uint8_t* p; int h, w, c;

@@ -1,0 +1,242 @@
+"""Flicker of a video's sequences: the temporal warping error of the input, the stage-1 atlas reconstruction, the
+neural filter's output and the final output, computed on the GPU (b200.flicker; DESIGN §4e).
+
+    python src/evaluate_flicker.py --video_name NAME [--sequences input,atlas,filter,final] [--gpus N] [--clips]
+
+Run from the directory that holds data/test/NAME (the pipeline's working directory).  Pair t uses the flow pre-pass's
+files data/test/NAME_flow/<t>_<t+1>.npy (F) and <t+1>_<t>.npy (B) of the input's sorted frames; missing pairs are
+computed first with the pre-pass.  A sequence's frames are its sorted files, matched to the input's by position, and are
+scored at their own resolution.  Writes results/NAME/flicker.json and prints a table.  With --gpus N the pairs are split
+into contiguous blocks over N ranks and rank 0 writes the same bytes as a one-GPU run."""
+import argparse
+import concurrent.futures as cf
+import json
+import math
+import os
+import sys
+import time
+from pathlib import Path
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+import numpy as np  # noqa: E402
+
+SEQUENCES = ("input", "atlas", "filter", "final")
+CONFIG = os.path.join(os.path.dirname(os.path.abspath(__file__)), "config", "config_flow_100.json")
+WINDOW_PAIRS = 8                    # with four sequences, one b200_warp_error call (B200_WARP_MAX_PAIRS = 32)
+DECODERS = min(8, os.cpu_count() or 1)
+
+
+def sequence_folders(name):
+    return {"input": os.path.join("data", "test", name),
+            "atlas": os.path.join("results", name, "stage_1", "output"),
+            "filter": os.path.join("results", name, "neural_filter", "output"),
+            "final": os.path.join("results", name, "final", "output")}
+
+
+def frame_files(folder):
+    """The frames of a sequence folder in order: *.png / *.jpg / *.jpeg, as the pre-pass lists them."""
+    return sorted(Path(folder).glob('*.*g'))
+
+
+def read_frame(path):
+    """A frame file as (H, W, 3) uint8 or uint16 (cv2's BGR order: the metric sums over the channels); grey is
+    repeated, a 4th channel dropped."""
+    import cv2
+    img = cv2.imread(str(path), cv2.IMREAD_UNCHANGED)
+    if img is None:
+        raise FileNotFoundError(f"cannot decode {path}")
+    if img.dtype not in (np.uint8, np.uint16):
+        raise ValueError(f"{path}: {img.dtype} pixels; frames are 8- or 16-bit")
+    if img.ndim == 2:
+        img = np.repeat(img[:, :, None], 3, axis=2)
+    return np.ascontiguousarray(img[:, :, :3])
+
+
+def pair_windows(p0, p1, k=WINDOW_PAIRS):
+    return [(a, min(a + k, p1)) for a in range(p0, p1, k)]
+
+
+def load_window(first, last, flow_dir, inputs, seq_frames):
+    """Flows of pairs [first, last) and each sequence's frames first .. last (those it has, decoded on DECODERS
+    threads), with the seconds spent loading flows and decoding frames."""
+    from src.preprocess_optical_flow import flow_files
+    t0 = time.perf_counter()
+    flows = [tuple(np.load(f).astype(np.float32, copy=False) for f in flow_files(flow_dir, inputs, p))
+             for p in range(first, last)]
+    t1 = time.perf_counter()
+    with cf.ThreadPoolExecutor(DECODERS) as pool:          # cv2 decodes without the GIL
+        frames = {s: list(pool.map(read_frame, files[first:last + 1])) for s, files in seq_frames.items()}
+    return flows, frames, t1 - t0, time.perf_counter() - t1
+
+
+def score_pairs(p0, p1, flow_dir, inputs, seq_frames, score_window, stats=None):
+    """(squared-error sum, |M|) of pairs [p0, p1) for each sequence (pairs a sequence has both frames of), with each
+    window's files read on a thread while the previous window is scored."""
+    out = {s: [] for s in seq_frames}
+    windows = pair_windows(p0, p1)
+    if not windows:
+        return out
+    loader = cf.ThreadPoolExecutor(1)
+    try:
+        load = lambda w: loader.submit(load_window, w[0], w[1], flow_dir, inputs, seq_frames)
+        nxt = load(windows[0])
+        for j in range(len(windows)):
+            flows, frames, t_flow, t_decode = nxt.result()
+            nxt = load(windows[j + 1]) if j + 1 < len(windows) else None
+            for s, v in score_window(flows, frames).items():
+                out[s] += v
+            if stats is not None:
+                stats["flow_load"] += t_flow
+                stats["decode"] += t_decode
+    finally:
+        loader.shutdown(wait=True, cancel_futures=True)
+    return out
+
+
+def clip_boundaries(n_frames):
+    """The pairs (c1 - 1, c1) that straddle two clips of the plan stage 1's --clips fits an n_frames video in."""
+    from b200.atlas import clip_plan
+    with open(CONFIG) as f:
+        max_frames = json.load(f)["maximum_number_of_frames"]
+    plan = clip_plan(n_frames, max_frames)
+    return plan, [c1 - 1 for _, c1 in plan[:-1]]
+
+
+def _mean(values):
+    v = [x for x in values if not math.isnan(x)]
+    return sum(v) / len(v) if v else None
+
+
+def report(name, pairs, resolutions, folders, scores, clips=None):
+    """The flicker.json document: per sequence its resolution, per-pair E(t) and |M| (E is null for an empty mask),
+    E_warp (mean over the non-empty pairs; null when there is none) and the empty-pair count.  With clips, the
+    boundary pairs and the means over boundary and interior pairs."""
+    from b200.flicker import pair_value
+    doc = {"video": name, "pairs": pairs, "sequences": {}}
+    if clips is not None:
+        doc["clips"] = {"plan": [list(c) for c in clips[0]], "boundary_pairs": clips[1]}
+    for s, sc in scores.items():
+        e = [pair_value(sse, n) for sse, n in sc]
+        entry = {"folder": folders[s], "resolution": list(resolutions[s]),
+                 "per_pair": [{"t": t, "E": None if math.isnan(v) else v, "mask": int(n)}
+                              for t, (v, (_, n)) in enumerate(zip(e, sc))],
+                 "E_warp": _mean(e), "empty_pairs": sum(1 for v in e if math.isnan(v))}
+        if clips is not None:
+            b = set(clips[1])
+            entry["E_boundary"] = _mean([v for t, v in enumerate(e) if t in b])
+            entry["E_interior"] = _mean([v for t, v in enumerate(e) if t not in b])
+        doc["sequences"][s] = entry
+    return doc
+
+
+def table(doc):
+    clips = "clips" in doc
+    head = "%-8s %11s %6s %6s %12s" % ("sequence", "resolution", "pairs", "empty", "E_warp")
+    lines = [head + (" %12s %12s" % ("E_boundary", "E_interior") if clips else "")]
+    fmt = lambda v: "%12s" % "-" if v is None else "%12.6g" % v
+    for s, e in doc["sequences"].items():
+        line = "%-8s %11s %6d %6d %s" % (s, "%dx%d" % tuple(e["resolution"]), len(e["per_pair"]), e["empty_pairs"],
+                                         fmt(e["E_warp"]))
+        if clips:
+            line += " %s %s" % (fmt(e["E_boundary"]), fmt(e["E_interior"]))
+        lines.append(line)
+    return "\n".join(lines)
+
+
+def evaluate(name, sequences, score_window, rank=0, world=1, pg=None, clips=False, stats=None):
+    """Scores rank's block of pairs; under a process group the blocks are gathered in pair order.  Returns the
+    flicker.json document on rank 0 (None on the other ranks)."""
+    folders = sequence_folders(name)
+    inputs = frame_files(folders["input"])
+    if len(inputs) < 2:
+        raise FileNotFoundError(f"{folders['input']} holds {len(inputs)} frames; the warping error needs two")
+    flow_dir = Path(folders["input"] + "_flow")
+    seq_frames = {}
+    for s in sequences:
+        files = frame_files(folders[s])
+        if s == "input" or len(files) >= 2:
+            seq_frames[s] = files[:len(inputs)]
+        elif rank == 0:
+            print("evaluate_flicker: no %s frames in %s, skipped" % (s, folders[s]), flush=True)
+    p0, p1 = 0, len(inputs) - 1
+    if world > 1:
+        from b200.launch import pair_block
+        p0, p1 = pair_block(rank, world, len(inputs))
+    mine = score_pairs(p0, p1, flow_dir, inputs, seq_frames, score_window, stats)
+    if world > 1:
+        import torch.distributed as dist
+        every = [None] * world
+        dist.all_gather_object(every, mine, group=pg)
+        merged = {s: [v for r in range(world) for v in every[r][s]] for s in seq_frames}
+    else:
+        merged = mine
+    if rank != 0:
+        return None
+    resolutions = {s: read_frame(files[0]).shape[:2] for s, files in seq_frames.items()}
+    plan = clip_boundaries(len(inputs)) if clips else None
+    return report(name, len(inputs) - 1, resolutions, folders, merged, plan)
+
+
+def write(doc, name):
+    path = os.path.join("results", name, "flicker.json")
+    os.makedirs(os.path.dirname(path), exist_ok=True)
+    with open(path, "w") as f:
+        f.write(json.dumps(doc, indent=1) + "\n")
+    return path
+
+
+def ensure_flows(name, rank=0, world=1):
+    """Computes the flow pairs of the input that are missing, with the pre-pass (sharded over the ranks)."""
+    from src import preprocess_optical_flow as P
+    vid = Path(sequence_folders(name)["input"])
+    frames = frame_files(vid)
+    missing = P.pending_pairs(vid.parent / (vid.name + "_flow"), frames, 0, max(len(frames) - 1, 0))
+    if world > 1:
+        import torch.distributed as dist
+        flag = [bool(missing)]
+        dist.broadcast_object_list(flag, src=0)
+        if flag[0]:
+            P.preprocess_sharded(vid, rank, world)
+    elif missing:
+        P.preprocess(argparse.Namespace(vid_path=vid, max_long_edge=2000))
+
+
+def main(argv=None):
+    cli = argparse.ArgumentParser(description="temporal warping error of a video's sequences")
+    cli.add_argument("--video_name", required=True)
+    cli.add_argument("--sequences", default=",".join(SEQUENCES),
+                     help="comma-separated subset of " + ",".join(SEQUENCES) + "; those whose folder has frames are scored")
+    cli.add_argument("--gpu", type=int, default=0)
+    cli.add_argument("--gpus", type=int, default=1, help="split the frame pairs over this many GPUs of the node")
+    cli.add_argument("--clips", action="store_true",
+                     help="list the pairs that straddle two of stage 1's --clips atlases apart")
+    opts = cli.parse_args(argv)
+    sequences = [s for s in opts.sequences.split(",") if s]
+    bad = [s for s in sequences if s not in SEQUENCES]
+    if bad or not sequences:
+        cli.error("unknown sequence(s) %s; choose from %s" % (",".join(bad), ",".join(SEQUENCES)))
+    from b200 import launch
+    env = launch.torchrun_env()
+    if env is None and opts.gpus > 1:
+        return launch.relaunch(__file__, sys.argv[1:] if argv is None else argv, opts.gpus)
+    if env is None:
+        os.environ["CUDA_VISIBLE_DEVICES"] = str(opts.gpu)
+        rank, world, device = 0, 1, "cuda:0"
+    else:
+        rank, world = env[0], env[1]
+        device, _ = launch.init(env[2])
+    from b200.flicker import FlickerScorer
+    ensure_flows(opts.video_name, rank, world)
+    scorer = FlickerScorer(device)
+    doc = evaluate(opts.video_name, sequences, scorer.score_window, rank, world, clips=opts.clips)
+    if rank == 0:
+        print("wrote", write(doc, opts.video_name))
+        print(table(doc), flush=True)
+    if env is not None:
+        launch.finish()
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())

@@ -18,6 +18,8 @@ parser.add_argument('--gpus', type=int, default=1,
 parser.add_argument('--class_name', type=str, default=None)
 parser.add_argument('--clips', action='store_true',
                     help="stage 1 fits a video longer than maximum_number_of_frames as clips, one atlas each")
+parser.add_argument('--evaluate_flicker', action='store_true',
+                    help="after stage 2, score the warping error of the input and of every output (results/<name>/flicker.json)")
 parser.add_argument('--ckpt_filter', type=str, default="./pretrained_weights/neural_filter.pth")
 parser.add_argument('--ckpt_local', type=str, default="./pretrained_weights/local_refinement_net.pth")
 
@@ -79,4 +81,12 @@ if __name__ == "__main__":
     rc = subprocess.call(stage1)
     if rc != 0:
         sys.exit(rc)
-    sys.exit(subprocess.call(stage2))
+    rc = subprocess.call(stage2)
+    if rc != 0 or not args.evaluate_flicker:
+        sys.exit(rc)
+    flicker = [sys.executable, os.path.join(HERE, "src", "evaluate_flicker.py"), "--video_name", name, "--gpu", str(args.gpu)]
+    if args.gpus > 1:
+        flicker += ["--gpus", str(args.gpus)]
+    if args.clips:
+        flicker += ["--clips"]
+    sys.exit(subprocess.call(flicker))

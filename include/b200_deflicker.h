@@ -528,6 +528,40 @@ int b200_frame_sse(const B200Video* video, int32_t frame, const float* rgb, doub
                    int64_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Temporal warping error of frame pairs (no reference counterpart; the metric of
+ * fast_blind_video_consistency that the paper scores deflickering with; DESIGN §4e).  For frames t
+ * and t+1 (frame0, frame1: (H, W, 3) uint8 or uint16 HWC, decoded as v / 255 or v / 65535 in fp32)
+ * and the pre-pass flows fwd = F (t -> t+1) and bwd = B (t+1 -> t), (Hf, Wf, 2) fp32 (x, y): at
+ * every pixel p, q = p + F(p); p is in the mask when q lies in [0, W-1] x [0, H-1] and
+ * |F + B~|^2 <= 0.01 (|F|^2 + |B~|^2) + 0.5, B~ = bilinear sample of B at q.  The pair's error is
+ * the sum over the mask of sum_c (frame0(p, c) - bilinear sample of frame1 at q)^2.  Flows of
+ * another size are first resized to (H, W) in the workspace (cv2.resize INTER_LINEAR arithmetic in
+ * fp32), x scaled by W / Wf and y by H / Hf.
+ * ------------------------------------------------------------------------------------------ */
+#define B200_WARP_MAX_PAIRS 32
+typedef struct {
+  const void* frame0;     /* frame t   (H, W, 3), uint8 when bits == 8, uint16 when bits == 16 */
+  const void* frame1;     /* frame t+1 (H, W, 3), the same type */
+  const float* fwd;       /* F (Hf, Wf, 2), 8-byte aligned */
+  const float* bwd;       /* B (Hf, Wf, 2), 8-byte aligned */
+  int32_t H, W;           /* the frames' size: the resolution the pair is scored at */
+  int32_t Hf, Wf;         /* the flows' size */
+  int32_t bits;           /* 8 or 16 */
+  int32_t reserved;
+} B200WarpPair;
+/* bytes of workspace a call on these pairs needs; -1 (message) for an invalid table */
+int64_t b200_warp_error_workspace_bytes(const B200WarpPair* pairs_host, int32_t n);
+/* Scores n (1..B200_WARP_MAX_PAIRS) pairs in one launch sequence.  sums [n][2] float64: the masked
+ * squared-error sum and the mask's pixel count.  error (fp32) and mask (uint8), each NULL or one
+ * value per pixel, pair after pair: error = the pixel's sum over c of the squared difference where q
+ * lies in the frame (0 where it does not), mask = 1 in the mask.  The per-pixel arithmetic is
+ * float64, the error is rounded to fp32 once, and sums[i][0] is the float64 sum of those fp32
+ * values over the mask in an order that depends on H * W only (no atomics): bit-identical across
+ * calls, graph replays, batch compositions and devices. */
+int b200_warp_error(const B200WarpPair* pairs_host, int32_t n, double* sums, float* error, uint8_t* mask,
+                    void* ws, int64_t ws_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * RAFT correlation — replaces CorrBlock (src/models/stage_1/core/corr.py:16-64) with an all-pairs pyramid, and
  * AlternateCorrBlock (corr.py:67-91) with the on-the-fly b200_corr_alt_* calls below, which take the place of the
  * reference's unshipped alt_cuda_corr extension.
