@@ -167,6 +167,7 @@ SIGNATURES = {
     "b200_frame_sse": (C.c_int, [C.POINTER(Video), _I32, _P, _P, _P, _I64, _P]),
     "b200_warp_error_workspace_bytes": (_I64, [C.POINTER(WarpPair), _I32]),
     "b200_warp_error": (C.c_int, [C.POINTER(WarpPair), _I32, _P, _P, _P, _P, _I64, _P]),
+    "b200_blend_frames": (C.c_int, [_P, _P, _I64, C.c_double, _P, _P, _P]),
     "b200_render_workspace_bytes": (_I64, [_I64]),
     "b200_render": (C.c_int, [_P, _I32, _I32, _I32, _I32, _I64, _I64, _P, _P, C.c_int, _P, _I64, _P]),
     "b200_corr_pyramid_floats": (_I64, [_I32, _I32]),

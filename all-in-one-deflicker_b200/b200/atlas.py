@@ -713,6 +713,23 @@ def psnr_device(video: DeviceVideo, f: int, rgb: torch.Tensor) -> float:
     return float(10.0 * math.log10(1.0 / (sse / (video.H * video.W * 3))))
 
 
+def blend_frames(a: torch.Tensor, b: torch.Tensor, w: float, out: Optional[torch.Tensor] = None,
+                 u8: Optional[torch.Tensor] = None, want_out: bool = True, want_u8: bool = False):
+    """b200_blend_frames: (1 - w) a + w b of two fp32 device tensors of one shape, in float64 rounded to fp32 once,
+    and its 8-bit quantisation as a render writes it.  Returns (out, u8) with the unrequested one None; `out` and `u8`
+    may be passed (graph capture)."""
+    if a.dtype != torch.float32 or b.dtype != torch.float32 or a.shape != b.shape or a.device.type != "cuda":
+        raise N.B200Error("blend_frames takes two fp32 device tensors of one shape")
+    a, b = a.contiguous(), b.contiguous()
+    if want_out and out is None:
+        out = torch.empty_like(a)
+    if want_u8 and u8 is None:
+        u8 = torch.empty(a.shape, dtype=torch.uint8, device=a.device)
+    N.check(N.lib().b200_blend_frames(N.ptr(a), N.ptr(b), a.numel(), float(w), N.ptr(out), N.ptr(u8),
+                                      N.current_stream()), "b200_blend_frames")
+    return out, u8
+
+
 def frame_range(rank: int, world: int, T: int):
     """Contiguous frame block owned by `rank` (SURVEY §8e): [t_begin, t_end)."""
     base, rem = divmod(T, world)
@@ -720,17 +737,49 @@ def frame_range(rank: int, world: int, T: int):
     return t0, t0 + base + (1 if rank < rem else 0)
 
 
-def clip_plan(T: int, max_frames: int) -> List[Tuple[int, int]]:
-    """The clips a T-frame video is fitted in, one atlas each: K = ceil(T / max_frames) contiguous frame ranges in
-    frame order, none longer than max_frames, their lengths differing by at most one.  T <= max_frames: [(0, T)]."""
-    K = max(1, -(-int(T) // int(max_frames)))
-    return [frame_range(k, K, T) for k in range(K)]
+def clip_plan(T: int, max_frames: int, overlap: int = 0) -> List[Tuple[int, int]]:
+    """The clips a T-frame video is fitted in, one atlas each, in frame order, none longer than max_frames (M), their
+    lengths differing by at most one, consecutive clips sharing exactly `overlap` (V) frames.  K = max(1,
+    ceil((T - V) / (M - V))), the least number of clips that can do so: the T + (K - 1) V frame slots are spread with
+    frame_range and clip k is shifted left by k V.  T <= M: [(0, T)].  V = 0 gives contiguous clips,
+    K = ceil(T / M).  Refused unless 0 <= V and 3 V + 1 <= M, which keeps at least one frame of every clip outside
+    its two overlap zones whatever T is."""
+    T, M, V = int(T), int(max_frames), int(overlap)
+    if V < 0 or 3 * V + 1 > M:
+        raise N.B200Error(f"clip overlap {V} with maximum_number_of_frames {M}: the overlap must be >= 0 and "
+                          f"3 * overlap + 1 <= maximum_number_of_frames (at most {max((M - 1) // 3, 0)} here)")
+    if T <= M:
+        return [(0, T)]
+    K = -(-(T - V) // (M - V))
+    slots = T + (K - 1) * V
+    return [(a - k * V, b - k * V) for k, (a, b) in ((k, frame_range(k, K, slots)) for k in range(K))]
 
 
-def video_clips(config: dict, n_frames: int) -> List[Tuple[int, int]]:
-    """clip_plan of an n_frames video under the config's maximum_number_of_frames.  Refused when there is more than
-    one clip and the config resumes from `checkpoint_path`, which holds one atlas."""
-    clips = clip_plan(n_frames, config["maximum_number_of_frames"])
+def clip_seams(plan: List[Tuple[int, int]]) -> List[Tuple[int, int]]:
+    """For each seam k between clips k and k+1 of a plan, the frames [a, b) they share: [c0 of clip k+1, c1 of clip
+    k).  Empty (a == b) for contiguous clips."""
+    return [(plan[k + 1][0], plan[k][1]) for k in range(len(plan) - 1)]
+
+
+def seam_weights(overlap: int) -> List[float]:
+    """Weight of clip k+1's render for the frames a + j, j = 0 .. V-1, of a seam: w_j = (j + 1) / (V + 1); clip k's
+    render takes 1 - w_j.  The jump between the two atlases is spread over V + 1 frame steps."""
+    V = int(overlap)
+    return [(j + 1) / (V + 1) for j in range(V)]
+
+
+def clip_own_frames(clip: Tuple[int, int], n_frames: int, overlap: int) -> Tuple[int, int]:
+    """The frames [a, b) of an n_frames video that a clip of clip_plan(n_frames, M, overlap) renders alone: the clip
+    less the `overlap` frames it shares with each neighbour.  The shared frames are written by the stitch."""
+    c0, c1 = clip
+    return c0 + (overlap if c0 > 0 else 0), c1 - (overlap if c1 < n_frames else 0)
+
+
+def video_clips(config: dict, n_frames: int, overlap: int = 0) -> List[Tuple[int, int]]:
+    """clip_plan of an n_frames video under the config's maximum_number_of_frames, consecutive clips sharing
+    `overlap` frames.  Refused when there is more than one clip and the config resumes from `checkpoint_path`, which
+    holds one atlas."""
+    clips = clip_plan(n_frames, config["maximum_number_of_frames"], overlap)
     if len(clips) > 1 and config.get("load_checkpoint"):
         raise N.B200Error(f"--clips fits {len(clips)} atlases to this {n_frames}-frame video (maximum_number_of_frames "
                           f"= {config['maximum_number_of_frames']}), but load_checkpoint resumes one atlas from "
@@ -741,6 +790,11 @@ def video_clips(config: dict, n_frames: int) -> List[Tuple[int, int]]:
 def rank_clips(clips: List[Tuple[int, int]], rank: int, world: int) -> List[Tuple[int, int]]:
     """The clips rank `rank` of `world` fits: clip k for k = rank (mod world)."""
     return clips[rank::world]
+
+
+def rank_seams(seams: List[Tuple[int, int]], rank: int, world: int) -> List[int]:
+    """The seams rank `rank` of `world` stitches: seam k for k = rank (mod world), as indices into `seams`."""
+    return list(range(len(seams)))[rank::world]
 
 
 def clip_name(clip: Tuple[int, int]) -> str:

@@ -1,7 +1,8 @@
 """Flicker of a video's sequences: the temporal warping error of the input, the stage-1 atlas reconstruction, the
 neural filter's output and the final output, computed on the GPU (b200.flicker; DESIGN §4e).
 
-    python src/evaluate_flicker.py --video_name NAME [--sequences input,atlas,filter,final] [--gpus N] [--clips]
+    python src/evaluate_flicker.py --video_name NAME [--sequences input,atlas,filter,final] [--gpus N]
+                                   [--clips [--clip_overlap V]]
 
 Run from the directory that holds data/test/NAME (the pipeline's working directory).  Pair t uses the flow pre-pass's
 files data/test/NAME_flow/<t>_<t+1>.npy (F) and <t+1>_<t>.npy (B) of the input's sorted frames; missing pairs are
@@ -94,13 +95,15 @@ def score_pairs(p0, p1, flow_dir, inputs, seq_frames, score_window, stats=None):
     return out
 
 
-def clip_boundaries(n_frames):
-    """The pairs (c1 - 1, c1) that straddle two clips of the plan stage 1's --clips fits an n_frames video in."""
-    from b200.atlas import clip_plan
+def clip_boundaries(n_frames, overlap=0):
+    """The pairs of the seams of the plan stage 1's --clips (--clip_overlap V) fits an n_frames video in: for the
+    frames [a, b) two clips share, the pairs t = a - 1 .. b - 1 (the step into the cross-fade, the V - 1 steps inside
+    it and the step out).  With V = 0 that is the one pair (c1 - 1, c1) that straddles two clips."""
+    from b200.atlas import clip_plan, clip_seams
     with open(CONFIG) as f:
         max_frames = json.load(f)["maximum_number_of_frames"]
-    plan = clip_plan(n_frames, max_frames)
-    return plan, [c1 - 1 for _, c1 in plan[:-1]]
+    plan = clip_plan(n_frames, max_frames, overlap)
+    return plan, [t for a, b in clip_seams(plan) for t in range(a - 1, b)]
 
 
 def _mean(values):
@@ -144,7 +147,7 @@ def table(doc):
     return "\n".join(lines)
 
 
-def evaluate(name, sequences, score_window, rank=0, world=1, pg=None, clips=False, stats=None):
+def evaluate(name, sequences, score_window, rank=0, world=1, pg=None, clips=False, stats=None, clip_overlap=0):
     """Scores rank's block of pairs; under a process group the blocks are gathered in pair order.  Returns the
     flicker.json document on rank 0 (None on the other ranks)."""
     folders = sequence_folders(name)
@@ -174,7 +177,7 @@ def evaluate(name, sequences, score_window, rank=0, world=1, pg=None, clips=Fals
     if rank != 0:
         return None
     resolutions = {s: read_frame(files[0]).shape[:2] for s, files in seq_frames.items()}
-    plan = clip_boundaries(len(inputs)) if clips else None
+    plan = clip_boundaries(len(inputs), clip_overlap) if clips else None
     return report(name, len(inputs) - 1, resolutions, folders, merged, plan)
 
 
@@ -211,7 +214,12 @@ def main(argv=None):
     cli.add_argument("--gpus", type=int, default=1, help="split the frame pairs over this many GPUs of the node")
     cli.add_argument("--clips", action="store_true",
                      help="list the pairs that straddle two of stage 1's --clips atlases apart")
+    cli.add_argument("--clip_overlap", type=int, default=0,
+                     help="with --clips: the frames consecutive clips share (stage 1's --clip_overlap); the pairs "
+                          "into, inside and out of each cross-fade are listed")
     opts = cli.parse_args(argv)
+    if opts.clip_overlap != 0 and not opts.clips:
+        cli.error("--clip_overlap is only meaningful with --clips")
     sequences = [s for s in opts.sequences.split(",") if s]
     bad = [s for s in sequences if s not in SEQUENCES]
     if bad or not sequences:
@@ -229,7 +237,8 @@ def main(argv=None):
     from b200.flicker import FlickerScorer
     ensure_flows(opts.video_name, rank, world)
     scorer = FlickerScorer(device)
-    doc = evaluate(opts.video_name, sequences, scorer.score_window, rank, world, clips=opts.clips)
+    doc = evaluate(opts.video_name, sequences, scorer.score_window, rank, world, clips=opts.clips,
+                   clip_overlap=opts.clip_overlap)
     if rank == 0:
         print("wrote", write(doc, opts.video_name))
         print(table(doc), flush=True)

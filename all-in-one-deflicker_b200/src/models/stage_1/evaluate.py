@@ -4,6 +4,7 @@ per-pixel maps and PSNR run in libb200deflicker.so; the reconstruction / residua
 composed with OpenCV (`ArtefactWriter`), tensorboard images go through torch.utils.tensorboard.  The texture-editing
 part of the segmentation variant's evaluation (:234-262, :340-600) is interactive-editing tooling and is not provided."""
 import os
+import time
 
 import cv2
 import numpy as np
@@ -71,9 +72,10 @@ class ArtefactWriter:
 
 def evaluate_model_single(trainer, resx, resy, number_of_frames, video_frames, results_folder, iteration,
                           vid_name=None, save_checkpoint=True, artefacts=False, writer=None, output_folder=None,
-                          frame_offset=0):
+                          frame_offset=0, write_frames=None):
     """Frame f's reconstruction goes to `<output_folder>/%05d.png % (frame_offset + f)` (default `<results_folder>/output`,
-    offset 0): a clip of a longer video writes its frames where they lie in the video."""
+    offset 0): a clip of a longer video writes its frames where they lie in the video.  With `write_frames` (a
+    collection of frames f) only those frames' files are written; everything else, PSNR included, covers every frame."""
     output_folder = os.path.join(results_folder, "output") if output_folder is None else output_folder
     os.makedirs(os.path.join(results_folder, '%06d' % iteration), exist_ok=True)
     os.makedirs(output_folder, exist_ok=True)
@@ -88,8 +90,9 @@ def evaluate_model_single(trainer, resx, resy, number_of_frames, video_frames, r
     ends = {}
     for f in range(number_of_frames):
         img, u8 = trainer.render_frame(f, int(resy), int(resx), number_of_frames, want_u8=True)
-        cv2.imwrite(os.path.join(output_folder, '%05d.png' % (frame_offset + f)),
-                    cv2.cvtColor(u8.cpu().numpy(), cv2.COLOR_RGB2BGR))       # evaluate.py:732-733
+        if write_frames is None or f in write_frames:
+            cv2.imwrite(os.path.join(output_folder, '%05d.png' % (frame_offset + f)),
+                        cv2.cvtColor(u8.cpu().numpy(), cv2.COLOR_RGB2BGR))   # evaluate.py:732-733
         psnrs[f] = A.psnr(video_frames[:, :, :, f], img.cpu())               # :740-743
         if art is not None:                                                  # :668-779, maps computed on the device
             uv, rig, flow = trainer.eval_maps(f)
@@ -108,11 +111,11 @@ def evaluate_model_single(trainer, resx, resy, number_of_frames, video_frames, r
 
 
 def evaluate_model(trainer, resx, resy, number_of_frames, video_frames, results_folder, iteration, mask_frames=None,
-                   vid_name=None, save_checkpoint=True, output_folder=None, frame_offset=0):
+                   vid_name=None, save_checkpoint=True, output_folder=None, frame_offset=0, write_frames=None):
     """Segmentation variant (evaluate.py:203-602): checkpoint with the reference's keys (:216-233), the composite
     reconstruction (:293-335) written to `output/`, the alpha mattes to `<iteration>/alpha/`, PSNR.  Texture editing,
-    atlas dumps and per-pixel loss videos are visualisation (out of scope).  `output_folder` and `frame_offset` as in
-    evaluate_model_single; the alpha mattes keep the clip's own frame numbers."""
+    atlas dumps and per-pixel loss videos are visualisation (out of scope).  `output_folder`, `frame_offset` and
+    `write_frames` as in evaluate_model_single; the alpha mattes keep the clip's own frame numbers."""
     output_folder = os.path.join(results_folder, "output") if output_folder is None else output_folder
     folder = os.path.join(results_folder, '%06d' % iteration)
     os.makedirs(os.path.join(folder, "alpha"), exist_ok=True)
@@ -127,8 +130,9 @@ def evaluate_model(trainer, resx, resy, number_of_frames, video_frames, results_
     psnrs = np.zeros((number_of_frames, 1))
     for f in range(number_of_frames):
         img, alpha, u8 = trainer.render_frame(f, int(resy), int(resx), number_of_frames, want_u8=True)
-        cv2.imwrite(os.path.join(output_folder, '%05d.png' % (frame_offset + f)),
-                    cv2.cvtColor(u8.cpu().numpy(), cv2.COLOR_RGB2BGR))
+        if write_frames is None or f in write_frames:
+            cv2.imwrite(os.path.join(output_folder, '%05d.png' % (frame_offset + f)),
+                        cv2.cvtColor(u8.cpu().numpy(), cv2.COLOR_RGB2BGR))
         cv2.imwrite(os.path.join(folder, 'alpha', '%05d.png' % f), (alpha.cpu().numpy() * 255).astype(np.uint8))
         psnrs[f] = A.psnr(video_frames[:, :, :, f], img.cpu())
     open(os.path.join(folder, "PSNR_%f" % psnrs.mean()), "w").close()
@@ -160,15 +164,17 @@ def artefact_payload_bytes(resx, resy):
     return 3 * resy * resx * 3 + 2 * (resy + 22) * 3 * resx * 3
 
 
-def evaluate_block_single(trainer, resx, resy, number_of_frames, results_folder, artefacts=False):
-    """The frames of trainer.video's resident block: writes `output/%05d.png`, returns (per-frame PSNR, packed artefact
-    images per frame or []).  The PSNR's squared error is summed on the device against the resident records
+def evaluate_block_single(trainer, resx, resy, number_of_frames, results_folder, artefacts=False, write_frames=None):
+    """The frames of trainer.video's resident block: writes `output/%05d.png` (of the frames in `write_frames` only,
+    when given), returns (per-frame PSNR, packed artefact images per frame or []).  The PSNR's squared error is summed on the device against the resident records
     (b200_frame_sse), and the original frame of the artefact images is read from them too."""
     video = trainer.video
     psnrs, payloads = [], []
     for f in range(video.t_begin, video.t_end):
         img, u8 = trainer.render_frame(f, int(resy), int(resx), number_of_frames, want_u8=True)
-        cv2.imwrite(os.path.join(results_folder, 'output', '%05d.png' % f), cv2.cvtColor(u8.cpu().numpy(), cv2.COLOR_RGB2BGR))
+        if write_frames is None or f in write_frames:
+            cv2.imwrite(os.path.join(results_folder, 'output', '%05d.png' % f),
+                        cv2.cvtColor(u8.cpu().numpy(), cv2.COLOR_RGB2BGR))
         psnrs.append(A.psnr_device(video, f, img))
         if artefacts:
             uv, rig, flow = trainer.eval_maps(f)
@@ -199,7 +205,8 @@ def write_evaluation_single(trainer, resx, resy, number_of_frames, results_folde
 
 
 def evaluate_model_single_sharded(trainer, resx, resy, number_of_frames, results_folder, iteration, vid_name=None,
-                                  save_checkpoint=True, artefacts=False, writer=None, process_group=None):
+                                  save_checkpoint=True, artefacts=False, writer=None, process_group=None,
+                                  write_frames=None):
     """evaluate_model_single over a process group whose ranks hold contiguous frame blocks (collective): the same
     checkpoint (written by rank 0 after the collective optimizer_state_dict), frames, marker and videos."""
     import torch.distributed as dist
@@ -216,7 +223,8 @@ def evaluate_model_single_sharded(trainer, resx, resy, number_of_frames, results
                         'model_F_mapping1_state_dict': {k: v.cpu() for k, v in trainer.state_dict("mapping").items()},
                         'optimizer_all_state_dict': opt},
                        '%s/checkpoint' % results_folder)
-    psnrs, payloads = evaluate_block_single(trainer, resx, resy, number_of_frames, results_folder, artefacts)
+    psnrs, payloads = evaluate_block_single(trainer, resx, resy, number_of_frames, results_folder, artefacts,
+                                            write_frames)
     merged = launch.gather_frame_values(psnrs, pg)
     received = []
     if artefacts:
@@ -230,22 +238,25 @@ def evaluate_model_single_sharded(trainer, resx, resy, number_of_frames, results
     return mean
 
 
-def evaluate_block_seg(trainer, resx, resy, number_of_frames, results_folder, iteration):
-    """Segmentation variant: the frames of trainer.video's block — `output/%05d.png`, `<iteration>/alpha/%05d.png` —
-    and their PSNR (device squared error against the resident records)."""
+def evaluate_block_seg(trainer, resx, resy, number_of_frames, results_folder, iteration, write_frames=None):
+    """Segmentation variant: the frames of trainer.video's block — `output/%05d.png` (of the frames in `write_frames`
+    only, when given), `<iteration>/alpha/%05d.png` — and their PSNR (device squared error against the resident
+    records)."""
     folder = os.path.join(results_folder, '%06d' % iteration)
     video = trainer.video
     psnrs = []
     for f in range(video.t_begin, video.t_end):
         img, alpha, u8 = trainer.render_frame(f, int(resy), int(resx), number_of_frames, want_u8=True)
-        cv2.imwrite(os.path.join(results_folder, 'output', '%05d.png' % f), cv2.cvtColor(u8.cpu().numpy(), cv2.COLOR_RGB2BGR))
+        if write_frames is None or f in write_frames:
+            cv2.imwrite(os.path.join(results_folder, 'output', '%05d.png' % f),
+                        cv2.cvtColor(u8.cpu().numpy(), cv2.COLOR_RGB2BGR))
         cv2.imwrite(os.path.join(folder, 'alpha', '%05d.png' % f), (alpha.cpu().numpy() * 255).astype(np.uint8))
         psnrs.append(A.psnr_device(video, f, img))
     return psnrs
 
 
 def evaluate_model_sharded(trainer, resx, resy, number_of_frames, results_folder, iteration, vid_name=None,
-                           save_checkpoint=True, process_group=None):
+                           save_checkpoint=True, process_group=None, write_frames=None):
     """evaluate_model over a process group whose ranks hold contiguous frame blocks (collective)."""
     import torch.distributed as dist
     from b200 import launch
@@ -263,11 +274,59 @@ def evaluate_model_sharded(trainer, resx, resy, number_of_frames, results_folder
                   'optimizer_all_state_dict': opt}
             torch.save(ck, '%s/checkpoint' % results_folder)
             torch.save(ck, '%s/checkpoint' % folder)
-    merged = launch.gather_frame_values(evaluate_block_seg(trainer, resx, resy, number_of_frames, results_folder, iteration),
-                                        pg)
+    merged = launch.gather_frame_values(evaluate_block_seg(trainer, resx, resy, number_of_frames, results_folder, iteration,
+                                                           write_frames), pg)
     mean = float(np.mean(merged))
     if rank == 0:
         open(os.path.join(folder, "PSNR_%f" % mean), "w").close()
         print("PSNR: %f" % mean)
     dist.barrier(pg)
     return mean
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Seams of overlapping clips (--clips --clip_overlap V): the V frames two consecutive clips share are a cross-fade of
+# the two atlases' renders, so the jump between the atlases is spread over V + 1 frame steps (DESIGN §5).
+
+def _render_rgb(trainer, f, H, W, T):
+    out = trainer.render_frame(f, H, W, T)
+    return out[0] if isinstance(out, tuple) else out          # SegTrainer: (rgb, alpha)
+
+
+def stitch_seams(plan, make_trainer, stage_folder, resx, resy, rank=0, world=1):
+    """Writes the shared frames of the seams of `plan` (b200.atlas.clip_plan with an overlap) that rank `rank` of
+    `world` owns (seam k for k = rank mod world, atlas.rank_seams) to `<stage_folder>/output/%05d.png`.  Frame a + j
+    of seam k, [a, b) = atlas.clip_seams(plan)[k], is b200_blend_frames of clip k's and clip k+1's renders, each at
+    its own clip-local frame index and frame count, with the weight w_j = (j + 1) / (V + 1) of atlas.seam_weights on
+    clip k+1, quantised and written (RGB -> BGR) as the evaluation writes a frame.  `make_trainer(path)` builds a
+    render-only trainer of the variant from a clip's `checkpoint` file: the parameters of the clip's last
+    evaluation, which wrote its other frames.  Every checkpoint must exist, so ranks call this after the clips'
+    barrier; when a clip has none (no evaluation ran, and no frame was written) nothing is stitched.  Returns the
+    number of frames written."""
+    seams = A.clip_seams(plan)
+    checkpoints = [os.path.join(str(stage_folder), A.clip_name(c), "checkpoint") for c in plan]
+    missing = [p for p in checkpoints if not os.path.exists(p)]
+    if missing:
+        if rank == 0:
+            print("stitch: no evaluation wrote %s; nothing was stitched" % missing[0], flush=True)
+        return 0
+    output_folder = os.path.join(str(stage_folder), "output")
+    os.makedirs(output_folder, exist_ok=True)
+    H, W = int(resy), int(resx)
+    written, start = 0, time.perf_counter()
+    for k in A.rank_seams(seams, rank, world):
+        (a, b), (l0, l1), (r0, r1) = seams[k], plan[k], plan[k + 1]
+        if b <= a:
+            continue
+        left, right = make_trainer(checkpoints[k]), make_trainer(checkpoints[k + 1])
+        for j, w in enumerate(A.seam_weights(b - a)):
+            t = a + j
+            _, u8 = A.blend_frames(_render_rgb(left, t - l0, H, W, l1 - l0), _render_rgb(right, t - r0, H, W, r1 - r0), w,
+                                   want_out=False, want_u8=True)
+            cv2.imwrite(os.path.join(output_folder, '%05d.png' % t), cv2.cvtColor(u8.cpu().numpy(), cv2.COLOR_RGB2BGR))
+            written += 1
+        left.release()
+        right.release()
+    print("stitch: rank %d wrote %d frames of %d seams in %.2f s" % (rank, written, len(A.rank_seams(seams, rank, world)),
+                                                                   time.perf_counter() - start), flush=True)
+    return written

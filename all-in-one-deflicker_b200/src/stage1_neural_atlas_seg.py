@@ -3,14 +3,16 @@ CLI, config keys, on-disk inputs and outputs as the reference script (src/stage1
 loop body (:195-319) runs in libb200deflicker.so (b200_seg_loss_grad + b200_adam_step).
 
     python src/stage1_neural_atlas_seg.py --vid_name NAME --class_name portrait [--config config_flow_100.json]
-                                          [--root data/test/] [--down 1] [--gpu 0] [--gpus 1] [--clips]
+                                          [--root data/test/] [--down 1] [--gpu 0] [--gpus 1]
+                                          [--clips [--clip_overlap V]]
 
 With --gpus N > 1 the script re-runs itself under `python -m torch.distributed.run --nproc-per-node N`; under torchrun
 (any world size) every rank computes a block of the flow pairs, holds a block of the frames and their mattes and
 evaluates those frames.
 
 With --clips a video longer than maximum_number_of_frames is fitted as clips (b200.atlas.clip_plan), one atlas each,
-the clips spread over the ranks under torchrun; see `fit_clips`.
+the clips spread over the ranks under torchrun; see `fit_clips`.  With --clip_overlap V consecutive clips share V
+frames, which are written once every clip is fitted as a cross-fade of the two atlases' renders; see `stitch`.
 
 The mattes of `<root>/<NAME>_seg/` are an input: the reference produces them with third-party models (CarveKit /
 detectron2 Mask-RCNN, src/preprocess_mask_*.py) that this repository does not ship; the script stops with a clear
@@ -36,25 +38,33 @@ from tqdm import tqdm  # noqa: E402
 from b200 import _native as N  # noqa: E402
 from b200 import atlas as A    # noqa: E402
 from b200 import seg as SG     # noqa: E402
-from src.models.stage_1.evaluate import evaluate_model  # noqa: E402
+from src.models.stage_1.evaluate import evaluate_model, stitch_seams  # noqa: E402
 from src.models.stage_1.unwrap_utils import load_mask_frames, mask_files, pre_train_mapping  # noqa: E402
 
 
-def main(config, args, clip=None, device=None):
-    """Fit the two-layer atlas of the video on `device` (default: the current CUDA device).  With `clip` = (c0, c1):
-    the run on a folder holding only frames [c0, c1), their flows and their mattes, its files under
-    stage_1/clip_<c0>_<c1>/ except the output frames, which go to stage_1/output/ at their frame numbers in the whole
-    video."""
+def frame_size(args):
+    """(resx, resy) the video is fitted at: its first frame's size divided by --down."""
     frames_list = sorted(glob.glob(os.path.join(args.vid_path, "*g")))
     first = cv2.imread(frames_list[0])
     resx, resy = first.shape[1], first.shape[0]
     if args.down is not None:
         resx, resy = int(resx / args.down), int(resy / args.down)
+    return resx, resy
+
+
+def main(config, args, clip=None, device=None, own=None):
+    """Fit the two-layer atlas of the video on `device` (default: the current CUDA device).  With `clip` = (c0, c1):
+    the run on a folder holding only frames [c0, c1), their flows and their mattes, its files under
+    stage_1/clip_<c0>_<c1>/ except the output frames, which go to stage_1/output/ at their frame numbers in the whole
+    video; with `own` = (a, b) the output frames of [a, b) only (the frames the clip shares with no other clip)."""
+    resx, resy = frame_size(args)
     data_folder = Path(args.vid_path)
     vid_name, vid_root = data_folder.name, data_folder.parent
     stage_folder = Path(f'./results/{vid_name}/stage_1')
     results_folder = stage_folder if clip is None else stage_folder / A.clip_name(clip)
     output = {} if clip is None else dict(output_folder=str(stage_folder / "output"), frame_offset=clip[0])
+    if own is not None:
+        output["write_frames"] = range(own[0] - clip[0], own[1] - clip[0])
     results_folder.mkdir(parents=True, exist_ok=True)
     with open('%s/config.json' % results_folder, 'w') as f:
         json.dump(config, f, indent=4)
@@ -95,17 +105,37 @@ def main(config, args, clip=None, device=None):
     trainer.release()
 
 
-def fit_clips(config, args, clips, device, seed):
+def fit_clips(config, args, clips, device, seed, overlap=0):
     """Fit one two-layer atlas per clip of `clips` on `device`, in order, with no process group: clip k is
     `main(config, args, clip)`, started from the CPU generator seeded with `seed`, so its files are those of a
     stand-alone run on a folder holding only its frames and mattes.  Nothing of a clip is alive when the next one is
-    loaded."""
+    loaded.  With `overlap` V > 0 (clips of clip_plan(T, M, V)) a clip leaves the output frames it shares with a
+    neighbour to `stitch`."""
+    n_frames = len(A.video_files(args.vid_path))
     for clip in clips:
         torch.manual_seed(seed)
         with torch.cuda.device(device):
-            main(config, args, clip, device)
+            main(config, args, clip, device, A.clip_own_frames(clip, n_frames, overlap) if overlap > 0 else None)
             gc.collect()
             torch.cuda.empty_cache()
+
+
+def stitch(config, args, plan, device, rank=0, world=1):
+    """The frames consecutive clips of `plan` share (--clip_overlap), for the seams rank `rank` of `world` owns:
+    stitch_seams with render-only SegTrainers loaded from the clips' checkpoints, in the precision of the clips'
+    evaluations."""
+    resx, resy = frame_size(args)
+    precision = N.PREC_TC if N.lib().b200_device_supports_tc() else N.PREC_FP32
+
+    def make_trainer(path):
+        ck = torch.load(path, map_location="cpu")
+        trainer = SG.SegTrainer(None, None, config, precision=precision, device=device, resx=resx)
+        trainer.load_state(dict(atlas=ck["F_atlas_state_dict"], mapping1=ck["model_F_mapping1_state_dict"],
+                                mapping2=ck["model_F_mapping2_state_dict"], alpha=ck["model_F_alpha_state_dict"]))
+        return trainer
+    with torch.cuda.device(device):
+        return stitch_seams(plan, make_trainer, Path(f'./results/{Path(args.vid_path).name}/stage_1'), resx, resy,
+                            rank, world)
 
 
 def check_clip_mattes(vid_path, clips):
@@ -122,11 +152,7 @@ def main_sharded(config, args, device, pg):
     from b200 import launch
     from src.models.stage_1.evaluate import evaluate_model_sharded
     rank, world = dist.get_rank(pg), dist.get_world_size(pg)
-    frames_list = sorted(glob.glob(os.path.join(args.vid_path, "*g")))
-    first = cv2.imread(frames_list[0])
-    resx, resy = first.shape[1], first.shape[0]
-    if args.down is not None:
-        resx, resy = int(resx / args.down), int(resy / args.down)
+    resx, resy = frame_size(args)
     data_folder = Path(args.vid_path)
     vid_name, vid_root = data_folder.name, data_folder.parent
     results_folder = Path(f'./results/{vid_name}/stage_1')
@@ -185,7 +211,12 @@ if __name__ == "__main__":
     parser.add_argument('--clips', action='store_true',
                         help="fit a video longer than maximum_number_of_frames as clips of at most that many frames, "
                              "one atlas each (spread over the GPUs with --gpus)")
+    parser.add_argument('--clip_overlap', type=int, default=0,
+                        help="with --clips: consecutive clips share this many frames, written as a cross-fade of the "
+                             "two atlases' renders")
     args = parser.parse_args()
+    if args.clip_overlap != 0 and not args.clips:
+        parser.error("--clip_overlap is only meaningful with --clips")
     from b200 import launch
     env = launch.torchrun_env()
     if env is None and args.gpus > 1:
@@ -194,7 +225,7 @@ if __name__ == "__main__":
     seg_dir = args.vid_path.rstrip("/") + "_seg"
     with open(os.path.join(HERE, "config", args.config)) as f:
         config = json.load(f)
-    clips = A.video_clips(config, len(A.video_files(args.vid_path))) if args.clips else [None]
+    clips = A.video_clips(config, len(A.video_files(args.vid_path)), args.clip_overlap) if args.clips else [None]
     if env is not None:
         if not glob.glob(os.path.join(seg_dir, "*g")):
             raise FileNotFoundError(f"{seg_dir} holds no mattes: produce them with the reference's mask pre-pass "
@@ -205,8 +236,11 @@ if __name__ == "__main__":
         if len(clips) > 1:
             check_clip_mattes(args.vid_path, clips)
             seed, done = launch.shared_seed(pg), launch.patient_group()
-            fit_clips(config, args, A.rank_clips(clips, env[0], env[1]), device, seed)
+            fit_clips(config, args, A.rank_clips(clips, env[0], env[1]), device, seed, args.clip_overlap)
             torch.distributed.barrier(group=done)
+            if args.clip_overlap > 0:
+                stitch(config, args, clips, device, env[0], env[1])
+                torch.distributed.barrier(group=done)
         else:
             main_sharded(config, args, device, pg)
         launch.finish()
@@ -222,6 +256,8 @@ if __name__ == "__main__":
                                 f"(class '{args.class_name}') or any segmentation tool, one image per frame")
     if len(clips) > 1:
         check_clip_mattes(args.vid_path, clips)
-        fit_clips(config, args, clips, torch.device("cuda"), torch.initial_seed())
+        fit_clips(config, args, clips, torch.device("cuda"), torch.initial_seed(), args.clip_overlap)
+        if args.clip_overlap > 0:
+            stitch(config, args, clips, torch.device("cuda"))
     else:
         main(config, args)

@@ -18,6 +18,9 @@ parser.add_argument('--gpus', type=int, default=1,
 parser.add_argument('--class_name', type=str, default=None)
 parser.add_argument('--clips', action='store_true',
                     help="stage 1 fits a video longer than maximum_number_of_frames as clips, one atlas each")
+parser.add_argument('--clip_overlap', type=int, default=0,
+                    help="with --clips: consecutive clips share this many frames, written as a cross-fade of the two "
+                         "atlases' renders")
 parser.add_argument('--evaluate_flicker', action='store_true',
                     help="after stage 2, score the warping error of the input and of every output (results/<name>/flicker.json)")
 parser.add_argument('--ckpt_filter', type=str, default="./pretrained_weights/neural_filter.pth")
@@ -47,6 +50,10 @@ def split_video(path, out_dir, fps):
 
 if __name__ == "__main__":
     args = parser.parse_args()
+    if args.clip_overlap != 0 and not args.clips:
+        parser.error("--clip_overlap is only meaningful with --clips")
+    if args.clip_overlap < 0:
+        parser.error("--clip_overlap must be >= 0")
     # The reference (test.py:17-31) always works on ./data/test/<name>: a video is split into that folder, a frame
     # folder is moved there.  Stage 1 (--root data/test/) and stage 2 (hard-coded ./data/test/<name>) both read it.
     if args.video_name is not None:
@@ -78,6 +85,8 @@ if __name__ == "__main__":
     if args.clips:
         # stage 2 runs over the whole video's output frames as it is
         stage1 += ["--clips"]
+    if args.clip_overlap > 0:
+        stage1 += ["--clip_overlap", str(args.clip_overlap)]
     rc = subprocess.call(stage1)
     if rc != 0:
         sys.exit(rc)
@@ -89,4 +98,6 @@ if __name__ == "__main__":
         flicker += ["--gpus", str(args.gpus)]
     if args.clips:
         flicker += ["--clips"]
+    if args.clip_overlap > 0:
+        flicker += ["--clip_overlap", str(args.clip_overlap)]
     sys.exit(subprocess.call(flicker))

@@ -562,6 +562,16 @@ int b200_warp_error(const B200WarpPair* pairs_host, int32_t n, double* sums, flo
                     void* ws, int64_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Cross-fade of two renders of one frame (no reference counterpart; the seams of overlapping clips,
+ * DESIGN §5).  For each of the n values: o = (float)((1 - w) (double)a + w (double)b), in float64
+ * with one IEEE rounding per operation and no fma, rounded to fp32 once, so w = 0 gives a and
+ * w = 1 gives b exactly (for finite values other than -0); u8 = (uint8_t)(int)((double)o * 255.0),
+ * the conversion of the stage-1 renders.  `out` (fp32) or `u8` may be NULL, not both.  w must be
+ * finite and in [0, 1].  Allocates nothing, does not synchronise, graph-capturable.
+ * ------------------------------------------------------------------------------------------ */
+int b200_blend_frames(const float* a, const float* b, int64_t n, double w, float* out, uint8_t* u8, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * RAFT correlation — replaces CorrBlock (src/models/stage_1/core/corr.py:16-64) with an all-pairs pyramid, and
  * AlternateCorrBlock (corr.py:67-91) with the on-the-fly b200_corr_alt_* calls below, which take the place of the
  * reference's unshipped alt_cuda_corr extension.
