@@ -317,6 +317,7 @@ class FlatTrainer:
 
     NETS = ()                   # flat-buffer order = optimiser-group order
     CONSTRUCTION_ORDER = ()     # order the reference script constructs (and so initialises) the networks
+    CHECKPOINT_KEYS = {}        # network -> key of its state dict in the reference's checkpoint, the atlas first
 
     def __init__(self, video: Optional[DeviceVideo], precision: int, device, lr: float, process_group,
                  resx: Optional[int]):
@@ -426,6 +427,25 @@ class FlatTrainer:
                     step = int(st["step"])
                 idx += 1
         self.step_count.fill_(step)
+
+    def checkpoint(self, iteration: int) -> dict:
+        """The reference's checkpoint (evaluate.py:216-233, :616-622): the atlas's state dict, the iteration, the other
+        networks' state dicts in CHECKPOINT_KEYS order, then optimizer_state_dict(); the state dicts on the CPU.
+        Collective under the fused optimiser: every rank calls it."""
+        cpu = lambda which: {k: v.cpu() for k, v in self.state_dict(which).items()}
+        keys = dict(self.CHECKPOINT_KEYS)
+        ck = {keys.pop("atlas"): cpu("atlas"), "iteration": iteration}
+        ck.update((key, cpu(which)) for which, key in keys.items())
+        ck["optimizer_all_state_dict"] = self.optimizer_state_dict()
+        return ck
+
+    def load_checkpoint(self, ck: dict, optimizer: bool = True) -> int:
+        """Load a `checkpoint` dict: the parameters of every network and, with `optimizer`, the Adam state.  Returns
+        its iteration."""
+        FlatTrainer.load_state(self, {which: ck[key] for which, key in self.CHECKPOINT_KEYS.items()})
+        if optimizer:
+            self.load_optimizer_state_dict(ck["optimizer_all_state_dict"])
+        return ck["iteration"]
 
     # ------------------------------------------------------------------ optimiser and exchange between ranks
     def adam(self, sl: Optional[slice] = None, m=None, v=None, step=None):
@@ -546,6 +566,7 @@ class AtlasTrainer(FlatTrainer):
     """Flat parameters/optimiser state of (mapping, atlas) + the fused step."""
 
     NETS = CONSTRUCTION_ORDER = ("mapping", "atlas")
+    CHECKPOINT_KEYS = dict(atlas="F_atlas_state_dict", mapping="model_F_mapping1_state_dict")
 
     def __init__(self, video: Optional[DeviceVideo], config: Optional[dict] = None, precision: int = N.PREC_FP32,
                  device="cuda", lr: float = 1e-4, process_group=None, resx: Optional[int] = None,

@@ -77,6 +77,8 @@ class SegTrainer(FlatTrainer):
 
     NETS = NETS
     CONSTRUCTION_ORDER = ("mapping1", "mapping2", "atlas", "alpha")   # order the script builds them (:127-161)
+    CHECKPOINT_KEYS = dict(atlas="F_atlas_state_dict", mapping1="model_F_mapping1_state_dict",
+                           mapping2="model_F_mapping2_state_dict", alpha="model_F_alpha_state_dict")
 
     def __init__(self, video: Optional[DeviceVideo], mask: Optional[torch.Tensor], config: Optional[dict] = None,
                  precision: int = N.PREC_FP32, device="cuda", lr: float = 1e-4, resx: Optional[int] = None,

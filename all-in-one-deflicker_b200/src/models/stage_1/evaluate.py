@@ -80,11 +80,7 @@ def evaluate_model_single(trainer, resx, resy, number_of_frames, video_frames, r
     os.makedirs(os.path.join(results_folder, '%06d' % iteration), exist_ok=True)
     os.makedirs(output_folder, exist_ok=True)
     if save_checkpoint:      # evaluate.py:616-622 — same file name and keys
-        torch.save({'F_atlas_state_dict': {k: v.cpu() for k, v in trainer.state_dict("atlas").items()},
-                    'iteration': iteration,
-                    'model_F_mapping1_state_dict': {k: v.cpu() for k, v in trainer.state_dict("mapping").items()},
-                    'optimizer_all_state_dict': trainer.optimizer_state_dict()},
-                   '%s/checkpoint' % results_folder)
+        torch.save(trainer.checkpoint(iteration), '%s/checkpoint' % results_folder)
     psnrs = np.zeros((number_of_frames, 1))
     art = ArtefactWriter(os.path.join(results_folder, '%06d' % iteration), vid_name or "video", resx, resy) if artefacts else None
     ends = {}
@@ -121,10 +117,7 @@ def evaluate_model(trainer, resx, resy, number_of_frames, video_frames, results_
     os.makedirs(os.path.join(folder, "alpha"), exist_ok=True)
     os.makedirs(output_folder, exist_ok=True)
     if save_checkpoint:
-        cpu = lambda which: {k: v.cpu() for k, v in trainer.state_dict(which).items()}
-        ck = {'F_atlas_state_dict': cpu("atlas"), 'iteration': iteration, 'model_F_mapping1_state_dict': cpu("mapping1"),
-              'model_F_mapping2_state_dict': cpu("mapping2"), 'model_F_alpha_state_dict': cpu("alpha"),
-              'optimizer_all_state_dict': trainer.optimizer_state_dict()}
+        ck = trainer.checkpoint(iteration)
         torch.save(ck, '%s/checkpoint' % results_folder)
         torch.save(ck, '%s/checkpoint' % folder)
     psnrs = np.zeros((number_of_frames, 1))
@@ -216,13 +209,9 @@ def evaluate_model_single_sharded(trainer, resx, resy, number_of_frames, results
     os.makedirs(os.path.join(results_folder, '%06d' % iteration), exist_ok=True)
     os.makedirs(os.path.join(results_folder, "output"), exist_ok=True)
     if save_checkpoint:
-        opt = trainer.optimizer_state_dict()
+        ck = trainer.checkpoint(iteration)        # collective: every rank gathers the Adam moments
         if rank == 0:
-            torch.save({'F_atlas_state_dict': {k: v.cpu() for k, v in trainer.state_dict("atlas").items()},
-                        'iteration': iteration,
-                        'model_F_mapping1_state_dict': {k: v.cpu() for k, v in trainer.state_dict("mapping").items()},
-                        'optimizer_all_state_dict': opt},
-                       '%s/checkpoint' % results_folder)
+            torch.save(ck, '%s/checkpoint' % results_folder)
     psnrs, payloads = evaluate_block_single(trainer, resx, resy, number_of_frames, results_folder, artefacts,
                                             write_frames)
     merged = launch.gather_frame_values(psnrs, pg)
@@ -266,12 +255,8 @@ def evaluate_model_sharded(trainer, resx, resy, number_of_frames, results_folder
     os.makedirs(os.path.join(folder, "alpha"), exist_ok=True)
     os.makedirs(os.path.join(results_folder, "output"), exist_ok=True)
     if save_checkpoint:
-        opt = trainer.optimizer_state_dict()
+        ck = trainer.checkpoint(iteration)        # collective: every rank gathers the Adam moments
         if rank == 0:
-            cpu = lambda which: {k: v.cpu() for k, v in trainer.state_dict(which).items()}
-            ck = {'F_atlas_state_dict': cpu("atlas"), 'iteration': iteration, 'model_F_mapping1_state_dict': cpu("mapping1"),
-                  'model_F_mapping2_state_dict': cpu("mapping2"), 'model_F_alpha_state_dict': cpu("alpha"),
-                  'optimizer_all_state_dict': opt}
             torch.save(ck, '%s/checkpoint' % results_folder)
             torch.save(ck, '%s/checkpoint' % folder)
     merged = launch.gather_frame_values(evaluate_block_seg(trainer, resx, resy, number_of_frames, results_folder, iteration,

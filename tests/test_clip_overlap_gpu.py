@@ -296,7 +296,8 @@ def test_atlas_script_with_overlap(atlas_run, tmp_path):
 def test_atlas_stitch_under_torchrun_and_emulated_ranks(atlas_run, tmp_path, monkeypatch):
     """The stitch under torch.distributed.run (two ranks when the node has two GPUs), and ranks 0 and 1 of 2 in this
     process, from the one-process run's checkpoints: the same shared frames."""
-    from src import stage1_neural_atlas as S
+    from src.models.stage_1 import driver as D
+    from src.stage1_neural_atlas import VARIANT
     work, cfg, path, _ = atlas_run
     one = work / "results" / VID / "stage_1"
     nproc = min(2, torch.cuda.device_count())
@@ -319,7 +320,7 @@ def test_atlas_stitch_under_torchrun_and_emulated_ranks(atlas_run, tmp_path, mon
         os.remove(str(emu / "results" / VID / "stage_1" / "output" / ("%05d.png" % t)))
     monkeypatch.chdir(emu)
     args = types.SimpleNamespace(vid_path=str(emu / "data" / "test" / VID), down=1)
-    assert [S.stitch(cfg, args, PLAN, DEV, r, 2) for r in range(2)] == [2, 2]
+    assert [D.stitch(VARIANT, cfg, args, PLAN, DEV, r, 2) for r in range(2)] == [2, 2]
     assert sorted(os.listdir(str(emu / "results" / VID / "stage_1" / "output"))) == \
         ["%05d.png" % t for a, b in SEAMS for t in range(a, b)]
     for a, b in SEAMS:

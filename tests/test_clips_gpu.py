@@ -306,7 +306,8 @@ def _args(vid_path, no_artefacts=False):
 def test_rank_clip_lists_in_one_process_equal_one_rank(clip_runs, tmp_path, monkeypatch):
     """Ranks 0..N-1 of N = 2 and 3 fit their clips one after the other on this GPU; together they write what the
     one-process run wrote."""
-    from src import stage1_neural_atlas as S
+    from src.models.stage_1 import driver as D
+    from src.stage1_neural_atlas import VARIANT
     work, cfg, _, _ = clip_runs
     one = work / "results" / VID / "stage_1"
     for world in (2, 3):
@@ -315,14 +316,15 @@ def test_rank_clip_lists_in_one_process_equal_one_rank(clip_runs, tmp_path, monk
         _write_video(data)
         monkeypatch.chdir(w)
         for rank in range(world):
-            S.fit_clips(cfg, _args(data), A.rank_clips(CLIPS, rank, world), DEV, SEED)
+            D.fit_clips(VARIANT, cfg, _args(data), A.rank_clips(CLIPS, rank, world), DEV, SEED)
         _check_clip_runs(w / "results" / VID / "stage_1", [one / A.clip_name(c) for c in CLIPS], data, cfg, w)
 
 
 def test_clip_run_peak_memory_is_the_largest_clips(clip_runs, tmp_path, monkeypatch):
     """max_memory_allocated of the three-clip run against a stand-alone fit of its largest clip (5 frames), in this
     process; the library's cached tensor-core job tables of every clip are released with its trainer."""
-    from src import stage1_neural_atlas as S
+    from src.models.stage_1 import driver as D
+    from src.stage1_neural_atlas import VARIANT
     work, cfg, _, _ = clip_runs
     w = tmp_path / "mem"
     _write_video(w / "data" / "test" / VID)
@@ -333,13 +335,13 @@ def test_clip_run_peak_memory_is_the_largest_clips(clip_runs, tmp_path, monkeypa
     tables = N.lib().b200_tc_cached_tables()
     torch.cuda.reset_peak_memory_stats(DEV)
     torch.manual_seed(SEED)
-    S.main(cfg, _args(tmp_path / "mem_one" / "data" / "test" / VID, True), None, DEV)
+    D.fit(VARIANT, cfg, _args(tmp_path / "mem_one" / "data" / "test" / VID, True), DEV)
     largest = torch.cuda.max_memory_allocated(DEV)
     assert N.lib().b200_tc_cached_tables() == tables
     monkeypatch.chdir(w)
     torch.cuda.empty_cache()
     torch.cuda.reset_peak_memory_stats(DEV)
-    S.fit_clips(cfg, _args(w / "data" / "test" / VID, True), CLIPS, DEV, SEED)
+    D.fit_clips(VARIANT, cfg, _args(w / "data" / "test" / VID, True), CLIPS, DEV, SEED)
     three = torch.cuda.max_memory_allocated(DEV)
     print(f"peak device memory: three clips {three} B, largest clip alone {largest} B")
     assert three <= 1.03 * largest, (three, largest)
