@@ -374,7 +374,7 @@ int b200_seg_loss_grad(const B200SegConfig* cfg, const B200Video* video, const f
   const int larger = video->W > video->H ? video->W : video->H;
   SampleGeom geo;
   geo.half_larger = half_of_i(larger);
-  geo.half_resx = half_of_i(cfg->resx);
+  geo.half_resx = half_of_i(cfg->resx > 0 ? cfg->resx : video->W);
   geo.half_frames = (float)((double)video->T / 2.0);
   geo.d_local = cfg->derivative_amount;
   geo.d_global = cfg->global_derivative_amount;

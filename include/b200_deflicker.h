@@ -148,7 +148,8 @@ typedef struct B200AtlasConfig {
   int32_t batch;             /* samples_batch (global)                                        */
   int32_t with_global;       /* include_global_rigidity_loss && i <= stop_global_rigidity     */
   int32_t precision;         /* B200_PREC_*                                                   */
-  int32_t resx;              /* width  — the gradient loss normalises by resx (loss_utils.py:138) */
+  int32_t resx;              /* width  — the gradient loss normalises by resx (loss_utils.py:138);
+                                <= 0 means the video's width W (the rest normalises by max(W, H)) */
   float uv_mapping_scale;
   float derivative_amount;
   float global_derivative_amount;
@@ -430,7 +431,8 @@ typedef struct B200SegConfig {
   int32_t batch;             /* samples_batch                                                  */
   int32_t with_global;       /* include_global_rigidity_loss && i <= stop_global_rigidity      */
   int32_t precision;         /* B200_PREC_*                                                    */
-  int32_t resx;              /* width (gradient-loss normalisation)                            */
+  int32_t resx;              /* width (gradient-loss normalisation); <= 0 means the video's
+                                width W, as for B200AtlasConfig::resx                           */
   float uv_mapping_scale;
   float derivative_amount;
   float global_derivative_amount;   /* global_rigidity_derivative_amount_fg == _bg (both 100 in the

@@ -265,11 +265,12 @@ def flow_loss_all(video: Video, jif, uv, resx, T: int, mapping, uv_scale: float)
     return err * resx / (2 * uv_scale)
 
 
-def eval_maps(video: Video, map_params, f: int, d: int = 1, uv_scale: float = 0.8):
+def eval_maps(video: Video, map_params, f: int, d: int = 1, uv_scale: float = 0.8, larger=None):
     """Per-pixel maps of frame ``f`` as the reference's evaluation computes them (evaluate.py:640-700): uv (H, W, 2),
-    rigidity loss (H, W), forward flow error (H, W; zero for the last frame)."""
+    rigidity loss (H, W), forward flow error (H, W; zero for the last frame).  ``larger`` overrides max(W, H) (the
+    tests' negative controls only)."""
     H, W, T = video.H, video.W, video.T
-    larger = np.maximum(np.int64(W), np.int64(H))
+    larger = np.maximum(np.int64(W), np.int64(H)) if larger is None else np.int64(larger)
     ys, xs = torch.where(torch.ones(H, W) > 0)
     mapping = lambda x: mlp_forward(MAPPING_SPEC, map_params, x)
     with torch.no_grad():
@@ -293,11 +294,14 @@ DEFAULT_CONFIG = dict(rgb_coeff=5000, optical_flow_coeff=500.0, gradient_loss_co
 
 
 def iteration_losses(video: Video, map_params, atlas_params, inds: torch.Tensor, it: int,
-                     cfg: dict = DEFAULT_CONFIG, device: str = "cpu") -> Dict[str, torch.Tensor]:
+                     cfg: dict = DEFAULT_CONFIG, device: str = "cpu", resx: Optional[int] = None,
+                     larger_dim: Optional[int] = None) -> Dict[str, torch.Tensor]:
     """Loss terms of one loop trip for sample indices ``inds`` ((B,1) int64 into the pixel
-    table).  Returns the individual terms and the weighted ``total`` (with grad)."""
+    table).  Returns the individual terms and the weighted ``total`` (with grad).  ``resx`` and
+    ``larger_dim`` override W and max(W, H) (the tests' negative controls only)."""
     H, W, T = video.H, video.W, video.T
-    larger_dim = int(np.maximum(W, H))
+    resx = W if resx is None else resx
+    larger_dim = int(np.maximum(W, H)) if larger_dim is None else larger_dim
     table = pixel_table(T, H, W)
     jif = table[:, inds]                                            # (3, B, 1)  :162
     rgb = video.frames[jif[1], jif[0], :, jif[2]].squeeze(1).to(device)     # :164
@@ -306,7 +310,7 @@ def iteration_losses(video: Video, map_params, atlas_params, inds: torch.Tensor,
     atlas = lambda x: mlp_forward(ATLAS_SPEC, atlas_params, x)
     uv = mapping(xyt)                                              # :174
     rgb_out = (atlas(uv * 0.5 + 0.5) + 1.0) * 0.5                  # :181
-    g = gradient_loss(video_to(video, "cpu"), jif, mapping, atlas, rgb_out, W)   # :186 (resx)
+    g = gradient_loss(video_to(video, "cpu"), jif, mapping, atlas, rgb_out, resx)   # :186
     rgb_l = (torch.norm(rgb_out - rgb, dim=1) ** 2).mean()         # :194
     rig = rigidity_loss(jif, cfg["derivative_amount"], larger_dim, T, mapping, uv,
                         uv_scale=cfg["uv_mapping_scale"])          # :196
@@ -360,10 +364,11 @@ def train_iteration(video, map_params, atlas_params, opt, inds, it, cfg=DEFAULT_
 # render + PSNR  (src/models/stage_1/evaluate.py:640-708, 733, 740-743)
 # ----------------------------------------------------------------------------------------
 def render_frame(map_params, atlas_params, f: int, H: int, W: int, T: int,
-                 chunk: int = 100000, device: str = "cpu") -> torch.Tensor:
+                 chunk: int = 100000, device: str = "cpu", larger=None) -> torch.Tensor:
     """RGB reconstruction of frame ``f`` as (H, W, 3) fp32; evaluate.py:644-666 (pixels of the
-    frame in row-major order, split with np.array_split into <=100k chunks)."""
-    larger_dim = np.maximum(np.int64(W), np.int64(H))
+    frame in row-major order, split with np.array_split into <=100k chunks).  ``larger`` overrides
+    max(W, H) (the tests' negative controls only)."""
+    larger_dim = np.maximum(np.int64(W), np.int64(H)) if larger is None else np.int64(larger)
     ys, xs = torch.where(torch.ones(H, W) > 0)
     parts = int(np.ceil(ys.shape[0] / chunk))
     out = torch.zeros(H, W, 3)

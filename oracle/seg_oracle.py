@@ -89,12 +89,15 @@ def flow_alpha_loss(video: O.Video, jif, alpha, resx, alpha_net):
 
 def seg_iteration_losses(video: O.Video, mask_frames: torch.Tensor, nets: Dict[str, Sequence[torch.Tensor]],
                          inds: torch.Tensor, it: int, cfg: dict = SEG_CONFIG,
-                         specs: Dict[str, MlpSpec] = None) -> Dict[str, torch.Tensor]:
+                         specs: Dict[str, MlpSpec] = None, resx: int = None,
+                         larger_dim: int = None) -> Dict[str, torch.Tensor]:
     """Loss terms of one trip of stage1_neural_atlas_seg.py:195-311.  ``nets`` holds the parameter lists
-    'mapping1', 'mapping2', 'alpha', 'atlas'; ``mask_frames`` is the (H, W, T) bootstrapping mask."""
+    'mapping1', 'mapping2', 'alpha', 'atlas'; ``mask_frames`` is the (H, W, T) bootstrapping mask.  ``resx`` and
+    ``larger_dim`` override W and max(W, H) (the tests' negative controls only)."""
     specs = specs or dict(mapping1=MAPPING1_SPEC, mapping2=MAPPING2_SPEC, alpha=ALPHA_SPEC, atlas=ATLAS_SPEC)
     H, W, T = video.H, video.W, video.T
-    larger_dim = int(np.maximum(W, H))
+    resx = W if resx is None else resx
+    larger_dim = int(np.maximum(W, H)) if larger_dim is None else larger_dim
     jif = O.pixel_table(T, H, W)[:, inds]                                    # :209
     rgb = video.frames[jif[1], jif[0], :, jif[2]].squeeze(1)                 # :211
     a_gt = mask_frames[jif[1], jif[0], jif[2]].squeeze(1).unsqueeze(-1)      # :215
@@ -106,7 +109,7 @@ def seg_iteration_losses(video: O.Video, mask_frames: torch.Tensor, nets: Dict[s
     rgb1 = (atlas(uv1 * 0.5 + 0.5) + 1.0) * 0.5                              # :236
     rgb2 = (atlas(uv2 * 0.5 - 0.5) + 1.0) * 0.5
     rgb_out = rgb1 * alpha + rgb2 * (1.0 - alpha)                            # :240
-    g = gradient_loss_seg(video, jif, mapping1, mapping2, atlas, alpha_net, rgb_out, W)   # :243
+    g = gradient_loss_seg(video, jif, mapping1, mapping2, atlas, alpha_net, rgb_out, resx)   # :243
     rgb_not = rgb1 * (1.0 - alpha)                                           # :249
     rgb_l = (torch.norm(rgb_out - rgb, dim=1) ** 2).mean()
     sparsity = (torch.norm(rgb_not, dim=1) ** 2).mean()
@@ -144,11 +147,11 @@ def make_optimizer(nets, lr: float = 1e-4):
     return torch.optim.Adam([{"params": list(nets[k])} for k in ("mapping1", "mapping2", "alpha", "atlas")], lr=lr)
 
 
-def render_frame_seg(nets, f: int, H: int, W: int, T: int, specs=None):
+def render_frame_seg(nets, f: int, H: int, W: int, T: int, specs=None, larger=None):
     """Reconstruction and alpha of frame ``f`` (evaluate.py `evaluate_model` :262-330 restricted to the RGB
-    composite and alpha): (H, W, 3), (H, W)."""
+    composite and alpha): (H, W, 3), (H, W).  ``larger`` overrides max(W, H) (the tests' negative controls only)."""
     specs = specs or dict(mapping1=MAPPING1_SPEC, mapping2=MAPPING2_SPEC, alpha=ALPHA_SPEC, atlas=ATLAS_SPEC)
-    larger_dim = np.maximum(np.int64(W), np.int64(H))
+    larger_dim = np.maximum(np.int64(W), np.int64(H)) if larger is None else np.int64(larger)
     ys, xs = torch.where(torch.ones(H, W) > 0)
     with torch.no_grad():
         xyt = torch.cat((xs.unsqueeze(1) / (larger_dim / 2) - 1, ys.unsqueeze(1) / (larger_dim / 2) - 1,
