@@ -453,9 +453,11 @@ int launch_loss(const float* uv, const float* y_atlas, const float* targets, int
 
 // ---------------------------------------------------------------------------------------------
 // Adam (torch.optim.Adam defaults: no weight decay, no amsgrad), src/stage1_neural_atlas.py:132-134.
-// Arithmetic order of torch's single-tensor implementation (_single_tensor_adam):
-//   m.lerp_(g, 1-b1);  v.mul_(b2).addcmul_(g, g, value=1-b2);
-//   denom = sqrt(v) / sqrt(1-b2^t) + eps;  p.addcdiv_(m, denom, value=-lr/(1-b1^t))
+// Arithmetic order (torch's single-tensor implementation, _single_tensor_adam, step by step):
+//   m.lerp_(g, 1-b1);  v.mul_(b2).addcmul_(g, g, value=1-b2);  denom = sqrt(v) / sqrt(1-b2^t) + eps;
+//   p = p + (-step_size * m) / denom   with step_size = fp32(lr/(1-b1^t)).
+// The last line is p.addcdiv_(m, denom, value=-step_size) in the operand order of torch's CPU addcdiv
+// (self + value * t1 / t2); torch's CUDA addcdiv rounds in another order and may differ in the last bit.
 // ---------------------------------------------------------------------------------------------
 __device__ unsigned int g_adam_ticket = 0u;
 
