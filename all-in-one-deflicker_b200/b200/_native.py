@@ -82,6 +82,14 @@ class WarpPair(C.Structure):
 WARP_MAX_PAIRS = 32
 
 
+class FidelityFrame(C.Structure):
+    _fields_ = [("frame", C.c_void_p), ("ref", C.c_void_p), ("H", C.c_int32), ("W", C.c_int32), ("Hr", C.c_int32),
+                ("Wr", C.c_int32), ("bits", C.c_int32), ("ref_bits", C.c_int32)]
+
+
+FIDELITY_MAX_FRAMES = 32
+
+
 class PngPlan(C.Structure):
     _fields_ = [("magic", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("n_blocks", C.c_int32),
                 ("n_chunks", C.c_int32), ("prefix_bytes", C.c_int32), ("suffix_bytes", C.c_int32),
@@ -167,6 +175,8 @@ SIGNATURES = {
     "b200_frame_sse": (C.c_int, [C.POINTER(Video), _I32, _P, _P, _P, _I64, _P]),
     "b200_warp_error_workspace_bytes": (_I64, [C.POINTER(WarpPair), _I32]),
     "b200_warp_error": (C.c_int, [C.POINTER(WarpPair), _I32, _P, _P, _P, _P, _I64, _P]),
+    "b200_fidelity_workspace_bytes": (_I64, [C.POINTER(FidelityFrame), _I32]),
+    "b200_fidelity": (C.c_int, [C.POINTER(FidelityFrame), _I32, _P, _P, _P, _I64, _P]),
     "b200_blend_frames": (C.c_int, [_P, _P, _I64, C.c_double, _P, _P, _P]),
     "b200_render_workspace_bytes": (_I64, [_I64]),
     "b200_render": (C.c_int, [_P, _I32, _I32, _I32, _I32, _I64, _I64, _P, _P, C.c_int, _P, _I64, _P]),

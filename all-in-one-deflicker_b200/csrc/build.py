@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 PKG = os.path.dirname(HERE)
 LIB = os.path.join(PKG, "b200", "libb200deflicker.so")
 HOSTLIB = os.path.join(PKG, "b200", "libb200_hostcheck.so")
-CU = ["c_api.cu", "mlp_simt.cu", "atlas_kernels.cu", "mlp_tc.cu", "loss_heads.cu", "seg.cu", "eval_maps.cu", "eval_sse.cu", "producer.cu", "conv_simt.cu", "conv_tma.cu", "raft_kernels.cu", "corr_alt.cu", "stage2_io.cu", "png_encode.cu", "warp_error.cu", "blend.cu"]
+CU = ["c_api.cu", "mlp_simt.cu", "atlas_kernels.cu", "mlp_tc.cu", "loss_heads.cu", "seg.cu", "eval_maps.cu", "eval_sse.cu", "producer.cu", "conv_simt.cu", "conv_tma.cu", "raft_kernels.cu", "corr_alt.cu", "stage2_io.cu", "png_encode.cu", "warp_error.cu", "blend.cu", "fidelity.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 

@@ -23,6 +23,11 @@ parser.add_argument('--clip_overlap', type=int, default=0,
                          "atlases' renders")
 parser.add_argument('--evaluate_flicker', action='store_true',
                     help="after stage 2, score the warping error of the input and of every output (results/<name>/flicker.json)")
+parser.add_argument('--fidelity', action='store_true',
+                    help="with --evaluate_flicker: also score SSIM and PSNR of every output against the input or "
+                         "--reference (results/<name>/fidelity.json)")
+parser.add_argument('--reference', type=str, default=None,
+                    help="with --fidelity: the folder of reference frames, for example a video's clean frames")
 parser.add_argument('--ckpt_filter', type=str, default="./pretrained_weights/neural_filter.pth")
 parser.add_argument('--ckpt_local', type=str, default="./pretrained_weights/local_refinement_net.pth")
 
@@ -54,6 +59,10 @@ if __name__ == "__main__":
         parser.error("--clip_overlap is only meaningful with --clips")
     if args.clip_overlap < 0:
         parser.error("--clip_overlap must be >= 0")
+    if args.fidelity and not args.evaluate_flicker:
+        parser.error("--fidelity is only meaningful with --evaluate_flicker")
+    if args.reference is not None and not args.fidelity:
+        parser.error("--reference is only meaningful with --fidelity")
     # The reference (test.py:17-31) always works on ./data/test/<name>: a video is split into that folder, a frame
     # folder is moved there.  Stage 1 (--root data/test/) and stage 2 (hard-coded ./data/test/<name>) both read it.
     if args.video_name is not None:
@@ -100,4 +109,9 @@ if __name__ == "__main__":
         flicker += ["--clips"]
     if args.clip_overlap > 0:
         flicker += ["--clip_overlap", str(args.clip_overlap)]
+    if args.fidelity:
+        flicker += ["--fidelity"]
+    if args.reference is not None:
+        # the script runs from this directory too, so a relative folder means the same
+        flicker += ["--reference", args.reference]
     sys.exit(subprocess.call(flicker))

@@ -564,6 +564,37 @@ int b200_warp_error(const B200WarpPair* pairs_host, int32_t n, double* sums, flo
                     void* ws, int64_t ws_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Fidelity of frames to a reference (no reference counterpart; the partner of the warping error,
+ * DESIGN §4f).  For a frame O ((H, W, 3) uint8 or uint16 HWC, decoded as v / 255 or v / 65535 in
+ * fp32) and a reference R ((Hr, Wr, 3), its own bit depth; resized to (H, W) with cv2.resize
+ * INTER_LINEAR arithmetic in fp32 when the sizes differ): per channel c and interior pixel p
+ * (5 <= x < W - 5, 5 <= y < H - 5), with G the separable Gaussian window (sigma 1.5, radius 5),
+ * mu_O = G*O, mu_R = G*R, var_O = G*O^2 - mu_O^2, var_R likewise, cov = G*(O R) - mu_O mu_R,
+ * SSIM = (2 mu_O mu_R + C1)(2 cov + C2) / ((mu_O^2 + mu_R^2 + C1)(var_O + var_R + C2)),
+ * C1 = 0.01^2, C2 = 0.03^2.  H and W must be at least 11.
+ * ------------------------------------------------------------------------------------------ */
+#define B200_FIDELITY_MAX_FRAMES 32
+typedef struct {
+  const void* frame;      /* O (H, W, 3), uint8 when bits == 8, uint16 when bits == 16 */
+  const void* ref;        /* R (Hr, Wr, 3), uint8 when ref_bits == 8, uint16 when ref_bits == 16 */
+  int32_t H, W;           /* O's size: the resolution the frame is scored at */
+  int32_t Hr, Wr;         /* R's size */
+  int32_t bits;           /* O's: 8 or 16 */
+  int32_t ref_bits;       /* R's: 8 or 16 */
+} B200FidelityFrame;
+/* bytes of workspace a call on these frames needs; -1 (message) for an invalid table */
+int64_t b200_fidelity_workspace_bytes(const B200FidelityFrame* frames_host, int32_t n);
+/* Scores n (1..B200_FIDELITY_MAX_FRAMES) frame pairs in one launch sequence.  sums [n][2] float64:
+ * the SSIM sum over the (H - 10)(W - 10) interior pixels and 3 channels, and the squared-error sum
+ * over all H W 3 values.  ssim_map (fp32), NULL or H * W * 3 values per pair, pair after pair: the
+ * SSIM of each interior pixel and channel rounded to fp32 once, NaN outside the interior.  The
+ * arithmetic is float64 with one IEEE rounding per operation, and the sums' order depends on H and
+ * W only (no atomics): bit-identical across calls, graph replays, batch compositions and devices.
+ * Allocates nothing, does not synchronise, graph-capturable. */
+int b200_fidelity(const B200FidelityFrame* frames_host, int32_t n, double* sums, float* ssim_map, void* ws,
+                  int64_t ws_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Cross-fade of two renders of one frame (no reference counterpart; the seams of overlapping clips,
  * DESIGN §5).  For each of the n values: o = (float)((1 - w) (double)a + w (double)b), in float64
  * with one IEEE rounding per operation and no fma, rounded to fp32 once, so w = 0 gives a and

@@ -1,11 +1,12 @@
 """The seam between clip atlases, without and with a cross-fade over overlapping frames (`--clips --clip_overlap V`).
 
-    python tools/clip_seams.py [--frames 120] [--max_frames 50] [--overlaps 0 8] [--height 270] [--width 480] [--out DIR]
+    python tools/clip_seams.py [--frames 120] [--max_frames 50] [--overlaps 0 8] [--height 270] [--width 480] [--out DIR] [--fidelity]
 
 Writes a seeded flickering synthetic video (b200.synth.quality_set: a translating texture with a per-frame gain and
 offset) with its exact flows, fits it with `src/stage1_neural_atlas.py --clips` at each overlap V with the shipped
 config's iteration count (maximum_number_of_frames set to --max_frames), and scores the stage-1 output with
-`src/evaluate_flicker.py --clips --clip_overlap V`.  Prints one JSON line per V: the plan, E_boundary and E_interior of
+`src/evaluate_flicker.py --clips --clip_overlap V` (with --fidelity, also the atlas output's SSIM and PSNR against the
+input, seam and interior frames apart).  Prints one JSON line per V: the plan, E_boundary and E_interior of
 the input and of the atlas output, the seam pairs' E(t), the wall time of the whole stage-1 run and of the stitch; and
 one line with the card's name and power limit, read in the same run.  Work files go to a temporary directory (or
 --out)."""
@@ -63,6 +64,8 @@ def main():
     ap.add_argument("--height", type=int, default=270)
     ap.add_argument("--width", type=int, default=480)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--fidelity", action="store_true",
+                    help="also score the atlas output's SSIM and PSNR against the input, seam and interior frames apart")
     args = ap.parse_args()
     import torch
     if torch.cuda.device_count() == 0:
@@ -88,7 +91,11 @@ def main():
         stage1_s = time.perf_counter() - t0
         m = re.search(r"stitch: rank 0 wrote (\d+) frames of \d+ seams in ([0-9.]+) s", out)
         run([sys.executable, os.path.join(pkg, "src", "evaluate_flicker.py"), "--video_name", "seams", "--sequences",
-             "input,atlas", "--clips"] + extra, work, env)
+             "input,atlas", "--clips"] + extra + (["--fidelity"] if args.fidelity else []), work, env)
+        fid = {}
+        if args.fidelity:
+            f = json.load(open(os.path.join(work, "results", "seams", "fidelity.json")))["sequences"]["atlas"]
+            fid = {k: f[k] for k in ("SSIM", "PSNR", "SSIM_seam", "SSIM_interior", "PSNR_seam", "PSNR_interior")}
         doc = json.load(open(os.path.join(work, "results", "seams", "flicker.json")))
         seqs = doc["sequences"]
         pairs = doc["clips"]["boundary_pairs"]
@@ -100,7 +107,8 @@ def main():
             "E_interior": {s: seqs[s]["E_interior"] for s in seqs},
             "atlas_seam_pairs": {t: seqs["atlas"]["per_pair"][t]["E"] for t in pairs},
             "stage1_s": round(stage1_s, 1),
-            "stitched_frames": int(m.group(1)) if m else 0, "stitch_s": float(m.group(2)) if m else None}), flush=True)
+            "stitched_frames": int(m.group(1)) if m else 0, "stitch_s": float(m.group(2)) if m else None,
+            **({"atlas_fidelity": fid} if fid else {})}), flush=True)
     if args.out is None:
         shutil.rmtree(work, ignore_errors=True)
 
